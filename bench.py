@@ -35,7 +35,8 @@ UNIT = "updates/s"
 
 
 def peaks():
-    p = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16; a power-limited card sustains less
+    p = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             m = json.load(f)
@@ -312,7 +313,7 @@ def time_config(model, dev, world, *, Bc, Hc, Wc, n_global, stride, steps=5, war
 
 
 def corr_nonresident_block(dev, feat, pk):
-    """corr_gather where the HBM roofline means something: a pyramid that does NOT fit the 126 MB L2 (BASELINE cfg 5's
+    """corr_gather where the HBM roofline means something: a pyramid that does NOT fit the 50 MB L2 (BASELINE cfg 5's
     clip: 100 frames of 90x160 maps at stride 4, 0.98 GB in fp32), 4096 tracks reading their own 8-frame windows
     (chained-tracking addressing), L2 flushed before every launch.  Both byte counts are given: SURVEY 8d's 66 440 B per
     unit (bf16 pyramid + bf16 row) and what this configuration actually moves (fp32 pyramid, (hi, lo) row)."""
@@ -384,6 +385,20 @@ def chain_block(dev, precision, feat):
     return out
 
 
+def dump_outputs(path: str, out) -> None:
+    """What Pips.forward returned in the last timed step, one float32 .npy per array (a few MB at the bench sizes): the
+    trajectory estimate after every refinement iteration (input pixels), the second-resolution estimates, and the
+    visibility logits.  The inputs are seeded, so two builds can be compared array for array."""
+    import numpy as np
+    preds, preds2, vis_e = out[0], out[1], out[2]
+    os.makedirs(path, exist_ok=True)
+    arrays = {"vis_e": vis_e}
+    arrays.update({f"trajs_e_iter{i}": p for i, p in enumerate(preds)})
+    arrays.update({f"trajs_e2_iter{i}": p for i, p in enumerate(preds2)})
+    for name, t in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 def run_ours(args, rank, world, local_rank):
     import torch.distributed as dist
     from pips_b200 import synthetic
@@ -397,7 +412,7 @@ def run_ours(args, rank, world, local_rank):
         model.shard_particles()
     rgbs_h, xys_h = rgbs_h.pin_memory(), xys_h.pin_memory()
     rgbs, xys = rgbs_h.to(dev), xys_h.to(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)             # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)             # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -414,16 +429,17 @@ def run_ours(args, rank, world, local_rank):
             return out[0][-1].cpu(), out[2].cpu()
 
     def timed(step, k):
-        """k steps, L2 flushed before each; returns (total seconds, [ms per step]) from CUDA events on this stream."""
-        evs = []
+        """k steps, L2 flushed before each; returns (total seconds, [ms per step], what the last step returned); times
+        from CUDA events on this stream."""
+        evs, out = [], None
         for _ in range(k):
             flush.zero_()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(); step(); e1.record()
+            e0.record(); out = step(); e1.record()
             evs.append((e0, e1))
         torch.cuda.synchronize()
         per = [a.elapsed_time(b) for a, b in evs]
-        return sum(per) / 1e3, per
+        return sum(per) / 1e3, per, out
 
     # sharded runs: the particle shares become speed-weighted after the 5th forward (pips_b200/sharding.py::_Balance) and the
     # next forward re-captures its CUDA graph at the new share -- all of that belongs to the warm-up
@@ -437,8 +453,11 @@ def run_ours(args, rank, world, local_rank):
         step_device()
     barrier()
     sampler.mark()
-    t_dev, per_dev = timed(step_device, args.steps)
+    t_dev, per_dev, last = timed(step_device, args.steps)
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
+    del last
     clocks = sampler.stop()
     if world > 1:
         all_clocks = [None] * world
@@ -450,7 +469,7 @@ def run_ours(args, rank, world, local_rank):
     launches = (model.engine.launches + (encoder_fast.LAUNCHES[0] if model.fnet_mode == 'tc' else 0)) * args.steps
     step_host()
     barrier()
-    t_e2e, per_e2e = timed(step_host, args.steps)
+    t_e2e, per_e2e, _ = timed(step_host, args.steps)
     barrier()
     if world > 1:
         t = torch.tensor([t_dev, t_e2e], device=dev, dtype=torch.float64)
@@ -475,7 +494,7 @@ def run_ours(args, rank, world, local_rank):
 
         if world == 1:
             if N_PER_GPU != 4096:
-                # the north-star target configuration: S=8, 384x512, N=4096, iters=6 on ONE B200 (>= 1 M updates/s asked)
+                # the north-star target configuration: S=8, 384x512, N=4096, iters=6 on ONE GPU
                 guarded("n4096_1gpu", lambda: time_config(model, dev, 1, Bc=B, Hc=H, Wc=W, n_global=4096, stride=STRIDE, seed=1234))
             guarded("cfg1_demo_shape_1gpu", lambda: time_config(fresh(4), dev, 1, Bc=1, Hc=360, Wc=640, n_global=256, stride=4, steps=10))
             guarded("cfg4_1gpu", lambda: time_config(fresh(8), dev, 1, Bc=1, Hc=720, Wc=1280, n_global=16384, stride=8))
@@ -520,10 +539,10 @@ def run_ours(args, rank, world, local_rank):
     achieved_tf = gemm_flop / (gemm_ms * 1e-3) / 1e12
     tc = args.precision != "fp32"
     mma_per_product = 3 if args.precision == "bf16x3" else 1
-    roofline = {"kernel": "gemm_tc2_kernel (tcgen05 cta_group::2; FC1+FC2 of the 12 channel-mixing blocks)" if tc else "gemm_f32_kernel",
+    roofline = {"kernel": "gemm_tc_pair_kernel (wgmma, W multicast in clusters of 2; FC1+FC2 of the 12 channel-mixing blocks)" if tc else "gemm_f32_kernel",
                 "bound": "tensor", "achieved": achieved_tf, "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s",
                 "frac": achieved_tf / pk["bf16_tflops_sustained"], "traffic": None,
-                "peak_source": pk["source"] + " (sustained bf16 cuBLAS)", "share_of_iteration": gemm_ms / sum(per_iter.values()),
+                "peak_source": pk["source"] + " (dense bf16)", "share_of_iteration": gemm_ms / sum(per_iter.values()),
                 "mma_issued_frac": achieved_tf * mma_per_product / pk["bf16_tflops_sustained"] if tc else None}
     e_f = 4 if args.feat == "fp32" else 2
     e_o = {"fp32": 4, "bf16x3": 4, "bf16": 2}[args.precision]
@@ -535,20 +554,6 @@ def run_ours(args, rank, world, local_rank):
                      "peak_source": pk["source"] + " (copy bandwidth)",
                      "note": "the 67 MB pyramid is L2-resident at this configuration: algorithmic gather bytes over the kernel time exceed the "
                              "HBM copy peak and are NOT an HBM fraction -- roofline_corr_hbm measures the kernel on a pyramid larger than L2"}
-    # DRAM bytes per launch come from an `ncu --set full` capture (tools/ncu_traffic.py writes the file together with the
-    # digest of the kernel sources it profiled); they are reported only when that digest is the library's that runs now.
-    try:
-        from pips_b200 import _build
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            tr = json.load(f)
-        if tr.get("source_digest") == _build.source_digest():
-            roofline["traffic"] = tr.get("gemm_fc_bytes_per_launch")
-            roofline_corr["traffic"] = tr.get("corr_gather_bytes_per_launch")
-            roofline["traffic_source"] = roofline_corr["traffic_source"] = tr.get("source")
-        else:
-            roofline["traffic_source"] = roofline_corr["traffic_source"] = "profiles/ncu_traffic.json is from other kernel sources: not reported"
-    except Exception:
-        pass
     corr_hbm = None
     if world == 1 and not args.no_extra:
         try:
@@ -573,7 +578,7 @@ def run_ours(args, rank, world, local_rank):
             e1.record(); torch.cuda.synchronize()
         model.fnet_mode = mode
         eager = {"value": updates / (e0.elapsed_time(e1) / 3e3), "unit": UNIT, "ms_per_step": e0.elapsed_time(e1) / 3,
-                 "what": "reference algorithm as eager torch ops on the same B200 (fp32, TF32 off)"}
+                 "what": "reference algorithm as eager torch ops on the same GPU (fp32, TF32 off)"}
     cpu = cpu_baseline_leg() if world == 1 and not args.no_cpu_baseline else None
     h2d = rgbs_h.numel() * rgbs_h.element_size() + xys_h.numel() * 4
     d2h = (B * S * n_global * 2 + B * S * n_global) * 4
@@ -583,7 +588,7 @@ def run_ours(args, rank, world, local_rank):
             "data": "synthetic",
             "config": {"workload": workload_name(world),
                        "precision": args.precision, "feat_dtype": args.feat, "parallelism": (f"particle-sharded dp{world}, shares " + ("speed-weighted " + str(shard_sizes_now) if shard_sizes_now else "equal")) if world > 1 else "single GPU",
-                       "includes": "fnet (tcgen05 convs) + pyramid + 6 refinement iterations + vis head", "fnet_mode": model.fnet_mode, "l2": "256 MB write between steps (L2 flushed); working set > L2"},
+                       "includes": "fnet (wgmma convs) + pyramid + 6 refinement iterations + vis head", "fnet_mode": model.fnet_mode, "l2": "256 MB write between steps (L2 flushed); working set > L2"},
             "clocks": clocks, "gpu_launches": launches,
             "e2e": {"value": updates / (t_e2e / args.steps), "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "ms_per_step": t_e2e / args.steps * 1e3},
@@ -631,6 +636,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager", action="store_true", help="skip the eager-torch restatement of the reference on this GPU")
     ap.add_argument("--no-extra", action="store_true", help="skip the other BASELINE configurations (n4096_1gpu, cfg1/4/5, strong_cfg3, cfg4_sharded)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<name>.npy (float32; seeded inputs: comparable between builds)")
     ap.add_argument("--particles", type=int, default=0, help="particles per GPU (default 1024 = BASELINE cfg2; 4096 = cfg3 on one GPU)")
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))

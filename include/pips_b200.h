@@ -1,4 +1,4 @@
-/* pips_b200 -- C ABI of the B200-native PIPs refinement hot path.
+/* pips_b200 -- C ABI of the H100-native PIPs refinement hot path.
  *
  * The reference (aharley/pips) has no FFI / plugin registry: its boundary is the Python class
  * nets.pips.Pips (nets/pips.py:400-611).  This header is what a reference-side binding (ctypes,
@@ -36,8 +36,8 @@ enum { PIPS_KITCHEN = 519, PIPS_KITCHEN_PAD = 576, PIPS_DIM = 512, PIPS_HIDDEN =
 enum { PIPS_FEAT_F32 = 0, PIPS_FEAT_BF16 = 1 };
 /* arithmetic of the mixer's dense layers */
 enum { PIPS_PREC_F32 = 0,      /* fp32 CUDA-core GEMMs (exact; validation / small problems)            */
-       PIPS_PREC_BF16X3 = 1,   /* tcgen05, operands split hi+lo bf16, 3 MMAs per product (~fp32)       */
-       PIPS_PREC_BF16 = 2 };   /* tcgen05, plain bf16 operands (fast mode, does not meet 1e-3 px)      */
+       PIPS_PREC_BF16X3 = 1,   /* wgmma,   operands split hi+lo bf16, 3 MMAs per product (~fp32)       */
+       PIPS_PREC_BF16 = 2 };   /* wgmma,   plain bf16 operands (fast mode, does not meet 1e-3 px)      */
 /* GEMM epilogues */
 enum { PIPS_EPI_BIAS = 0,        /* out_f32 = acc + bias                                              */
        PIPS_EPI_BIAS_GELU = 1,   /* out    = gelu_erf(acc + bias)  (bf16 hi[/lo] or fp32)             */
@@ -89,7 +89,7 @@ int pips_tokenmix(float* x, int seqs, const float* ln1_w, const float* ln1_b,
                   const float* w1 /* (32,8) */, const float* b1, const float* w2 /* (8,32) */, const float* b2,
                   const float* ln2_w, const float* ln2_b, void* y_hi, void* y_lo, float* y_f32, void* stream);
 
-/* the same with the two contractions as tcgen05 MMAs (channels as the M dimension, bf16x3 folded into K); bf16
+/* the same with the two contractions as wgmma MMAs (channels as the M dimension, bf16x3 folded into K); bf16
  * outputs only.  Selected inside pips_tokenmix by PIPS_B200_TOKENMIX=tc; see csrc/tokenmix_tc.cu for its status. */
 int pips_tokenmix_tc(float* x, int seqs, const float* ln1_w, const float* ln1_b, const float* w1, const float* b1,
                      const float* w2, const float* b2, const float* ln2_w, const float* ln2_b, void* y_hi, void* y_lo,
@@ -172,7 +172,7 @@ int pips_inorm_apply_pair(const float* y, const float* stats_y, const float* r, 
 int pips_resize_pair(const float* src, int N, int Hs, int Ws, int C, void* dst_hi, void* dst_lo, int Ho, int Wo, int Ctot, int c_off,
                      void* stream);
 /* nn.Conv2d (3x3 / 1x1, stride 1 / 2; nets/pips.py:135-136,:170,:221-223) as an implicit GEMM on the tensor cores
- * (tcgen05, CTA pairs, bf16x3).  x_hi/x_lo (N,H,W,Cp) bf16 with Cp % 64 == 0; w_hi/w_lo (BN, R*S*Cp) bf16,
+ * (wgmma, bf16x3).  x_hi/x_lo (N,H,W,Cp) bf16 with Cp % 64 == 0; w_hi/w_lo (BN, R*S*Cp) bf16,
  * k = (r*S + s)*Cp + ci, BN = Cout rounded up to 64/128/256 with zero rows; out (N,Ho,Wo,Cout) fp32; bias may be NULL. */
 int pips_conv_tc(const void* x_hi, const void* x_lo, int N, int H, int W, int Cp, const void* w_hi, const void* w_lo,
                  int Cout, int R, int S, int stride, int pad, const float* bias, float* out, void* stream);

@@ -1,4 +1,4 @@
-"""pips_b200: B200-native (sm_100a) implementation of the PIPs inference hot path.
+"""pips_b200: H100-native (sm_90a) implementation of the PIPs inference hot path.
 
 ``from pips_b200 import Pips`` is a drop-in for ``from nets.pips import Pips`` of aharley/pips.
 """

@@ -1,4 +1,4 @@
-"""In-tree build of libpips_b200.so with nvcc for sm_100a (no torch headers, no libcuda link).
+"""In-tree build of libpips_b200.so with nvcc for sm_90a (no torch headers, no libcuda link).
 
 The shared object stays inside the package directory so that it travels with the repo snapshot to
 the GPU box; it is git-ignored.  ``build()`` is idempotent (mtime check) and cheap to call.
@@ -14,8 +14,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "lib", "obj")
 LIB = os.path.join(HERE, "lib", "libpips_b200.so")
-SOURCES = ["abi.cu", "pyramid.cu", "corr_gather.cu", "mixer_simt.cu", "tokenmix_tc.cu", "gemm_tc.cu", "gemm_tc2.cu", "conv_tc.cu", "conv_rows.cu", "encoder_ops.cu", "heatmap.cu", "peer.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+SOURCES = ["abi.cu", "pyramid.cu", "corr_gather.cu", "mixer_simt.cu", "tokenmix_tc.cu", "gemm_tc.cu", "conv_tc.cu", "conv_rows.cu", "encoder_ops.cu", "heatmap.cu", "peer.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
 
@@ -86,7 +86,7 @@ def build(verbose: bool = False, force: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(lambda s: _compile(s, log), SOURCES))
     if force or not os.path.exists(LIB) or any(os.path.getmtime(o) > os.path.getmtime(LIB) for o in objs):
-        cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+        cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -36,10 +36,10 @@ int current_device() {
 int sm_count() {
     static int n[kMaxDevices] = {};
     const int dev = current_device();
-    if (dev < 0 || dev >= kMaxDevices) return 148;
+    if (dev < 0 || dev >= kMaxDevices) return 132;
     if (n[dev] == 0) {
         int v = 0;
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         n[dev] = v;
     }
     return n[dev];
@@ -84,7 +84,7 @@ extern "C" int pips_split_bf16(const float* src, void* hi, void* lo, size_t n, v
     if (!src || !hi) return fail("pips_split_bf16: null pointer");
     if (n == 0) return 0;
     size_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > sm_count() * 16) blocks = sm_count() * 16;
     split_bf16_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         src, static_cast<__nv_bfloat16*>(hi), static_cast<__nv_bfloat16*>(lo), n);
     cudaError_t e = cudaGetLastError();

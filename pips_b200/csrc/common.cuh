@@ -36,7 +36,7 @@ bool encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, uint32_t rank, vo
 
 // ---- programmatic dependent launch (PDL).  Kernels of the per-iteration chain are launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's CTAs may become resident and run their
-// prologue (barrier init, TMEM allocation, tensor-map prefetch, weight staging into shared memory) while the previous
+// prologue (barrier init, tensor-map prefetch, weight staging into shared memory) while the previous
 // kernel drains; pdl_wait() blocks until every prerequisite grid has completed and its writes are visible, so it must
 // precede the first access to any buffer another kernel of the chain writes (and any global write).  pdl_trigger()
 // (issued at kernel entry) lets the dependent grid be scheduled as soon as all CTAs of this grid have started.
@@ -101,27 +101,13 @@ __device__ __forceinline__ float gelu_fast(float x) {
     return x * (x > 0.0f ? 1.0f - q : q);
 }
 
-// ---- packed fp32 pairs (Blackwell FFMA2 / FMUL2 / FADD2: one issue slot for two lanes of math) ----
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-    float2 d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;"
-        : "=l"(reinterpret_cast<uint64_t&>(d))
-        : "l"(reinterpret_cast<const uint64_t&>(a)), "l"(reinterpret_cast<const uint64_t&>(b)), "l"(reinterpret_cast<const uint64_t&>(c)));
-    return d;
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-    float2 d;
-    asm("mul.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<uint64_t&>(d)) : "l"(reinterpret_cast<const uint64_t&>(a)), "l"(reinterpret_cast<const uint64_t&>(b)));
-    return d;
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-    float2 d;
-    asm("add.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<uint64_t&>(d)) : "l"(reinterpret_cast<const uint64_t&>(a)), "l"(reinterpret_cast<const uint64_t&>(b)));
-    return d;
-}
+// ---- fp32 pairs: the same roundings per element as the scalar intrinsics (no contraction across calls) ----
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 bcast2(float v) { return make_float2(v, v); }
 
-// gelu_fast on two values at once: identical arithmetic per lane (same roundings), half the issue slots.
+// gelu_fast on two values at once: identical arithmetic per lane (same roundings).
 __device__ __forceinline__ float2 gelu_fast2(float2 x) {
     const float2 d = fma2(bcast2(0.27599915312530316f), make_float2(fabsf(x.x), fabsf(x.y)), bcast2(1.0f));
     float2 t;
@@ -144,7 +130,7 @@ __device__ __forceinline__ float2 gelu_fast2(float2 x) {
 // GELU(x) = x Phi(x) on two values, written without the sign select of gelu_fast2 (above):
 //   Phi(-|x|) = q(t) e^{-x^2/2},  t = 1 / (1 + p |x|)      (same 6-term fit)
 //   x Phi(x)  = x/2 + |x| (1/2 - Phi(-|x|))                 for both signs
-// 19 issue slots per pair instead of 24.  The rearrangement rounds 1/2 - Phi(-|x|) once more: an ABSOLUTE error of
+// The rearrangement rounds 1/2 - Phi(-|x|) once more: an ABSOLUTE error of
 // <= |x| 3e-8 (1e-7 at x = -3), far below the 2^-17 relative error of the bf16 (hi, lo) pair the value is then split into.
 __device__ __forceinline__ float2 gelu_fast2_abs(float2 x) {
     const float2 a = make_float2(fabsf(x.x), fabsf(x.y));

@@ -2,43 +2,36 @@
 // layer1 (nets/pips.py:135-136, :215) -- as an implicit GEMM that loads every input row ONCE.
 //
 // conv_tc.cu loads the A tile of each of the 9 filter taps as its own TMA box: 9 x 32 KB per 128-pixel tile, which at
-// Cin = 64 (one K-chunk per tap, 384 clk of MMAs per chunk) needs ~100 B/clk/SM from L2 -- 1.6x the SM's ingest limit;
-// ncu (round 1): tensor pipe 35 %.  Here a tile is 128 pixels of ONE output row and the CTA walks DOWN the image:
-//   * the three input rows a tile needs (y-1, y, y+1; 130 pixels each with the left/right halo, zero-filled outside the
-//     image by TMA) live in a 4-slot ring of row buffers; moving to the next output row loads ONE new row (33 KB for the
-//     (hi, lo) pair) -- 8.7x less operand traffic than 9 boxes per tile;
-//   * filter tap (dr, ds) is the 128 contiguous 128-byte pixels starting at pixel ds of ring row y+dr: an UMMA
+// Cin = 64 (one K-chunk per tap) makes operand traffic from L2, not the tensor cores, the limit.  Here a tile is 64
+// pixels of ONE output row and the CTA walks DOWN the image:
+//   * the three input rows a tile needs (y-1, y, y+1; 66 pixels each with the left/right halo, zero-filled outside the
+//     image by TMA) live in a 4-slot ring of row buffers; moving to the next output row loads ONE new row (16.5 KB for
+//     the (hi, lo) pair) -- 8.7x less operand traffic than 9 boxes per tile;
+//   * filter tap (dr, ds) is the 64 contiguous 128-byte pixels starting at pixel ds of ring row y+dr: a wgmma
 //     descriptor whose start address is offset by ds pixels (the swizzle follows absolute address bits: base offset 0);
-//   * all 9 taps' weights (72 KB per CTA) are loaded once per CTA and stay resident;
-//   * a CTA pair (cta_group::2, M = 256) covers 256 pixels of the row; the accumulator is 64 TMEM columns, 4 in flight;
-//   * InstanceNorm statistics (nets/pips.py:154-157) are accumulated in the epilogue: per work item (image, 256-pixel
-//     column block, 8 rows) and CTA one partial (sum, sum of squares) per channel -- the layout pips_inorm_finalize
-//     reduces in fp64, deterministic and independent of the batch size; the separate statistics pass over the 400 MB
-//     layer-1 activations disappears.
-//   * two MMAs per K step instead of three: these N = 64 MMAs are dispatch-bound (ncu: tensor pipe 45 % active at ~70 clk
-//     per instruction against 32 clk of math), so the hi*hi and hi*lo terms share ONE instruction with N = 128 --
-//     B = [w_hi ; w_lo], rank 0's shared memory holding the w_hi rows and rank 1's the w_lo rows -- into two 64-column
-//     partial accumulators, and lo*hi is a second instruction (N = 64) into the first; the epilogue adds the two partials.
+//   * all 9 taps' weights (144 KB, hi and lo) are loaded once per CTA and stay resident;
+//   * one consumer warpgroup (wgmma m64n64k16, accumulator in registers) per CTA; a work item is (image, 256-pixel column
+//     block, 8 rows, 128-pixel half "rank"), done as two 64-pixel strips;
+//   * InstanceNorm statistics (nets/pips.py:154-157) are accumulated in the epilogue: per work item one partial (sum, sum
+//     of squares) per channel -- the layout pips_inorm_finalize reduces in fp64, deterministic and independent of the
+//     batch size; the separate statistics pass over the layer-1 activations disappears.
 // Same bf16x3 products (hi*hi + lo*hi + hi*lo, fp32 accumulation) and K order (tap-major, then channel) as conv_tc.cu.
 #include "gemm_common.cuh"
 
 namespace pips {
 
-constexpr int R_THREADS = 384;                       // warp 0 TMA, 1 MMA, 2 TMEM, 3 idle, 4..11 epilogue
+constexpr int R_THREADS = 256;                       // warp 0 TMA, warps 1..3 idle, warps 4..7 the consumer warpgroup
 constexpr int R_ROWS_PER_ITEM = 8;
-constexpr int R_RING = 3;
-constexpr int R_BOX_PX = 130;                        // 128 output pixels + 1 halo pixel on each side
+constexpr int R_RING = 4;
+constexpr int R_STRIP = 64;                          // output pixels per tile
+constexpr int R_BOX_PX = R_STRIP + 2;                // + 1 halo pixel on each side
 constexpr uint32_t R_ROW_TX = R_BOX_PX * 128;        // bytes TMA writes per row and operand half (hi or lo)
-constexpr uint32_t R_ROW_BYTES = 17 * 1024;          // slot stride (1 KB aligned: SWIZZLE_128B pattern repeats every 1 KB)
-// Filter operands per tap and CTA (see "two MMAs per K step" below): [main: 64 rows x 128 B | second: 32 rows x 128 B]
-//   main    rank 0: w_hi rows 0..63     rank 1: w_lo rows 0..63      -> B of the N = 128 MMA  a_hi . [w_hi ; w_lo]
-//   second  rank 0: w_hi rows 0..31     rank 1: w_hi rows 32..63     -> B of the N = 64 MMA   a_lo . w_hi
-constexpr uint32_t R_W_MAIN = 64 * 128, R_W_SECOND = 32 * 128, R_W_TAP = R_W_MAIN + R_W_SECOND;   // 12 KB
-constexpr uint32_t R_OFF_W = R_RING * 2 * R_ROW_BYTES;            // 102 KB
-constexpr uint32_t R_OFF_COMB = R_OFF_W + 9 * R_W_TAP;            // +108 KB
-constexpr uint32_t R_OFF_BARS = R_OFF_COMB + 8 * 64 * 4;          // 8 epilogue warps x (32 sums + 32 sums of squares)
+constexpr uint32_t R_ROW_BYTES = 9 * 1024;           // slot stride (1 KB aligned: SWIZZLE_128B pattern repeats every 1 KB)
+constexpr uint32_t R_W_HALF = 64 * 128, R_W_TAP = 2 * R_W_HALF;   // per tap: [w_hi 64 rows x 128 B | w_lo]
+constexpr uint32_t R_OFF_W = R_RING * 2 * R_ROW_BYTES;            // 72 KB
+constexpr uint32_t R_OFF_COMB = R_OFF_W + 9 * R_W_TAP;            // +144 KB
+constexpr uint32_t R_OFF_BARS = R_OFF_COMB + 4 * 64 * 2 * 4;      // 4 consumer warps x 64 channels x (sum, sum of squares)
 constexpr uint32_t R_SMEM_BYTES = R_OFF_BARS + 256 + 1024;
-constexpr int R_ACC = 4;                             // accumulator stages of 128 TMEM columns (two partial sums, see below)
 
 struct RowsArgs {
     int N, H, W;
@@ -48,7 +41,7 @@ struct RowsArgs {
     float* partial;             // optional (N, px_blocks * row_chunks * 2, 2, 64)
 };
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(R_THREADS, 1)
+__global__ void __launch_bounds__(R_THREADS, 1)
 conv_rows_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                  const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo, const RowsArgs a) {
     pdl_trigger();
@@ -56,223 +49,165 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     float* comb = reinterpret_cast<float*>(smem + R_OFF_COMB);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + R_OFF_BARS);
-    const uint32_t wfull = smem_u32(bars);                 // leader: all 9 taps of both CTAs loaded
-    const uint32_t rfull0 = wfull + 8;                     // leader: ring slot filled in both CTAs
-    const uint32_t rempty0 = rfull0 + 8 * R_RING;          // per CTA: ring slot free (multicast commit)
-    const uint32_t tfull0 = rempty0 + 8 * R_RING;          // per CTA
-    const uint32_t tempty0 = tfull0 + 8 * R_ACC;           // leader
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 1 + 2 * R_RING + 2 * R_ACC);
+    const uint32_t wfull = smem_u32(bars);                 // all 9 taps loaded
+    const uint32_t rfull0 = wfull + 8;                     // ring slot filled
+    const uint32_t rempty0 = rfull0 + 8 * R_RING;          // ring slot free
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
     const int items_img = a.px_blocks * a.row_chunks;
-    const int num_items = a.N * items_img;
+    const int num_work = a.N * items_img * 2;              // (item, rank)
 
-    cluster_sync_all();
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&map_a_hi); tma_prefetch_desc(&map_a_lo);
         tma_prefetch_desc(&map_w_hi); tma_prefetch_desc(&map_w_lo);
     }
     if (warp == 1 && lane == 0) {
-        mbar_init(wfull, 2);
+        mbar_init(wfull, 1);
         for (int s = 0; s < R_RING; ++s) {
-            mbar_init(rfull0 + 8 * s, 2);
+            mbar_init(rfull0 + 8 * s, 1);
             mbar_init(rempty0 + 8 * s, 1);
-        }
-        for (int s = 0; s < R_ACC; ++s) {
-            mbar_init(tfull0 + 8 * s, 1);
-            mbar_init(tempty0 + 8 * s, 2 * (R_THREADS - 128));
         }
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc_pair(smem_u32(tmem_slot), R_ACC * 128);
-        tmem_relinquish_pair();
-    }
-    tc_fence_before();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
     const uint32_t ring0 = smem_u32(smem), wsm0 = smem_u32(smem + R_OFF_W);
 
     if (warp < 4) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
-        if (warp == 0) {
-            // ------------------------------------------------------------ TMA producer (both CTAs)
-            if (lane == 0) {
-                // the filter is a constant of the forward: loaded before the dependency wait
-                const uint32_t wb = leader_addr(wfull);
-                if (leader) mbar_arrive_expect_tx(wfull, 2 * 9 * R_W_TAP);
-                else mbar_arrive_cluster(wfull, 0);
-                const CUtensorMap* main_map = leader ? &map_w_hi : &map_w_lo;
-                for (int tap = 0; tap < 9; ++tap) {
-                    tma_load_2d_pair(wsm0 + tap * R_W_TAP, main_map, wb, tap * 64, 0);
-                    tma_load_2d_pair(wsm0 + tap * R_W_TAP + R_W_SECOND, main_map, wb, tap * 64, 32);
-                    tma_load_2d_pair(wsm0 + tap * R_W_TAP + R_W_MAIN, &map_w_hi, wb, tap * 64, static_cast<int>(rank) * 32);
-                }
-                pdl_wait();                                   // the activation comes from the previous kernel
-                uint32_t ld = 0;                              // rows loaded so far: slot = ld % R_RING
-                for (int item = pair; item < num_items; item += num_pairs) {
-                    const int img = item / items_img, rem = item - img * items_img;
-                    const int px = rem / a.row_chunks, y0 = (rem - px * a.row_chunks) * R_ROWS_PER_ITEM;
-                    const int y1 = min(a.H, y0 + R_ROWS_PER_ITEM);
-                    const int x0 = px * 256 + static_cast<int>(rank) * 128 - 1;
+        if (warp == 0 && lane == 0) {
+            // ------------------------------------------------------------ TMA producer
+            // the filter is a constant of the forward: loaded before the dependency wait
+            mbar_arrive_expect_tx(wfull, 9 * R_W_TAP);
+            for (int tap = 0; tap < 9; ++tap) {
+                tma_load_2d(wsm0 + tap * R_W_TAP, &map_w_hi, wfull, tap * 64, 0);
+                tma_load_2d(wsm0 + tap * R_W_TAP + R_W_HALF, &map_w_lo, wfull, tap * 64, 0);
+            }
+            pdl_wait();                                   // the activation comes from the previous kernel
+            uint32_t ld = 0;                              // rows loaded so far: slot = ld % R_RING
+            for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
+                const int item = work >> 1, rank = work & 1;
+                const int img = item / items_img, rem = item - img * items_img;
+                const int px = rem / a.row_chunks, y0 = (rem - px * a.row_chunks) * R_ROWS_PER_ITEM;
+                const int y1 = min(a.H, y0 + R_ROWS_PER_ITEM);
+                for (int strip = 0; strip < 2; ++strip) {
+                    const int xs = px * 256 + rank * 128 + strip * R_STRIP;
+                    if (xs >= a.W) continue;              // strip outside the image: nothing to compute
                     for (int yy = y0 - 1; yy <= y1; ++yy, ++ld) {
                         const uint32_t slot = ld % R_RING, phase = (ld / R_RING) & 1;
                         mbar_wait(rempty0 + 8 * slot, phase ^ 1);
-                        const uint32_t fb = leader_addr(rfull0 + 8 * slot);
-                        if (leader) mbar_arrive_expect_tx(rfull0 + 8 * slot, 2 * 2 * R_ROW_TX);
-                        else mbar_arrive_cluster(rfull0 + 8 * slot, 0);
-                        tma_load_4d_pair(ring0 + slot * 2 * R_ROW_BYTES, &map_a_hi, fb, 0, x0, yy, img);
-                        tma_load_4d_pair(ring0 + slot * 2 * R_ROW_BYTES + R_ROW_BYTES, &map_a_lo, fb, 0, x0, yy, img);
+                        const uint32_t fb = rfull0 + 8 * slot;
+                        mbar_arrive_expect_tx(fb, 2 * R_ROW_TX);
+                        tma_load_4d(ring0 + slot * 2 * R_ROW_BYTES, &map_a_hi, fb, 0, xs - 1, yy, img);
+                        tma_load_4d(ring0 + slot * 2 * R_ROW_BYTES + R_ROW_BYTES, &map_a_lo, fb, 0, xs - 1, yy, img);
                     }
                 }
             }
-            __syncwarp();
-        } else if (warp == 1) {
-            // ------------------------------------------------------------ MMA issuer (leader only)
-            // The whole warp runs this loop (warp-uniform control flow and values, so descriptors live in uniform
-            // registers); one elected lane issues.  With `if (lane == 0)` around the loop the compiler moved every operand
-            // of every MMA from vector to uniform registers under an election loop -- 14 instructions per MMA, which for
-            // these short N = 64 MMAs (108 per tile) made instruction issue, not the tensor pipe, the limit.
-            if (leader) {
-                constexpr uint32_t idesc_wide = umma_idesc_bf16(256, 128), idesc_narrow = umma_idesc_bf16(256, 64);
-                const bool elected = elect_one();
-                mbar_wait(wfull, 0);
-                uint32_t base_ld = 0, waited = 0;             // first ring index of the item; rows already waited for
-                int it = 0;
-                for (int item = pair; item < num_items; item += num_pairs) {
-                    const int rem = item % items_img;
-                    const int y0 = (rem % a.row_chunks) * R_ROWS_PER_ITEM;
-                    const int ntiles = min(a.H, y0 + R_ROWS_PER_ITEM) - y0;
-                    for (int j = 0; j < ntiles; ++j, ++it) {
-                        const uint32_t as = it % R_ACC, aphase = (it / R_ACC) & 1;
-                        mbar_wait(tempty0 + 8 * as, aphase ^ 1);
-                        tc_fence_after();
-                        const uint32_t d_tmem = tmem_base + as * 128;
-#pragma unroll
-                        for (int dr = 0; dr < 3; ++dr) {
-                            // rows arrive in order; the taps of filter row dr need ring index base + j + dr.  Waiting per filter
-                            // row (not for all three rows up front) and releasing a row right after its last use (below) lets a
-                            // 3-slot ring suffice: the load of the next row has 1.3 tile times before the tensor pipe needs it.
-                            while (waited <= base_ld + j + dr) {
-                                mbar_wait(rfull0 + 8 * (waited % R_RING), (waited / R_RING) & 1);
-                                ++waited;
-                            }
-                            tc_fence_after();
-                            const uint32_t row = ring0 + ((base_ld + j + dr) % R_RING) * 2 * R_ROW_BYTES;
-#pragma unroll
-                            for (int ds = 0; ds < 3; ++ds) {
-                                const uint32_t wt = wsm0 + (dr * 3 + ds) * R_W_TAP;
-                                // start address on pixel ds of the row buffer: the tensor core applies the 128-byte swizzle to
-                                // ABSOLUTE shared-memory address bits (as TMA did when it wrote the row), so a start that is a
-                                // whole number of 128-byte rows into the 1 KB pattern needs nothing else -- descriptor base
-                                // offset 0.  (Measured: with base offset = (addr >> 7) & 7 every ds != 0 tap is wrong.)
-                                const uint64_t a_hi = umma_desc_sw128(row + ds * 128);
-                                const uint64_t a_lo = umma_desc_sw128(row + R_ROW_BYTES + ds * 128);
-                                const uint64_t w_main = umma_desc_sw128(wt), w_second = umma_desc_sw128(wt + R_W_MAIN);
-#pragma unroll
-                                for (int k = 0; k < BK / UMMA_K; ++k) {
-                                    const uint64_t adv = static_cast<uint64_t>((k * UMMA_K * 2) >> 4);
-                                    if (elected) {
-                                        umma_f16_pair(d_tmem, a_hi + adv, w_main + adv, idesc_wide, (dr | ds | k) != 0);   // hi*hi | hi*lo
-                                        umma_f16_pair(d_tmem, a_lo + adv, w_second + adv, idesc_narrow, 1);                // + lo*hi
-                                    }
-                                }
-                            }
-                            // ring row base + j (input row y-1) had its last use in the dr = 0 taps of this tile
-                            if (dr == 0 && elected) umma_commit_pair(rempty0 + 8 * ((base_ld + j) % R_RING));
-                        }
-                        if (elected) {
-                            umma_commit_pair(tfull0 + 8 * as);
-                            if (j == ntiles - 1) {                                                 // the item's last two rows
-                                umma_commit_pair(rempty0 + 8 * ((base_ld + j + 1) % R_RING));
-                                umma_commit_pair(rempty0 + 8 * ((base_ld + j + 2) % R_RING));
-                            }
-                        }
-                        __syncwarp();
-                    }
-                    base_ld += ntiles + 2;
-                }
-            }
-            __syncwarp();
         }
     } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-        // ------------------------------------------------------------ epilogue (both CTAs, own 128 pixels)
+        // ------------------------------------------------------------ consumer warpgroup: MMA + epilogue
         pdl_wait();
-        const int q = warp & 3, half = (warp - 4) >> 2;       // TMEM lane quadrant; output channels half*32 .. +31
-        int it = 0;
-        for (int item = pair; item < num_items; item += num_pairs) {
+        const int w4 = warp & 3;
+        const bool releaser = (threadIdx.x & 127) == 0;
+        mbar_wait(wfull, 0);
+        uint32_t base_ld = 0, waited = 0;                 // first ring index of the strip; rows already waited for
+        float acc[32];
+        for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
+            const int item = work >> 1, rank = work & 1;
             const int img = item / items_img, rem = item - img * items_img;
             const int px = rem / a.row_chunks, chunk = rem - px * a.row_chunks;
             const int y0 = chunk * R_ROWS_PER_ITEM, ntiles = min(a.H, y0 + R_ROWS_PER_ITEM) - y0;
-            const int x = px * 256 + static_cast<int>(rank) * 128 + q * 32 + lane;
-            const bool ok = x < a.W;
-            float s[32], sq[32];
+            // statistics of this thread's columns 8j + 2(lane%4), +1
+            float ssum[8][2], ssq[8][2];
 #pragma unroll
-            for (int c = 0; c < 32; ++c) { s[c] = 0.f; sq[c] = 0.f; }
-            for (int j = 0; j < ntiles; ++j, ++it) {
-                const uint32_t as = it % R_ACC, aphase = (it / R_ACC) & 1;
-                mbar_wait(tfull0 + 8 * as, aphase);
-                tc_fence_after();
-                uint32_t v[32], v2[32];
-                const uint32_t tcol = tmem_base + as * 128 + half * 32 + (static_cast<uint32_t>(q * 32) << 16);
-                tmem_ld_32x32(tcol, v);                       // hi*hi + lo*hi
-                tmem_ld_32x32(tcol + 64, v2);                 // hi*lo
-                tmem_ld_wait();
+            for (int j = 0; j < 8; ++j) { ssum[j][0] = ssum[j][1] = 0.f; ssq[j][0] = ssq[j][1] = 0.f; }
+            for (int strip = 0; strip < 2; ++strip) {
+                const int xs = px * 256 + rank * 128 + strip * R_STRIP;
+                if (xs >= a.W) continue;
+                for (int j = 0; j < ntiles; ++j) {
+                    wgmma_fence();
 #pragma unroll
-                for (int c = 0; c < 32; ++c) v[c] = __float_as_uint(__uint_as_float(v[c]) + __uint_as_float(v2[c]));
-                tc_fence_before();
-                mbar_arrive_cluster(tempty0 + 8 * as, 0);     // values are in registers: the accumulator can be reused
-                if (ok) {
-                    float* orow = a.out + ((static_cast<size_t>(img) * a.H + (y0 + j)) * a.W + x) * 64 + half * 32;
+                    for (int dr = 0; dr < 3; ++dr) {
+                        // rows arrive in order; the taps of filter row dr need ring index base + j + dr
+                        while (waited <= base_ld + j + dr) {
+                            mbar_wait(rfull0 + 8 * (waited % R_RING), (waited / R_RING) & 1);
+                            ++waited;
+                        }
+                        const uint32_t row = ring0 + ((base_ld + j + dr) % R_RING) * 2 * R_ROW_BYTES;
 #pragma unroll
-                    for (int c = 0; c < 32; c += 4)
-                        *reinterpret_cast<float4*>(orow + c) = make_float4(__uint_as_float(v[c]), __uint_as_float(v[c + 1]),
-                                                                           __uint_as_float(v[c + 2]), __uint_as_float(v[c + 3]));
+                        for (int ds = 0; ds < 3; ++ds) {
+                            const uint32_t wt = wsm0 + (dr * 3 + ds) * R_W_TAP;
+                            // start address on pixel ds of the row buffer: the tensor core applies the 128-byte swizzle to
+                            // ABSOLUTE shared-memory address bits (as TMA did when it wrote the row), so a start that is a
+                            // whole number of 128-byte rows into the 1 KB pattern needs nothing else -- descriptor base offset 0
+                            const uint64_t a_hi = wgmma_desc_sw128(row + ds * 128);
+                            const uint64_t a_lo = wgmma_desc_sw128(row + R_ROW_BYTES + ds * 128);
+                            const uint64_t w_hi = wgmma_desc_sw128(wt), w_lo = wgmma_desc_sw128(wt + R_W_HALF);
 #pragma unroll
-                    for (int c = 0; c < 32; ++c) {
-                        const float f = __uint_as_float(v[c]);
-                        s[c] += f;
-                        sq[c] = fmaf(f, f, sq[c]);
+                            for (int k = 0; k < BK / MMA_K; ++k) {
+                                const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);
+                                wgmma_n64(acc, a_hi + adv, w_hi + adv, (dr | ds | k) != 0);
+                                wgmma_n64(acc, a_lo + adv, w_hi + adv, 1);
+                                wgmma_n64(acc, a_hi + adv, w_lo + adv, 1);
+                            }
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_acc_ready(acc);
+                    if (releaser) {
+                        mbar_arrive(rempty0 + 8 * ((base_ld + j) % R_RING));          // input row y-1: last use was this tile
+                        if (j == ntiles - 1) {                                          // the strip's last two rows
+                            mbar_arrive(rempty0 + 8 * ((base_ld + j + 1) % R_RING));
+                            mbar_arrive(rempty0 + 8 * ((base_ld + j + 2) % R_RING));
+                        }
+                    }
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int x = xs + w4 * 16 + (lane >> 2) + 8 * h;
+                        if (x < a.W) {
+                            float* orow = a.out + ((static_cast<size_t>(img) * a.H + (y0 + j)) * a.W + x) * 64 + 2 * (lane & 3);
+#pragma unroll
+                            for (int c = 0; c < 8; ++c) {
+                                const float2 o = make_float2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]);
+                                *reinterpret_cast<float2*>(orow + 8 * c) = o;
+                                ssum[c][0] += o.x; ssum[c][1] += o.y;
+                                ssq[c][0] = fmaf(o.x, o.x, ssq[c][0]); ssq[c][1] = fmaf(o.y, o.y, ssq[c][1]);
+                            }
+                        }
                     }
                 }
+                base_ld += ntiles + 2;
             }
             if (a.partial) {
-                // transpose-reduce over the warp's 32 pixels: lane c ends with the totals of channel half*32 + c
+                // totals over the pixels a warp's lanes hold (lanes with equal lane % 4 share columns), then over the
+                // four warps in a fixed order
+                float* mine = comb + w4 * 128;               // [column][sum, squares]
 #pragma unroll
-                for (int w = 16; w >= 1; w >>= 1) {
-                    const bool up = lane & w;
+                for (int c = 0; c < 8; ++c) {
 #pragma unroll
-                    for (int i = 0; i < w; ++i) {
-                        const float send_s = up ? s[i] : s[i + w], keep_s = up ? s[i + w] : s[i];
-                        const float send_q = up ? sq[i] : sq[i + w], keep_q = up ? sq[i + w] : sq[i];
-                        s[i] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, w);
-                        sq[i] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, w);
+                    for (int e = 0; e < 2; ++e) {
+                        float s = ssum[c][e], q = ssq[c][e];
+#pragma unroll
+                        for (int w = 4; w <= 16; w <<= 1) {
+                            s += __shfl_xor_sync(0xffffffffu, s, w);
+                            q += __shfl_xor_sync(0xffffffffu, q, w);
+                        }
+                        if (lane < 4) {
+                            const int col = 8 * c + 2 * lane + e;
+                            mine[col * 2] = s; mine[col * 2 + 1] = q;
+                        }
                     }
                 }
-                comb[(warp - 4) * 64 + lane] = s[0];
-                comb[(warp - 4) * 64 + 32 + lane] = sq[0];
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                if (q == 0) {                                  // warps 4 and 8: the four pixel quadrants in a fixed order
-                    const float* c0 = comb + (half * 4) * 64;
-                    const float ts = ((c0[lane] + c0[64 + lane]) + c0[128 + lane]) + c0[192 + lane];
-                    const float tq = ((c0[32 + lane] + c0[96 + lane]) + c0[160 + lane]) + c0[224 + lane];
+                asm volatile("bar.sync 1, 128;" ::: "memory");
+                const int col = threadIdx.x - 128;
+                if (col < 64) {
                     float* p = a.partial + ((static_cast<size_t>(img) * items_img + rem) * 2 + rank) * 128;
-                    p[half * 32 + lane] = ts;
-                    p[64 + half * 32 + lane] = tq;
+                    p[col] = ((comb[col * 2] + comb[128 + col * 2]) + comb[256 + col * 2]) + comb[384 + col * 2];
+                    p[64 + col] = ((comb[col * 2 + 1] + comb[128 + col * 2 + 1]) + comb[256 + col * 2 + 1]) + comb[384 + col * 2 + 1];
                 }
-                asm volatile("bar.sync 1, 256;" ::: "memory");  // comb is rewritten by the next item
+                asm volatile("bar.sync 1, 128;" ::: "memory");  // comb is rewritten by the next item
             }
         }
     }
-
-    tc_fence_before();
-    cluster_sync_all();
-    if (warp == 2) tmem_dealloc_pair(tmem_base, R_ACC * 128);
 }
 
 }  // namespace pips
@@ -307,7 +242,7 @@ extern "C" int pips_conv_rows(const void* x_hi, const void* x_lo, int N, int H, 
     {
         cuuint64_t gdim[2] = {9 * 64, 64};
         cuuint64_t gstr[1] = {9 * 64 * 2};
-        cuuint32_t box[2] = {64, 32};
+        cuuint32_t box[2] = {64, 64};
         cuuint32_t estr[2] = {1, 1};
         if (!encode_tiled(&mw_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_hi), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B) ||
             !encode_tiled(&mw_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_lo), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
@@ -318,10 +253,9 @@ extern "C" int pips_conv_rows(const void* x_hi, const void* x_lo, int N, int H, 
         cudaError_t e = ensure_dyn_smem(conv_rows_kernel, attr, R_SMEM_BYTES);
         if (e != cudaSuccess) return fail_cuda("pips_conv_rows: smem attribute", e);
     }
-    const int items = N * a.px_blocks * a.row_chunks;
-    const int max_pairs = sm_count() / 2;
-    const int pairs = items < max_pairs ? items : max_pairs;
-    cudaError_t e = launch_pdl(conv_rows_kernel, dim3(2 * pairs), dim3(R_THREADS), R_SMEM_BYTES, static_cast<cudaStream_t>(stream), ma_hi, ma_lo,
+    const int work = 2 * N * a.px_blocks * a.row_chunks;
+    const int grid = work < sm_count() ? work : sm_count();
+    cudaError_t e = launch_pdl(conv_rows_kernel, dim3(grid), dim3(R_THREADS), R_SMEM_BYTES, static_cast<cudaStream_t>(stream), ma_hi, ma_lo,
                                mw_hi, mw_lo, a);
     if (e == cudaSuccess) e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail_cuda("pips_conv_rows: launch", e);

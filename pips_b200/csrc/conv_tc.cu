@@ -1,14 +1,16 @@
-// 2-D convolution of the feature encoder as an implicit GEMM on CTA pairs (tcgen05.mma.cta_group::2).
+// 2-D convolution of the feature encoder as an implicit GEMM on the Hopper tensor cores (wgmma).
 //
 //   out[n, oy, ox, co] = sum_{r,s,ci} in[n, oy*st + r - pad, ox*st + s - pad, ci] * w[co, r, s, ci]   (+ bias[co])
 //
 // for the 3x3 / 1x1, stride 1 / 2 convolutions of BasicEncoder's residual stages and head
 // (nets/pips.py:135-136, :170, :221-223).  Activations are channels-last bf16 (hi, lo) pairs (v ~= hi + lo)
 // written by pips_inorm_apply / pips_resize_pair, weights are packed (Cout_pad, taps*Cp) bf16 (hi, lo), and
-// every product is evaluated as hi*hi + lo*hi + hi*lo with fp32 accumulation in TMEM -- the same bf16x3
-// scheme as the mixer GEMMs (gemm_tc2.cu), whose pipeline this kernel reuses:
-//   GEMM-M  = output pixels, one CTA = TH rows x TW columns = 128 pixels (a pair = two adjacent tiles)
-//   GEMM-N  = output channels (64 / 128 / 256; W rows split between the two CTAs of the pair)
+// every product is evaluated as hi*hi + lo*hi + hi*lo with fp32 accumulation -- the same bf16x3
+// scheme as the mixer GEMMs (gemm_tc.cu), whose pipeline this kernel reuses (TMA producer warp, two consumer
+// warpgroups of 64 pixels each):
+//   GEMM-M  = output pixels, one CTA = TH rows x TW columns = 128 pixels; CTAs 2p and 2p+1 ("ranks" of pair p)
+//             take two adjacent tiles, the unit of the statistics layout below
+//   GEMM-N  = output channels (64 / 128 / 256)
 //   GEMM-K  = taps x input channels; one K-chunk = 64 channels of one filter tap
 // The A tile of a K-chunk is ONE 4-D TMA box {64 ch, TW px, TH rows, 1 image} of the input at the tap's
 // offset (element strides = conv stride; out-of-bounds = zero padding), so no im2col buffer exists anywhere.
@@ -19,8 +21,8 @@ namespace pips {
 constexpr int C_THREADS = 384;
 constexpr uint32_t C_A_BYTES = 128 * BK * 2;          // 128 pixels x 64 channels bf16
 constexpr int C_MAX_STAGES = 8;
-constexpr uint32_t C_RING_BYTES = 192 * 1024;         // smem ring: stage = A_hi | A_lo | W_hi | W_lo, 2*(16 KB + BN/2*128 B)
-constexpr uint32_t C_COMB_BYTES = 8 * 4 * 64 * 4;      // statistics exchange: 8 epilogue warps x up to 4 chunks x (32 sums + 32 squares)
+constexpr uint32_t C_RING_BYTES = 200 * 1024;         // smem ring: stage = A_hi | A_lo | W_hi | W_lo, 2*(16 KB + BN*128 B)
+constexpr uint32_t C_COMB_BYTES = 8 * 8 * 64 * 4;      // statistics exchange: 8 consumer warps x 8 column quarters x (sum, squares) x 32
 constexpr uint32_t C_SMEM_BYTES = C_RING_BYTES + C_COMB_BYTES + 1024 + 256;
 
 struct ConvArgs {
@@ -30,7 +32,7 @@ struct ConvArgs {
     int TW, TH;                 // pixel tile: TW * TH == 128
     int tiles_x, tiles_y;       // tiles per image
     int BN;                     // GEMM-N tile == padded Cout: 64, 128 or 256
-    int stages;                 // ring depth: 3 (BN = 256) .. 4 (BN = 64)
+    int stages;                 // ring depth: 3 (BN = 256) .. 8 (BN = 64)
     const float* bias;          // [Cout] or null
     float* out;
     // Work items: the tiles of ONE image in groups of G consecutive pair tiles (pt_img pair tiles per image, groups_img
@@ -42,7 +44,8 @@ struct ConvArgs {
     float* partial;             // optional
 };
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(C_THREADS, 1)
+template <int BN>
+__global__ void __launch_bounds__(C_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo, const ConvArgs a) {
     pdl_trigger();
@@ -52,225 +55,167 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_RING_BYTES + C_COMB_BYTES);
     const uint32_t full0 = smem_u32(bars);
     const uint32_t empty0 = full0 + 8 * C_MAX_STAGES;
-    const uint32_t tfull0 = empty0 + 8 * C_MAX_STAGES;
-    const uint32_t tempty0 = tfull0 + 16;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * C_MAX_STAGES + 4);
     const int C_STAGES = a.stages;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
+    const int rank = blockIdx.x & 1;
     const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
 
     const int tiles_img = a.tiles_x * a.tiles_y;
     const int num_items = a.N * a.groups_img;
     const int chunks = a.Cp / BK;
     const int num_kb = a.R * a.S * chunks;
-    const uint32_t w_bytes = static_cast<uint32_t>(a.BN / 2) * BK * 2;       // this CTA's half of the weight tile
-    const uint32_t stage_tx = 2 * (C_A_BYTES + w_bytes);                      // per CTA: hi + lo
-    const uint32_t C_STAGE_BYTES = stage_tx;                                  // multiple of 1 KB for every BN
-    const uint32_t off_w_hi = 2 * C_A_BYTES, off_w_lo = 2 * C_A_BYTES + w_bytes;
+    constexpr uint32_t W_BYTES = BN * BK * 2;
+    constexpr uint32_t C_STAGE_BYTES = 2 * (C_A_BYTES + W_BYTES);             // hi + lo; multiple of 1 KB
+    constexpr uint32_t off_w_hi = 2 * C_A_BYTES, off_w_lo = 2 * C_A_BYTES + W_BYTES;
 
-    cluster_sync_all();
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&map_a_hi); tma_prefetch_desc(&map_a_lo);
         tma_prefetch_desc(&map_w_hi); tma_prefetch_desc(&map_w_lo);
     }
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < C_STAGES; ++s) {
-            mbar_init(full0 + 8 * s, 2);
-            mbar_init(empty0 + 8 * s, 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull0 + 8 * s, 1);
-            mbar_init(tempty0 + 8 * s, 2 * (C_THREADS - 128));
+            mbar_init(full0 + 8 * s, 1);
+            mbar_init(empty0 + 8 * s, 2);
         }
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc_pair(smem_u32(tmem_slot), 512);
-        tmem_relinquish_pair();
-    }
-    tc_fence_before();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
     pdl_wait();                                         // the activation operand comes from the previous kernel
 
     if (warp < 4) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
-        if (warp == 0) {
-            // ------------------------------------------------------------ TMA producer (both CTAs)
-            if (lane == 0) {
-                uint32_t stage = 0, phase = 0;
-                for (int item = pair; item < num_items; item += num_pairs) {
-                  const int img = item / a.groups_img, p0 = (item - img * a.groups_img) * a.G, p1 = min(a.pt_img, p0 + a.G);
-                  for (int ptl = p0; ptl < p1; ++ptl) {
-                    const int rem = 2 * ptl + static_cast<int>(rank);       // tile inside the image; == tiles_img: a tile past the
-                                                                            // last one (odd tile count), computed but never stored
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == 0 && lane == 0) {
+            // ------------------------------------------------------------ TMA producer
+            uint32_t stage = 0, phase = 0;
+            for (int item = pair; item < num_items; item += num_pairs) {
+                const int img = item / a.groups_img, p0 = (item - img * a.groups_img) * a.G, p1 = min(a.pt_img, p0 + a.G);
+                for (int ptl = p0; ptl < p1; ++ptl) {
+                    const int rem = 2 * ptl + rank;     // tile inside the image; == tiles_img: a tile past the
+                                                        // last one (odd tile count), computed but never stored
                     const int oy0 = (rem / a.tiles_x) * a.TH, ox0 = (rem % a.tiles_x) * a.TW;
-                    const int n0 = static_cast<int>(rank) * (a.BN / 2);
                     int kb = 0;
                     for (int r = 0; r < a.R; ++r) {
                         for (int s = 0; s < a.S; ++s) {
                             const int ix = ox0 * a.sx + s - a.px, iy = oy0 * a.sy + r - a.py;
                             for (int c = 0; c < chunks; ++c, ++kb) {
                                 mbar_wait(empty0 + 8 * stage, phase ^ 1);
-                                const uint32_t fb = leader_addr(full0 + 8 * stage);
-                                if (leader) mbar_arrive_expect_tx(full0 + 8 * stage, 2 * stage_tx);
-                                else mbar_arrive_cluster(full0 + 8 * stage, 0);
+                                const uint32_t fb = full0 + 8 * stage;
+                                mbar_arrive_expect_tx(fb, C_STAGE_BYTES);
                                 const uint32_t base = smem_u32(smem + stage * C_STAGE_BYTES);
-                                tma_load_4d_pair(base, &map_a_hi, fb, c * BK, ix, iy, img);
-                                tma_load_4d_pair(base + C_A_BYTES, &map_a_lo, fb, c * BK, ix, iy, img);
-                                tma_load_2d_pair(base + off_w_hi, &map_w_hi, fb, kb * BK, n0);
-                                tma_load_2d_pair(base + off_w_lo, &map_w_lo, fb, kb * BK, n0);
+                                tma_load_4d(base, &map_a_hi, fb, c * BK, ix, iy, img);
+                                tma_load_4d(base + C_A_BYTES, &map_a_lo, fb, c * BK, ix, iy, img);
+                                tma_load_2d(base + off_w_hi, &map_w_hi, fb, kb * BK, 0);
+                                tma_load_2d(base + off_w_lo, &map_w_lo, fb, kb * BK, 0);
                                 if (++stage == C_STAGES) { stage = 0; phase ^= 1; }
                             }
                         }
                     }
-                  }
                 }
             }
-            __syncwarp();
-        } else if (warp == 1) {
-            // ------------------------------------------------------------ MMA issuer (leader only)
-            // whole warp, warp-uniform control flow (descriptors stay in uniform registers); one elected lane issues
-            if (leader) {
-                const bool elected = elect_one();
-                const uint32_t idesc = umma_idesc_bf16(256, a.BN);
-                uint32_t stage = 0, phase = 0;
-                int it = 0;
-                for (int item = pair; item < num_items; item += num_pairs) {
-                  const int g0 = (item % a.groups_img) * a.G, ntl = min(a.pt_img, g0 + a.G) - g0;
-                  for (int jt = 0; jt < ntl; ++jt, ++it) {
-                    const uint32_t as = it & 1, aphase = (it >> 1) & 1;
-                    mbar_wait(tempty0 + 8 * as, aphase ^ 1);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + as * 256;
-                    for (int kb = 0; kb < num_kb; ++kb) {
-                        mbar_wait(full0 + 8 * stage, phase);
-                        tc_fence_after();
-                        const uint32_t base = smem_u32(smem + stage * C_STAGE_BYTES);
-                        const uint64_t a_hi = umma_desc_sw128(base);
-                        const uint64_t a_lo = umma_desc_sw128(base + C_A_BYTES);
-                        const uint64_t w_hi = umma_desc_sw128(base + off_w_hi);
-                        const uint64_t w_lo = umma_desc_sw128(base + off_w_lo);
-#pragma unroll
-                        for (int k = 0; k < BK / UMMA_K; ++k) {
-                            const uint64_t adv = static_cast<uint64_t>((k * UMMA_K * 2) >> 4);
-                            if (elected) umma_f16_pair(d_tmem, a_hi + adv, w_hi + adv, idesc, (kb | k) != 0);
-                            if (elected) umma_f16_pair(d_tmem, a_lo + adv, w_hi + adv, idesc, 1);
-                            if (elected) umma_f16_pair(d_tmem, a_hi + adv, w_lo + adv, idesc, 1);
-                        }
-                        if (elected) umma_commit_pair(empty0 + 8 * stage);
-                        if (elected && kb == num_kb - 1) umma_commit_pair(tfull0 + 8 * as);
-                        if (++stage == C_STAGES) { stage = 0; phase ^= 1; }
-                    }
-                  }
-                }
-            }
-            __syncwarp();
         }
     } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-        // ------------------------------------------------------------ epilogue (both CTAs, own 128 pixels)
-        const int q = warp & 3;
-        const int half = (warp - 4) >> 2;
-        const int half_cols = a.BN / 2;                       // 32, 64 or 128 columns per epilogue half
-        int it = 0;
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        // ------------------------------------------------------------ consumers: MMA + epilogue, 64 pixels each
+        const int wg = (warp - 4) >> 2, w4 = warp & 3;
+        const bool releaser = (threadIdx.x & 127) == 0;
+        constexpr int NJ = BN / 8;                            // 8-column blocks of the accumulator
+        float acc[BN / 2];
+        uint32_t stage = 0, phase = 0;
         for (int item = pair; item < num_items; item += num_pairs) {
             const int img = item / a.groups_img, grp = item - img * a.groups_img;
             const int p0 = grp * a.G, p1 = min(a.pt_img, p0 + a.G);
-            float ssum[4] = {0.f, 0.f, 0.f, 0.f}, ssq[4] = {0.f, 0.f, 0.f, 0.f};     // lane j: channel chunk*32 + j of this warp's half
-            for (int ptl = p0; ptl < p1; ++ptl, ++it) {
-                const uint32_t as = it & 1, aphase = (it >> 1) & 1;
-                const int rem = 2 * ptl + static_cast<int>(rank);
-                const int i = q * 32 + lane;                      // pixel index inside the tile
-                const int oy = (rem / a.tiles_x) * a.TH + i / a.TW, ox = (rem % a.tiles_x) * a.TW + i % a.TW;
-                const bool ok = rem < tiles_img && oy < a.Ho && ox < a.Wo;
-                float* orow = a.out + ((static_cast<size_t>(img) * a.Ho + oy) * a.Wo + ox) * a.Cout;
-                mbar_wait(tfull0 + 8 * as, aphase);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + as * 256 + half * half_cols + (static_cast<uint32_t>(q * 32) << 16);
+            // per-warp statistics of the item: mine[column] = (sum, sum of squares) over the warp's pixels
+            float* mine = comb + (warp - 4) * (BN * 2);
+            if (a.partial) {
+                for (int i = lane; i < BN * 2; i += 32) mine[i] = 0.f;
+                __syncwarp();
+            }
+            for (int ptl = p0; ptl < p1; ++ptl) {
+                int prev = -1;
+                for (int kb = 0; kb < num_kb; ++kb) {
+                    mbar_wait(full0 + 8 * stage, phase);
+                    const uint32_t base = smem_u32(smem + stage * C_STAGE_BYTES);
+                    const uint64_t a_hi = wgmma_desc_sw128(base + wg * (C_A_BYTES / 2));
+                    const uint64_t a_lo = wgmma_desc_sw128(base + C_A_BYTES + wg * (C_A_BYTES / 2));
+                    const uint64_t w_hi = wgmma_desc_sw128(base + off_w_hi);
+                    const uint64_t w_lo = wgmma_desc_sw128(base + off_w_lo);
+                    wgmma_fence();
 #pragma unroll
-                for (int ci = 0; ci < 4; ++ci) {
-                    const int c0 = ci * 32;
-                    if (c0 < half_cols) {                         // warp-uniform
-                        uint32_t v[32];
-                        tmem_ld_32x32(taddr + c0, v);
-                        tmem_ld_wait();
-                        const int col = half * half_cols + c0;
-                        if (ok && col < a.Cout) {
+                    for (int k = 0; k < BK / MMA_K; ++k) {
+                        const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);
+                        wgmma_tile<BN>(acc, a_hi + adv, w_hi + adv, (kb | k) != 0);
+                        wgmma_tile<BN>(acc, a_lo + adv, w_hi + adv, 1);
+                        wgmma_tile<BN>(acc, a_hi + adv, w_lo + adv, 1);
+                    }
+                    wgmma_commit();
+                    if (prev >= 0) {
+                        wgmma_wait<1>();
+                        if (releaser) mbar_arrive(empty0 + 8 * prev);
+                    }
+                    prev = static_cast<int>(stage);
+                    if (++stage == C_STAGES) { stage = 0; phase ^= 1; }
+                }
+                wgmma_wait<0>();
+                wgmma_acc_ready(acc);
+                if (releaser) mbar_arrive(empty0 + 8 * prev);
+
+                const int rem = 2 * ptl + rank;
+                const int i0 = wg * 64 + w4 * 16 + (lane >> 2);             // pixel index inside the tile (and i0 + 8)
+                bool ok[2];
+                float* orow[2];
 #pragma unroll
-                            for (int j = 0; j < 32; j += 4) {
-                                if (col + j < a.Cout) {           // Cout is a multiple of 4
-                                    float4 o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                                                           __uint_as_float(v[j + 3]));
-                                    if (a.bias) {
-                                        const float4 b = __ldg(reinterpret_cast<const float4*>(a.bias + col + j));
-                                        o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w;
-                                        v[j] = __float_as_uint(o.x); v[j + 1] = __float_as_uint(o.y);
-                                        v[j + 2] = __float_as_uint(o.z); v[j + 3] = __float_as_uint(o.w);
-                                    }
-                                    *reinterpret_cast<float4*>(orow + col + j) = o;
-                                }
-                            }
+                for (int h = 0; h < 2; ++h) {
+                    const int i = i0 + 8 * h;
+                    const int oy = (rem / a.tiles_x) * a.TH + i / a.TW, ox = (rem % a.tiles_x) * a.TW + i % a.TW;
+                    ok[h] = rem < tiles_img && oy < a.Ho && ox < a.Wo;
+                    orow[h] = a.out + ((static_cast<size_t>(img) * a.Ho + oy) * a.Wo + ox) * a.Cout;
+                }
+#pragma unroll
+                for (int j = 0; j < NJ; ++j) {
+                    const int col = 8 * j + 2 * (lane & 3);
+                    const bool cok = col < a.Cout;                    // Cout is a multiple of 4: column pairs are whole
+                    float2 b = make_float2(0.f, 0.f);
+                    if (a.bias && cok) b = __ldg(reinterpret_cast<const float2*>(a.bias + col));
+                    float2 s = make_float2(0.f, 0.f), q = make_float2(0.f, 0.f);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (ok[h] && cok) {
+                            const float2 o = make_float2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
+                            *reinterpret_cast<float2*>(orow[h] + col) = o;
+                            s.x += o.x; s.y += o.y;
+                            q.x = fmaf(o.x, o.x, q.x); q.y = fmaf(o.y, o.y, q.y);
                         }
-                        if (a.partial) {
-                            // transpose-reduce over the warp's 32 pixels (pixels outside the image contribute 0):
-                            // lane j ends with this tile's totals of channel col + j
-                            float s[32], sq[32];
+                    }
+                    if (a.partial) {
+                        // totals over the warp's 16 pixels: lanes with equal lane % 4 hold the same columns
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) {
-                                const float f = ok ? __uint_as_float(v[j]) : 0.f;
-                                s[j] = f; sq[j] = f * f;
-                            }
-#pragma unroll
-                            for (int w = 16; w >= 1; w >>= 1) {
-                                const bool up = lane & w;
-#pragma unroll
-                                for (int j = 0; j < w; ++j) {
-                                    const float send_s = up ? s[j] : s[j + w], keep_s = up ? s[j + w] : s[j];
-                                    const float send_q = up ? sq[j] : sq[j + w], keep_q = up ? sq[j + w] : sq[j];
-                                    s[j] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, w);
-                                    sq[j] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, w);
-                                }
-                            }
-                            ssum[ci] += s[0];
-                            ssq[ci] += sq[0];
+                        for (int w = 4; w <= 16; w <<= 1) {
+                            s.x += __shfl_xor_sync(0xffffffffu, s.x, w); s.y += __shfl_xor_sync(0xffffffffu, s.y, w);
+                            q.x += __shfl_xor_sync(0xffffffffu, q.x, w); q.y += __shfl_xor_sync(0xffffffffu, q.y, w);
                         }
-                        __syncwarp();
+                        if (lane < 4 && cok) {
+                            mine[col * 2] += s.x; mine[col * 2 + 1] += q.x;
+                            mine[col * 2 + 2] += s.y; mine[col * 2 + 3] += q.y;
+                        }
                     }
                 }
-                tc_fence_before();
-                mbar_arrive_cluster(tempty0 + 8 * as, 0);
             }
             if (a.partial) {
-                float* mine = comb + (warp - 4) * 256;            // [chunk][sum 32 | squares 32]
-#pragma unroll
-                for (int ci = 0; ci < 4; ++ci) { mine[ci * 64 + lane] = ssum[ci]; mine[ci * 64 + 32 + lane] = ssq[ci]; }
+                // the 8 consumer warps' totals in a fixed order
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-                if (q == 0) {                                      // warps 4 and 8: the four pixel quadrants in a fixed order
-                    const float* c4 = comb + (half * 4) * 256;
-                    float* p = a.partial + ((static_cast<size_t>(img) * a.groups_img + grp) * 2 + rank) * 2 * a.Cout;
+                float* p = a.partial + ((static_cast<size_t>(img) * a.groups_img + grp) * 2 + rank) * 2 * a.Cout;
+                for (int col = threadIdx.x - 128; col < a.Cout; col += 256) {
+                    float s = 0.f, q = 0.f;
 #pragma unroll
-                    for (int ci = 0; ci < 4; ++ci) {
-                        const int col = half * half_cols + ci * 32 + lane;
-                        if (ci * 32 < half_cols && col < a.Cout) {
-                            const float* e = c4 + ci * 64;
-                            p[col] = ((e[lane] + e[256 + lane]) + e[512 + lane]) + e[768 + lane];
-                            p[a.Cout + col] = ((e[32 + lane] + e[256 + 32 + lane]) + e[512 + 32 + lane]) + e[768 + 32 + lane];
-                        }
-                    }
+                    for (int w = 0; w < 8; ++w) { s += comb[w * (BN * 2) + col * 2]; q += comb[w * (BN * 2) + col * 2 + 1]; }
+                    p[col] = s;
+                    p[a.Cout + col] = q;
                 }
                 asm volatile("bar.sync 1, 256;" ::: "memory");    // comb is rewritten by the next item
             }
         }
     }
-
-    tc_fence_before();
-    cluster_sync_all();
-    if (warp == 2) tmem_dealloc_pair(tmem_base, 512);
 }
 
 }  // namespace pips
@@ -292,6 +237,23 @@ static void conv_geometry(int Ho, int Wo, int sx, ConvArgs& a) {
     a.groups_img = (a.pt_img + a.G - 1) / a.G;
 }
 
+template <int BN>
+static int conv_tc_launch(const CUtensorMap& ma_hi, const CUtensorMap& ma_lo, const CUtensorMap& mw_hi, const CUtensorMap& mw_lo,
+                          const ConvArgs& a, void* stream) {
+    static bool attr[kMaxDevices] = {};
+    {
+        cudaError_t e = ensure_dyn_smem(conv_tc_kernel<BN>, attr, C_SMEM_BYTES);
+        if (e != cudaSuccess) return fail_cuda("pips_conv_tc: smem attribute", e);
+    }
+    const int items = a.N * a.groups_img;
+    const int max_pairs = sm_count() / 2;
+    const int pairs = items < max_pairs ? items : max_pairs;
+    cudaError_t e = launch_pdl(conv_tc_kernel<BN>, dim3(2 * pairs), dim3(C_THREADS), C_SMEM_BYTES, static_cast<cudaStream_t>(stream), ma_hi,
+                               ma_lo, mw_hi, mw_lo, a);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail_cuda("pips_conv_tc: launch", e);
+}
+
 static int conv_tc_impl(const void* x_hi, const void* x_lo, int N, int H, int W, int Cp, const void* w_hi, const void* w_lo,
                         int Cout, int R, int S, int sy, int sx, int py, int px, const float* bias, float* out, float* partial,
                         void* stream) {
@@ -306,9 +268,9 @@ static int conv_tc_impl(const void* x_hi, const void* x_lo, int N, int H, int W,
     a.N = N; a.Ho = Ho; a.Wo = Wo; a.Cout = Cout; a.Cp = Cp; a.R = R; a.S = S; a.sy = sy; a.sx = sx; a.py = py; a.px = px;
     a.BN = Cout <= 64 ? 64 : (Cout <= 128 ? 128 : 256);
     {
-        const uint32_t stage = 2 * (C_A_BYTES + static_cast<uint32_t>(a.BN / 2) * BK * 2);
+        const uint32_t stage = 2 * (C_A_BYTES + static_cast<uint32_t>(a.BN) * BK * 2);
         int st = static_cast<int>(C_RING_BYTES / stage);
-        a.stages = st > C_MAX_STAGES ? C_MAX_STAGES : st;      // BN 256: 3 x 64 KB, 128: 4 x 48 KB, 64: 4 x 40 KB
+        a.stages = st > C_MAX_STAGES ? C_MAX_STAGES : st;      // BN 256: 2 x 96 KB, 128: 3 x 64 KB, 64: 4 x 48 KB
     }
     conv_geometry(Ho, Wo, sx, a);
     a.bias = bias; a.out = out; a.partial = partial;
@@ -328,24 +290,15 @@ static int conv_tc_impl(const void* x_hi, const void* x_lo, int N, int H, int W,
         const int K = R * S * Cp;
         cuuint64_t gdim[2] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(a.BN)};
         cuuint64_t gstr[1] = {static_cast<cuuint64_t>(K) * 2};
-        cuuint32_t box[2] = {static_cast<cuuint32_t>(BK), static_cast<cuuint32_t>(a.BN / 2)};
+        cuuint32_t box[2] = {static_cast<cuuint32_t>(BK), static_cast<cuuint32_t>(a.BN)};
         cuuint32_t estr[2] = {1, 1};
         if (!encode_tiled(&mw_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_hi), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B) ||
             !encode_tiled(&mw_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_lo), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
             return fail("pips_conv_tc: weight tensor map failed");
     }
-    static bool attr[kMaxDevices] = {};
-    {
-        cudaError_t e = ensure_dyn_smem(conv_tc_kernel, attr, C_SMEM_BYTES);
-        if (e != cudaSuccess) return fail_cuda("pips_conv_tc: smem attribute", e);
-    }
-    const int items = N * a.groups_img;
-    const int max_pairs = sm_count() / 2;
-    const int pairs = items < max_pairs ? items : max_pairs;
-    cudaError_t e = launch_pdl(conv_tc_kernel, dim3(2 * pairs), dim3(C_THREADS), C_SMEM_BYTES, static_cast<cudaStream_t>(stream), ma_hi, ma_lo,
-                               mw_hi, mw_lo, a);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail_cuda("pips_conv_tc: launch", e);
+    return a.BN == 64 ? conv_tc_launch<64>(ma_hi, ma_lo, mw_hi, mw_lo, a, stream)
+         : a.BN == 128 ? conv_tc_launch<128>(ma_hi, ma_lo, mw_hi, mw_lo, a, stream)
+                       : conv_tc_launch<256>(ma_hi, ma_lo, mw_hi, mw_lo, a, stream);
 }
 
 extern "C" int pips_conv_tc(const void* x_hi, const void* x_lo, int N, int H, int W, int Cp, const void* w_hi, const void* w_lo,

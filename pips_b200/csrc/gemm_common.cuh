@@ -1,4 +1,4 @@
-// Shared pieces of the tcgen05 dense-layer kernels (gemm_tc.cu: one CTA per tile; gemm_tc2.cu: CTA pairs).
+// Shared pieces of the wgmma kernels (gemm_tc.cu, conv_tc.cu, conv_rows.cu).
 #pragma once
 #include <cuda_bf16.h>
 
@@ -8,8 +8,7 @@
 namespace pips {
 
 constexpr int BK = 64;                       // 64 bf16 = one 128-byte swizzle row
-constexpr int UMMA_K = 16;
-constexpr uint32_t EPI_STAGE_BYTES = 8 * 4096;     // 8 epilogue warps x 4 KB store-staging tile
+constexpr int MMA_K = 16;
 
 struct GemmArgs {
     int M, N, K;                 // valid rows / cols, K multiple of 64
@@ -20,107 +19,51 @@ struct GemmArgs {
     __nv_bfloat16* out_hi;       // BIAS_GELU target (row stride ldh); out_lo may be null
     __nv_bfloat16* out_lo;
     int ldh;
-    // CTA-pair kernel only (gemm_tc2.cu): tiles [0, pair_full_tiles) are 256x256; then pair p < pair_narrow_tiles takes
-    // the 256x128 tile p of the remaining 256x256 tiles split in two column halves (0: no narrow tiles)
-    int pair_full_tiles, pair_narrow_tiles;
 };
 
-
-// Bias of one 32-column chunk (same for every row).  Kept separate from epilogue_chunk so that the loads can
-// be issued BEFORE tcgen05.wait::ld and overlap the TMEM load (the wait is a compiler barrier for memory ops).
-__device__ __forceinline__ void load_bias_chunk(const GemmArgs& args, int col, float (&b)[32]) {
-    if (col + 32 <= args.N) {
+// Epilogue of a warpgroup's 64 x BN accumulator (wgmma fragment layout, ptx.cuh): bias, then GELU + (hi, lo) split, or
+// fp32 store with optional residual.  Every thread owns column pairs (col, col + 1) of two rows, so stores are 8-byte
+// (fp32) or 4-byte (bf16 pair) pieces and the four threads of a quad cover 32 / 16 contiguous bytes of a row.
+// `row0` is the first of the warpgroup's 64 rows, `n0` the tile's first column.
+template <int BN>
+__device__ __forceinline__ void epilogue_frag(const GemmArgs& args, const float (&acc)[BN / 2], int row0, int n0) {
+    const int lane = threadIdx.x & 31;
+    const int r0 = row0 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+    const bool gelu = args.epilogue == PIPS_EPI_BIAS_GELU, resid = args.epilogue == PIPS_EPI_BIAS_RESID;
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-            const float4 t = __ldg(reinterpret_cast<const float4*>(args.bias + col + j));
-            b[j] = t.x; b[j + 1] = t.y; b[j + 2] = t.z; b[j + 3] = t.w;
-        }
-    } else {
+    for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + 2 * (lane & 3);
+        if (col >= args.N) continue;
+        const bool two = col + 1 < args.N;
+        const float2 b = make_float2(__ldg(args.bias + col), two ? __ldg(args.bias + col + 1) : 0.f);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) b[j] = col + j < args.N ? __ldg(args.bias + col + j) : 0.f;
-    }
-}
-
-// Epilogue of one 32-column chunk of the warp's 32 output rows (one row per thread): bias, then GELU + (hi, lo)
-// split, or fp32 store with optional residual.  `col` and the chunk predicates are warp-uniform.
-// `b` holds this chunk's bias on entry; once it is consumed the bias of column `next_col` (if >= 0) is loaded into
-// it, so those loads are in flight during the GELU / store work and the next TMEM wait.
-// `row0` is the first of the warp's 32 rows (thread = row0 + lane); `stage` the warp's 4 KB smem staging tile.
-__device__ __forceinline__ void epilogue_chunk(const GemmArgs& args, const uint32_t (&v)[32], float (&b)[32], int row0,
-                                               int col, int next_col, uint8_t* stage) {
-    const int row = row0 + (threadIdx.x & 31);
-    const bool row_ok = row < args.M;
-    float f[32];
-#pragma unroll
-    for (int j = 0; j < 32; j += 2) {
-        const float2 t = add2(make_float2(__uint_as_float(v[j]), __uint_as_float(v[j + 1])), make_float2(b[j], b[j + 1]));
-        f[j] = t.x; f[j + 1] = t.y;
-    }
-    if (next_col >= 0) load_bias_chunk(args, next_col, b);
-    if (col >= args.N) return;                           // warp-uniform
-    const bool full_chunk = col + 32 <= args.N;
-    if (args.epilogue == PIPS_EPI_BIAS_GELU) {
-        if (full_chunk) {
-            // Transpose through the warp's 4 KB staging tile so that global stores are 64-byte runs of full
-            // sectors (4 rows x {hi 64 B, lo 64 B} per instruction) instead of 32 scattered 16-byte pieces.
-            // Row r of the tile is [hi: 4 x 16 B | lo: 4 x 16 B], piece p stored at p ^ (r & 7): conflict-free
-            // both for the row-per-thread writes and the 8-threads-per-row reads.
-            const int lane = threadIdx.x & 31;
-            uint8_t* myrow = stage + lane * 128;
-#pragma unroll
-            for (int p = 0; p < 4; ++p) {
-                uint32_t hw[4], lw[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const float2 g = gelu_fast2_abs(make_float2(f[8 * p + 2 * e], f[8 * p + 2 * e + 1]));
-                    hw[e] = cvt_bf16x2(g.x, g.y);
-                    const float2 lo = fma2(make_float2(__uint_as_float(hw[e] << 16), __uint_as_float(hw[e] & 0xffff0000u)),
-                                           bcast2(-1.0f), g);                       // g - hi, one rounding
-                    lw[e] = cvt_bf16x2(lo.x, lo.y);
+        for (int h = 0; h < 2; ++h) {
+            const int row = r0 + 8 * h;
+            if (row >= args.M) continue;
+            const float2 f = add2(make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]), b);
+            if (gelu) {
+                const float2 g = gelu_fast2_abs(f);
+                const uint32_t hw = cvt_bf16x2(g.x, g.y);
+                const float2 lo = fma2(make_float2(__uint_as_float(hw << 16), __uint_as_float(hw & 0xffff0000u)), bcast2(-1.0f), g);   // g - hi, one rounding
+                const uint32_t lw = cvt_bf16x2(lo.x, lo.y);
+                const size_t o = static_cast<size_t>(row) * args.ldh + col;
+                if (two) {
+                    *reinterpret_cast<uint32_t*>(args.out_hi + o) = hw;
+                    if (args.out_lo) *reinterpret_cast<uint32_t*>(args.out_lo + o) = lw;
+                } else {
+                    args.out_hi[o] = __ushort_as_bfloat16(static_cast<unsigned short>(hw & 0xffffu));
+                    if (args.out_lo) args.out_lo[o] = __ushort_as_bfloat16(static_cast<unsigned short>(lw & 0xffffu));
                 }
-                *reinterpret_cast<uint4*>(myrow + ((p ^ (lane & 7)) << 4)) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                *reinterpret_cast<uint4*>(myrow + (((p + 4) ^ (lane & 7)) << 4)) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-            }
-            __syncwarp();
-            const int piece = lane & 7;
-            __nv_bfloat16* dst = piece < 4 ? args.out_hi : args.out_lo;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int r = i * 4 + (lane >> 3);
-                const uint4 d = *reinterpret_cast<const uint4*>(stage + r * 128 + ((piece ^ (r & 7)) << 4));
-                const int grow = row0 + r;
-                if (dst && grow < args.M)
-                    *reinterpret_cast<uint4*>(dst + static_cast<size_t>(grow) * args.ldh + col + (piece & 3) * 8) = d;
-            }
-            __syncwarp();
-        } else if (row_ok) {
-            __nv_bfloat16* ph = args.out_hi + static_cast<size_t>(row) * args.ldh + col;
-            __nv_bfloat16* pl = args.out_lo ? args.out_lo + static_cast<size_t>(row) * args.ldh + col : nullptr;
-            for (int e = 0; e < 32; ++e) {
-                if (col + e < args.N) {
-                    const float g = gelu_fast(f[e]);
-                    const __nv_bfloat16 h = __float2bfloat16_rn(g);
-                    ph[e] = h;
-                    if (pl) pl[e] = __float2bfloat16_rn(g - __bfloat162float(h));
+            } else {
+                float* po = args.out_f32 + static_cast<size_t>(row) * args.ldo + col;
+                if (two) {
+                    float2 o = f;
+                    if (resid) { const float2 r = *reinterpret_cast<const float2*>(po); o.x += r.x; o.y += r.y; }
+                    *reinterpret_cast<float2*>(po) = o;
+                } else {
+                    po[0] = resid ? po[0] + f.x : f.x;
                 }
             }
-        }
-    } else if (row_ok) {
-        float* po = args.out_f32 + static_cast<size_t>(row) * args.ldo + col;
-        const bool resid = args.epilogue == PIPS_EPI_BIAS_RESID;
-        if (full_chunk) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-                float4 o = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-                if (resid) {
-                    const float4 r = *reinterpret_cast<const float4*>(po + j);
-                    o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
-                }
-                *reinterpret_cast<float4*>(po + j) = o;
-            }
-        } else {
-            for (int j = 0; j < 32; ++j)
-                if (col + j < args.N) po[j] = resid ? po[j] + f[j] : f[j];
         }
     }
 }

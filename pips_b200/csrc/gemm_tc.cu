@@ -1,23 +1,24 @@
-// Mixer dense layers on the 5th-gen tensor cores (tcgen05.mma, accumulators in TMEM).
+// Mixer dense layers on the Hopper tensor cores (wgmma, accumulators in registers).
 //
 //   C[M,N] = epilogue( A[M,K] . W[N,K]^T + bias[N] )
 //
 // A (activations) and W (nn.Linear weight, (out,in) == N x K, K-major) are bf16.  In the
 // "bf16x3" precision mode both operands are carried as a (hi, lo) bf16 pair with
 // v ~= hi + lo, and the product is evaluated as A_hi.W_hi + A_lo.W_hi + A_hi.W_lo with fp32
-// accumulation in TMEM (relative error ~2^-16 per product instead of 2^-8), which is what the
+// accumulation (relative error ~2^-16 per product instead of 2^-8), which is what the
 // 1e-3 px parity target of the refinement loop needs (reference: fp32 nn.Linear,
 // nets/pips.py:104-107,:115,:122).
 //
 // Structure (one CTA per SM, persistent over 128 x BN output tiles; BN = 256 for large problems, 128 / 64 when
 // 256-wide tiles would leave most SMs without a tile -- few particles: the demo clip, chained windows):
-//   warp 0      TMA producer   : cp.async.bulk.tensor 128B-swizzled K-chunks of A and W -> smem ring
-//   warp 1      MMA issuer     : one elected lane issues tcgen05.mma (M=128,N=256,K=16) per chunk/term
-//   warp 2      TMEM allocator
-//   warps 4..11 epilogue       : tcgen05.ld the fp32 tile (one row per thread, two warps per lane quadrant),
-//                                bias / GELU(erf) / residual / hi-lo split, vectorised stores
-// The accumulator is double-buffered in TMEM (2 x 256 columns) so the epilogue of tile i
-// overlaps the MMAs of tile i+1.
+//   warp 0       TMA producer  : cp.async.bulk.tensor 128B-swizzled K-chunks of A and W -> smem ring
+//   warps 4..7   consumer warpgroup 0: rows 0..63 of the tile   } wgmma m64nNk16 straight from the ring, then the
+//   warps 8..11  consumer warpgroup 1: rows 64..127             } epilogue from registers (bias / GELU / residual / split)
+// The producer runs ahead through the ring while a warpgroup is in its epilogue.
+//
+// CLUSTER = 2 ("pair" tiles, 256 x 256 per cluster): the two CTAs of a cluster take the two 128-row halves of the tile
+// and share its W tile -- each loads one 128-row half of W and TMA-multicasts it into both shared memories, which
+// halves the W traffic from L2.  A ring slot is then released by the consumers of BOTH CTAs.
 #include <stdlib.h>
 
 #include "gemm_common.cuh"
@@ -25,7 +26,7 @@
 namespace pips {
 
 constexpr int BM = 128;
-constexpr int GEMM_THREADS = 384;                 // 4 control warps + 8 epilogue warps
+constexpr int GEMM_THREADS = 384;                 // producer warpgroup + 2 consumer warpgroups
 constexpr uint32_t A_TILE_BYTES = BM * BK * 2;     // 16 KB
 
 template <int TERMS, int BN>
@@ -33,39 +34,35 @@ struct GemmCfg {
     static constexpr uint32_t kWTileBytes = BN * BK * 2;                  // 32 / 16 / 8 KB
     static constexpr int kOperandCopies = TERMS == 3 ? 2 : 1;             // hi (+ lo)
     static constexpr uint32_t kStageBytes = kOperandCopies * (A_TILE_BYTES + kWTileBytes);
-    static constexpr uint32_t kFixedBytes = EPI_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+    static constexpr uint32_t kFixedBytes = 1024 /*align*/ + 256 /*barriers*/;
     static constexpr int kFit = static_cast<int>((227u * 1024u - kFixedBytes) / kStageBytes);
     static constexpr int kStages = kFit > 8 ? 8 : kFit;                   // x3: 2 / 3 / 4 for BN = 256 / 128 / 64
-    static constexpr uint32_t kSmemBytes = kStages * kStageBytes + EPI_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+    static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kFixedBytes;
 };
 
-template <int TERMS, int BN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-               const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-               const GemmArgs args) {
+template <int TERMS, int BN, int CLUSTER>
+__device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const CUtensorMap& map_a_lo, const CUtensorMap& map_w_hi,
+                                             const CUtensorMap& map_w_lo, const GemmArgs& args) {
     using Cfg = GemmCfg<TERMS, BN>;
     constexpr int kStages = Cfg::kStages;
     constexpr uint32_t W_TILE_BYTES = Cfg::kWTileBytes;
+    static_assert(CLUSTER == 1 || BN == 256, "cluster tiles are 256 columns wide");
     extern __shared__ uint8_t smem_raw[];
     // 128B swizzle atoms need 1024-byte alignment
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint8_t* epi_stage = smem + kStages * Cfg::kStageBytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + EPI_STAGE_BYTES);
-    // barrier layout: full[kStages], empty[kStages], tmem_full[2], tmem_empty[2]
-    const uint32_t full0 = smem_u32(bars);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
+    const uint32_t full0 = smem_u32(bars);                  // full[kStages], empty[kStages]
     const uint32_t empty0 = full0 + 8 * kStages;
-    const uint32_t tfull0 = empty0 + 8 * kStages;
-    const uint32_t tempty0 = tfull0 + 16;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
+    const uint32_t rank = CLUSTER == 2 ? cluster_ctarank() : 0;
+    const int worker = blockIdx.x / CLUSTER, num_workers = gridDim.x / CLUSTER;     // a CTA, or a cluster of two
     pdl_trigger();
 
-    const int tiles_m = (args.M + BM - 1) / BM;
+    constexpr int TM = BM * CLUSTER;
     const int tiles_n = (args.N + BN - 1) / BN;
-    const int num_tiles = tiles_m * tiles_n;
+    const int num_tiles = ((args.M + TM - 1) / TM) * tiles_n;
     const int num_kb = args.K / BK;
 
     if (warp == 0 && lane == 0) {
@@ -79,33 +76,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < kStages; ++s) {
             mbar_init(full0 + 8 * s, 1);
-            mbar_init(empty0 + 8 * s, 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(tfull0 + 8 * s, 1);
-            mbar_init(tempty0 + 8 * s, GEMM_THREADS - 128);
+            mbar_init(empty0 + 8 * s, 2 * CLUSTER);         // one arrival per consumer warpgroup that reads the slot's W
         }
         fence_barrier_init();
     }
-    if (warp == 2) {
-        tmem_alloc(smem_u32(tmem_slot), 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    if (CLUSTER == 2) cluster_sync_all();                   // the peer's barriers exist before anything is sent to them
+    else __syncthreads();
     pdl_wait();                                             // operands and the residual stream come from the previous kernel
 
-    // Register budget per warpgroup: the control warps (0-3) need few, the epilogue warpgroups (4-7, 8-11) many.
+    // Register budget per warpgroup: the producer warpgroup needs few, the consumers hold the accumulator.
     if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
-    if (warp == 0) {
-        // ------------------------------------------------------------ TMA producer
-        if (lane == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == 0 && lane == 0) {
+            // ------------------------------------------------------------ TMA producer
             uint32_t stage = 0, phase = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                const int m0 = (t / tiles_n) * BM;
+            for (int t = worker; t < num_tiles; t += num_workers) {
+                const int m0 = (t / tiles_n) * TM + static_cast<int>(rank) * BM;
                 const int n0 = (t % tiles_n) * BN;
                 for (int kb = 0; kb < num_kb; ++kb) {
                     mbar_wait(empty0 + 8 * stage, phase ^ 1);
@@ -114,100 +100,87 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
                     const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
                     const int k0 = kb * BK;
                     tma_load_2d(base, &map_a_hi, fb, k0, m0);
-                    tma_load_2d(base + A_TILE_BYTES, &map_w_hi, fb, k0, n0);
-                    if (TERMS == 3) {
-                        tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES, &map_a_lo, fb, k0, m0);
-                        tma_load_2d(base + 2 * A_TILE_BYTES + W_TILE_BYTES, &map_w_lo, fb, k0, n0);
+                    if (TERMS == 3) tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES, &map_a_lo, fb, k0, m0);
+                    if (CLUSTER == 2) {
+                        // this CTA's half of the W tile (box = 128 rows), into both CTAs
+                        const uint32_t half = rank * (W_TILE_BYTES / 2);
+                        tma_load_2d_multicast(base + A_TILE_BYTES + half, &map_w_hi, fb, k0, n0 + static_cast<int>(rank) * (BN / 2), 3);
+                        if (TERMS == 3)
+                            tma_load_2d_multicast(base + 2 * A_TILE_BYTES + W_TILE_BYTES + half, &map_w_lo, fb, k0,
+                                                  n0 + static_cast<int>(rank) * (BN / 2), 3);
+                    } else {
+                        tma_load_2d(base + A_TILE_BYTES, &map_w_hi, fb, k0, n0);
+                        if (TERMS == 3) tma_load_2d(base + 2 * A_TILE_BYTES + W_TILE_BYTES, &map_w_lo, fb, k0, n0);
                     }
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
                 }
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ------------------------------------------------------------ MMA issuer
-        // whole warp, warp-uniform control flow (descriptors stay in uniform registers); one elected lane issues
-        {
-            const bool elected = elect_one();
-            constexpr uint32_t idesc = umma_idesc_bf16(BM, BN);
-            uint32_t stage = 0, phase = 0;
-            int it = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-                const uint32_t as = it & 1, aphase = (it >> 1) & 1;
-                mbar_wait(tempty0 + 8 * as, aphase ^ 1);      // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + as * BN;
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait(full0 + 8 * stage, phase);
-                    tc_fence_after();
-                    const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
-                    const uint64_t a_hi = umma_desc_sw128(base);
-                    const uint64_t w_hi = umma_desc_sw128(base + A_TILE_BYTES);
-                    const uint64_t a_lo = umma_desc_sw128(base + A_TILE_BYTES + W_TILE_BYTES);
-                    const uint64_t w_lo = umma_desc_sw128(base + 2 * A_TILE_BYTES + W_TILE_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {
-                        const uint64_t adv = static_cast<uint64_t>((k * UMMA_K * 2) >> 4);   // 32 B per K=16 step
-                        if (elected) umma_f16(d_tmem, a_hi + adv, w_hi + adv, idesc, (kb | k) != 0);
-                        if (TERMS == 3) {
-                            if (elected) umma_f16(d_tmem, a_lo + adv, w_hi + adv, idesc, 1);
-                            if (elected) umma_f16(d_tmem, a_hi + adv, w_lo + adv, idesc, 1);
-                        }
-                    }
-                    if (elected) umma_commit(empty0 + 8 * stage);          // smem slot reusable once these MMAs retire
-                    if (elected && kb == num_kb - 1) umma_commit(tfull0 + 8 * as);
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-        __syncwarp();
-    }
     } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-        // ------------------------------------------------------------ epilogue (256 threads)
-        // Two warps per TMEM lane quadrant (a warp may only touch lanes 32*(warp%4)..+31); each takes half
-        // of the tile's 256 columns.  Thread = one output row; tcgen05.ld of the next 32-column chunk is
-        // in flight while the current one goes through bias / GELU / split / store.
-        const int q = warp & 3;
-        const int half = (warp - 4) >> 2;
-        uint8_t* my_stage = epi_stage + (warp - 4) * 4096;
-        int it = 0;
-        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-            const uint32_t as = it & 1, aphase = (it >> 1) & 1;
-            const int m0 = (t / tiles_n) * BM;
-            const int n0 = (t % tiles_n) * BN + half * (BN / 2);
-            const int row0 = m0 + q * 32;
-            mbar_wait(tfull0 + 8 * as, aphase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + as * BN + half * (BN / 2) + (static_cast<uint32_t>(q * 32) << 16);
-
-            uint32_t va[32], vb[32];
-            float bias[32];
-            tmem_ld_32x32(taddr, va);
-            load_bias_chunk(args, n0, bias);
-            constexpr int NCH = BN / 64;                         // 32-column chunks per half tile: 4 / 2 / 1
-#pragma unroll 1
-            for (int c = 0; c < NCH; c += 2) {
-                const int c0 = c * 32;
-                tmem_ld_wait();
-                if (c + 1 < NCH) tmem_ld_32x32(taddr + c0 + 32, vb);
-                epilogue_chunk(args, va, bias, row0, n0 + c0, c + 1 < NCH ? n0 + c0 + 32 : -1, my_stage);
-                __syncwarp();                                    // tcgen05.ld / wait are warp-collective
-                if (c + 1 < NCH) {
-                    tmem_ld_wait();
-                    if (c + 2 < NCH) tmem_ld_32x32(taddr + c0 + 64, va);
-                    epilogue_chunk(args, vb, bias, row0, n0 + c0 + 32, c + 2 < NCH ? n0 + c0 + 64 : -1, my_stage);
-                    __syncwarp();
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        // ------------------------------------------------------------ consumers: MMA + epilogue, 64 rows each
+        const int wg = (warp - 4) >> 2;
+        const bool releaser = (threadIdx.x & 127) == 0;
+        float acc[BN / 2];
+        uint32_t stage = 0, phase = 0;
+        for (int t = worker; t < num_tiles; t += num_workers) {
+            const int m0 = (t / tiles_n) * TM + static_cast<int>(rank) * BM;
+            const int n0 = (t % tiles_n) * BN;
+            int prev = -1;                                   // ring slot whose MMAs are still in flight
+            for (int kb = 0; kb < num_kb; ++kb) {
+                mbar_wait(full0 + 8 * stage, phase);
+                const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
+                const uint64_t a_hi = wgmma_desc_sw128(base + wg * (A_TILE_BYTES / 2));
+                const uint64_t w_hi = wgmma_desc_sw128(base + A_TILE_BYTES);
+                const uint64_t a_lo = wgmma_desc_sw128(base + A_TILE_BYTES + W_TILE_BYTES + wg * (A_TILE_BYTES / 2));
+                const uint64_t w_lo = wgmma_desc_sw128(base + 2 * A_TILE_BYTES + W_TILE_BYTES);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {
+                    const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);   // 32 B per K=16 step
+                    wgmma_tile<BN>(acc, a_hi + adv, w_hi + adv, (kb | k) != 0);
+                    if (TERMS == 3) {
+                        wgmma_tile<BN>(acc, a_lo + adv, w_hi + adv, 1);
+                        wgmma_tile<BN>(acc, a_hi + adv, w_lo + adv, 1);
+                    }
                 }
+                wgmma_commit();
+                if (prev >= 0) {
+                    wgmma_wait<1>();                         // the previous slot's MMAs have retired: slot reusable
+                    if (releaser) {
+                        mbar_arrive(empty0 + 8 * prev);
+                        if (CLUSTER == 2) mbar_arrive_cluster(empty0 + 8 * prev, rank ^ 1);
+                    }
+                }
+                prev = static_cast<int>(stage);
+                if (++stage == kStages) { stage = 0; phase ^= 1; }
             }
-            tc_fence_before();
-            mbar_arrive(tempty0 + 8 * as);
+            wgmma_wait<0>();
+            wgmma_acc_ready(acc);
+            if (releaser) {
+                mbar_arrive(empty0 + 8 * prev);
+                if (CLUSTER == 2) mbar_arrive_cluster(empty0 + 8 * prev, rank ^ 1);
+            }
+            epilogue_frag<BN>(args, acc, m0 + wg * 64, n0);
         }
     }
+    if (CLUSTER == 2) cluster_sync_all();                   // nobody leaves while the peer may still signal or write to us
+}
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 512);
+template <int TERMS, int BN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+               const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
+               const GemmArgs args) {
+    gemm_tc_body<TERMS, BN, 1>(map_a_hi, map_a_lo, map_w_hi, map_w_lo, args);
+}
+
+template <int TERMS>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
+gemm_tc_pair_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+                    const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
+                    const GemmArgs args) {
+    gemm_tc_body<TERMS, 256, 2>(map_a_hi, map_a_lo, map_w_hi, map_w_lo, args);
 }
 
 // ---------------------------------------------------------------------------------- host side
@@ -222,9 +195,6 @@ static bool make_operand_map(CUtensorMap* map, const void* ptr, int rows, int K,
                         CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-int gemm_tc_pair_dispatch(const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo, int ldw,
-                          int w_rows, const GemmArgs& args, cudaStream_t st);       // gemm_tc2.cu
-
 // 0: automatic, 1: pair kernel, 64/128/256: single-CTA kernel with that tile width
 static int forced_tile() {
     const char* e = getenv("PIPS_B200_GEMM_TILE");
@@ -236,6 +206,9 @@ static int forced_tile() {
 
 int launch_single(int bn, bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo,
                   int ldw, int w_rows, const GemmArgs& args, cudaStream_t st);
+
+int launch_pair(bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo, int ldw,
+                int w_rows, const GemmArgs& args, cudaStream_t st);
 
 static bool use_pair_kernel() {
     static int v = -1;
@@ -276,7 +249,7 @@ extern "C" int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_r
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // Tile shape.  Every variant accumulates each output element over K in the same order (same MMA K-steps, same
     // hi/lo term order), so the choice changes the schedule, not the bits (tests/test_kernels_gpu.py).
-    //   pair  256x256 per CTA pair (cta_group::2): least operand traffic; needs enough pair tiles to fill the GPU
+    //   pair  256x256 per cluster of two CTAs (W multicast): least operand traffic; needs enough pair tiles to fill the GPU
     //   128 x {256,128,64} single CTA: when 256-wide tiles would leave most SMs idle (few particles)
     const int force = forced_tile();                  // PIPS_B200_GEMM_TILE = pair | 256 | 128 | 64 (tests, profiling)
     const bool pair_ok = use_pair_kernel() && M > 128 && (a_rows % 256) == 0 && (w_rows % 256) == 0;
@@ -292,7 +265,7 @@ extern "C" int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_r
     else if (force > 1) { pair = false; bn = force; }
     if ((w_rows % bn) != 0) { bn = 256; pair = pair && pair_ok; }   // TMA boxes must stay inside the weight allocation
     if (pair)
-        return gemm_tc_pair_dispatch(a_hi, x3 ? a_lo : nullptr, lda, a_rows, w_hi, x3 ? w_lo : nullptr, ldw, w_rows, args, st);
+        return launch_pair(x3, a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, args, st);
     return launch_single(bn, x3, a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, args, st);
 }
 
@@ -312,6 +285,38 @@ static int launch_variant(const CUtensorMap& ma_hi, const CUtensorMap& ma_lo, co
     cudaError_t e = launch_pdl(gemm_tc_kernel<TERMS, BN>, dim3(grid), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, ma_hi, ma_lo, mw_hi, mw_lo, args);
     if (e == cudaSuccess) e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail_cuda("pips_gemm_tc: launch", e);
+}
+
+template <int TERMS>
+static int launch_pair_variant(const CUtensorMap& ma_hi, const CUtensorMap& ma_lo, const CUtensorMap& mw_hi, const CUtensorMap& mw_lo,
+                               const GemmArgs& args, cudaStream_t st) {
+    using Cfg = GemmCfg<TERMS, 256>;
+    static bool attr[kMaxDevices] = {};
+    {
+        cudaError_t e = ensure_dyn_smem(gemm_tc_pair_kernel<TERMS>, attr, Cfg::kSmemBytes);
+        if (e != cudaSuccess) return fail_cuda("pips_gemm_tc (pair): smem attribute", e);
+    }
+    const int tiles = ((args.M + 255) / 256) * ((args.N + 255) / 256);
+    const int max_pairs = sm_count() / 2;
+    const int pairs = tiles < max_pairs ? tiles : max_pairs;
+    cudaError_t e = launch_pdl(gemm_tc_pair_kernel<TERMS>, dim3(2 * pairs), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, ma_hi, ma_lo, mw_hi,
+                               mw_lo, args);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail_cuda("pips_gemm_tc (pair): launch", e);
+}
+
+int launch_pair(bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo, int ldw,
+                int w_rows, const GemmArgs& args, cudaStream_t st) {
+    CUtensorMap ma_hi, ma_lo, mw_hi, mw_lo;                  // every box is 128 rows: a CTA's rows of A, its half of the W tile
+    if (!make_operand_map(&ma_hi, a_hi, a_rows, args.K, lda, BM)) return fail("pips_gemm_tc (pair): tensor map (A hi) failed");
+    if (!make_operand_map(&mw_hi, w_hi, w_rows, args.K, ldw, 128)) return fail("pips_gemm_tc (pair): tensor map (W hi) failed");
+    ma_lo = ma_hi;
+    mw_lo = mw_hi;
+    if (x3) {
+        if (!make_operand_map(&ma_lo, a_lo, a_rows, args.K, lda, BM)) return fail("pips_gemm_tc (pair): tensor map (A lo) failed");
+        if (!make_operand_map(&mw_lo, w_lo, w_rows, args.K, ldw, 128)) return fail("pips_gemm_tc (pair): tensor map (W lo) failed");
+    }
+    return x3 ? launch_pair_variant<3>(ma_hi, ma_lo, mw_hi, mw_lo, args, st) : launch_pair_variant<1>(ma_hi, ma_lo, mw_hi, mw_lo, args, st);
 }
 
 int launch_single(int bn, bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo,

@@ -1,5 +1,5 @@
 // CUDA-core parts of the DeltaBlock mixer and the state update:
-//   pips_gemm_f32   exact fp32 dense layer (PIPS_PREC_F32; also the on-device cross-check of the tcgen05 path)
+//   pips_gemm_f32   exact fp32 dense layer (PIPS_PREC_F32; also the on-device cross-check of the wgmma path)
 //   pips_tokenmix   LN -> token-mixing MLP over the S=8 frames -> +x -> LN   (K = 8/32: not a tensor-core shape)
 //   pips_ln_pool    final LN + mean over S
 //   pips_update     GroupNorm/Linear/GELU feature update + coord update + frame-0 lock
@@ -308,7 +308,7 @@ extern "C" int pips_tokenmix(float* x, int seqs, const float* ln1_w, const float
     if (seqs <= 0) return fail("pips_tokenmix: no sequences");
     if (!y_hi && !y_f32) return fail("pips_tokenmix: no output buffer");
     {
-        // bf16 / bf16x3 precisions run the tensor-core kernel (tokenmix_tc.cu: both contractions as tcgen05 MMAs, software-
+        // bf16 / bf16x3 precisions run the tensor-core kernel (tokenmix_tc.cu: both contractions as wgmma MMAs,
         // pipelined over the four channel tiles, 4 CTAs per SM); PIPS_B200_TOKENMIX=simt keeps the CUDA-core kernel below,
         // which is also the fp32-precision path.
         static int use_tc = -1;

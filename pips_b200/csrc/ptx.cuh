@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM).
+// Thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor, with cluster multicast), warpgroup MMA (wgmma), clusters.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -70,64 +70,7 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* map, uint3
         : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16/fp16 inputs with fp32 accumulate.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Arrives on `bar` once every MMA previously issued by this thread has completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets row (lane base + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-
-// K-major, 128-byte-swizzled operand tile (rows of 64 bf16 = 128 B, 8-row groups 1024 B apart):
-// the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B and a {64, rows} box.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);      // start address, 16 B units
-    d |= static_cast<uint64_t>(0) << 16;                          // leading byte offset (unused: one swizzle atom along K)
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;                  // stride byte offset between 8-row groups
-    d |= static_cast<uint64_t>(1) << 46;                          // descriptor version (sm_100)
-    d |= static_cast<uint64_t>(2) << 61;                          // SWIZZLE_128B
-    return d;
-}
-// bf16 x bf16 -> fp32, both operands K-major.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// ---------------------------------------------------------------- CTA pairs (cluster of 2, cta_group::2)
+// ---------------------------------------------------------------- clusters
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -136,9 +79,7 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
 }
-// address of the same smem offset in the leader (rank 0) CTA of the pair, as a shared::cluster address
-__device__ __forceinline__ uint32_t leader_addr(uint32_t local) { return local & 0xFEFFFFFFu; }
-
+// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t local_bar, uint32_t cta) {
     asm volatile(
         "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
@@ -146,40 +87,99 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t local_bar, uint32_t
         ::"r"(local_bar), "r"(cta)
         : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const void* map, uint32_t leader_bar, int c0, int c1) {
+// one load, written to the same offset (and signalled on the same barrier offset) in every CTA of `cta_mask`
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const void* map, uint32_t bar, int c0, int c1, uint16_t cta_mask) {
     asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1)
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
 }
-__device__ __forceinline__ void tma_load_4d_pair(uint32_t dst, const void* map, uint32_t leader_bar, int c0, int c1, int c2, int c3) {
+
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, accumulators in registers)
+// D[64 x N, registers of the 128 threads of a warpgroup] (+)= A[64 x 16, smem desc] * B[N x 16, smem desc]^T, bf16 inputs,
+// fp32 accumulation, both operands K-major.  Thread (warp w of the warpgroup, lane l) holds, for every 8-column block j,
+//   d[4j], d[4j+1]: row 16w + l/4,     columns 8j + 2(l%4), +1        d[4j+2], d[4j+3]: row 16w + l/4 + 8, same columns.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+// keeps the compiler from reading accumulator registers before the wgmma_wait that makes them valid
+template <int R>
+__device__ __forceinline__ void wgmma_acc_ready(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+#define PIPS_ACC4(d, i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define PIPS_ACC8(d, i) PIPS_ACC4(d, i), PIPS_ACC4(d, i + 4)
+#define PIPS_ACC16(d, i) PIPS_ACC8(d, i), PIPS_ACC8(d, i + 8)
+#define PIPS_ACC32(d, i) PIPS_ACC16(d, i), PIPS_ACC16(d, i + 16)
+#define PIPS_ACC64(d, i) PIPS_ACC32(d, i), PIPS_ACC32(d, i + 32)
+
+__device__ __forceinline__ void wgmma_n8(float (&d)[4], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3}, "
+        "%4, %5, p, 1, 1, 0, 0;\n\t}"
+        : PIPS_ACC4(d, 0)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
         : "memory");
 }
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, 0, 0;\n\t}"
+        : PIPS_ACC16(d, 0)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
         : "memory");
 }
-// arrive (once all previously issued MMAs are done) on the barrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-        ::"r"(bar), "h"(static_cast<uint16_t>(3))
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t}"
+        : PIPS_ACC32(d, 0)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
         : "memory");
+}
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : PIPS_ACC64(d, 0)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
+
+// 64 x BN tile: BN = 256 as two N = 128 instructions on the two 128-row halves of the B tile (128-byte rows)
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    if constexpr (BN == 64) {
+        wgmma_n64(d, a_desc, b_desc, accumulate);
+    } else if constexpr (BN == 128) {
+        wgmma_n128(d, a_desc, b_desc, accumulate);
+    } else {
+        static_assert(BN == 256, "tile widths: 64, 128, 256");
+        wgmma_n128(*reinterpret_cast<float(*)[64]>(&d[0]), a_desc, b_desc, accumulate);
+        wgmma_n128(*reinterpret_cast<float(*)[64]>(&d[64]), a_desc, b_desc + ((128 * 128) >> 4), accumulate);
+    }
+}
+
+// K-major, 128-byte-swizzled operand tile (rows of 64 bf16 = 128 B, 8-row groups 1024 B apart):
+// the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B and a {64, rows} box.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);      // start address, 16 B units
+    d |= static_cast<uint64_t>(1) << 16;                          // leading byte offset (unused: one swizzle atom along K)
+    d |= static_cast<uint64_t>(1024 >> 4) << 32;                  // stride byte offset between 8-row groups
+    d |= static_cast<uint64_t>(1) << 62;                          // SWIZZLE_128B
+    return d;
 }
 
 }  // namespace pips

@@ -117,7 +117,7 @@ static int pyramid_common(const float* fmaps, bool nhwc, int frames, int H, int 
         }
         if (lvl_bf16) {
             size_t blocks = (n / 4 + 255) / 256;
-            if (blocks > 148 * 8) blocks = 148 * 8;
+            if (blocks > sm_count() * 8) blocks = sm_count() * 8;
             f32_to_bf16_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(fmaps, static_cast<__nv_bfloat16*>(lvl_bf16[0]), n / 4);
         }
     } else {
@@ -131,7 +131,7 @@ static int pyramid_common(const float* fmaps, bool nhwc, int frames, int H, int 
         const int ho = hi / 2, wo = wi / 2;
         const size_t total = static_cast<size_t>(frames) * ho * wo * 32;
         size_t blocks = (total + 255) / 256;
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > sm_count() * 8) blocks = sm_count() * 8;
         avgpool2_nhwc_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(
             lvl_f32[l - 1], lvl_f32[l], lvl_bf16 ? static_cast<__nv_bfloat16*>(lvl_bf16[l]) : nullptr, frames, hi, wi, ho, wo);
         e = cudaGetLastError();

@@ -5,22 +5,16 @@
 //   x += z;  out = LN2(x)                                                    (nets/pips.py:117, :93-109, :100)
 //
 // K = 8 and K = 32 are far too small for a conventional tensor-core GEMM, but with the CHANNELS as the MMA's M
-// dimension each track is four M = 128 tiles and the per-channel MLP becomes
+// dimension each track is four 128-row tiles (two wgmma M = 64 blocks each) and the per-channel MLP becomes
 //   GEMM1  H (128 x 32) = A1 (128 x 16) . B^T      A1 row c = [y_hi[0..8) | y_lo[0..8)]   (bf16, K-major, no swizzle)
-//   GEMM2  Z (128 x 16) = G  (128 x 64) . B^T      G  row c = [g_hi[0..32) | g_lo[0..32)]
+//   GEMM2  Z (128 x 8)  = G  (128 x 64) . B^T      G  row c = [g_hi[0..32) | g_lo[0..32)]
 // where the bf16x3 split is folded into K: B = [w_hi | w_hi] gives hi*hi + lo*hi in one MMA and B' = [w_lo | 0]
-// adds hi*lo.  8 tcgen05.mma per tile replace 512 FMAs per channel; LayerNorm, GELU, the hi/lo splits and all
-// global traffic stay on the CUDA cores (thread t owns channels 4t..4t+3 == lane t of tile 0..3, so loads and
-// stores are 16-byte vectors).  One CTA = 128 threads = the 128 TMEM lanes.
-//
-// Round 2 (this version): the round-1 kernel ran one track at a time per CTA with every MMA round trip exposed and
-// only 2 CTAs per SM (87 KB of smem, 256 TMEM columns): 0.147 ms per launch at 4096 tracks, slower than the CUDA-core
-// kernel (0.117 ms).  Now
-//   * the G operand is double-buffered per TILE (2 x 16 KB instead of 4 x 16 KB) and Z_i overwrites the TMEM columns
-//     of H_i (consumed by then): 55 KB of smem and 128 TMEM columns per CTA -> 4 CTAs (16 warps) per SM;
-//   * the second contraction is software-pipelined over the four tiles: GELU(H_{i+1}) runs on the CUDA cores while
-//     the tensor cores execute GEMM2 of tile i (one mbarrier per G buffer);
-//   * the 8-row LayerNorm statistics use a transposing butterfly (9 shuffles per reduction instead of 40).
+// adds hi*lo.  A handful of wgmma per tile replace 512 FMAs per channel; LayerNorm, GELU, the hi/lo splits and all
+// global traffic stay on the CUDA cores (thread t owns channels 4t..4t+3 == row t of tile 0..3, so loads and
+// stores are 16-byte vectors).  One CTA = 128 threads = one warpgroup; accumulators are wgmma register fragments:
+// GELU is applied on the H fragment and written to the G operand in shared memory, GEMM2 of tile i runs while GEMM1
+// of tile i+1 is issued, and the Z fragments return to the thread-per-row layout through shared memory (in G's place).
+// 55 KB of shared memory per CTA -> 4 CTAs (16 warps) per SM.
 #include "mixer_common.cuh"
 #include "ptx.cuh"
 
@@ -28,36 +22,29 @@ namespace pips {
 
 constexpr int TT_THREADS = 128;
 constexpr int TT_CTAS_PER_SM = 4;
-constexpr uint32_t TT_TMEM_COLS = 128;               // H_i: columns [32 i, 32 i + 32); Z_i overwrites [32 i, 32 i + 16)
 constexpr uint32_t TT_A1_TILE = 128 * 32;            // 4 KB: 128 rows x K=16 bf16
-constexpr uint32_t TT_G_TILE = 128 * 128;            // 16 KB: 128 rows x K=64 bf16
+constexpr uint32_t TT_G_TILE = 128 * 128;            // 16 KB: 128 rows x K=64 bf16; later Z: 4 tiles x 128 rows x 8 fp32
 constexpr uint32_t TT_OFF_A1 = 0;
-constexpr uint32_t TT_OFF_G = TT_OFF_A1 + 4 * TT_A1_TILE;          // two G buffers (tiles i and i+1 in flight)
-constexpr uint32_t TT_OFF_B1A = TT_OFF_G + 2 * TT_G_TILE;          // [w1_hi | w1_hi]  32 rows x 32 B
+constexpr uint32_t TT_OFF_X = TT_OFF_A1 + 4 * TT_A1_TILE;          // copy of the track's x for the residual (8 x 2 KB)
+constexpr uint32_t TT_OFF_G = TT_OFF_X + 8 * 2048;
+constexpr uint32_t TT_OFF_B1A = TT_OFF_G + TT_G_TILE;              // [w1_hi | w1_hi]  32 rows x 32 B
 constexpr uint32_t TT_OFF_B1B = TT_OFF_B1A + 1024;                 // [w1_lo | 0]
-constexpr uint32_t TT_OFF_B2A = TT_OFF_B1B + 1024;                 // [w2_hi | w2_hi]  16 rows x 128 B
-constexpr uint32_t TT_OFF_B2B = TT_OFF_B2A + 2048;                 // [w2_lo | 0]
-constexpr uint32_t TT_OFF_MISC = TT_OFF_B2B + 2048;                // barriers, tmem slot, reductions, biases
-constexpr uint32_t TT_SMEM = TT_OFF_MISC + 512 + 128;              // + alignment slack; 4 CTAs: 4 x (55.9 + 1) KB <= 228 KB
+constexpr uint32_t TT_OFF_B2A = TT_OFF_B1B + 1024;                 // [w2_hi | w2_hi]  8 rows x 128 B
+constexpr uint32_t TT_OFF_B2B = TT_OFF_B2A + 1024;                 // [w2_lo | 0]
+constexpr uint32_t TT_OFF_MISC = TT_OFF_B2B + 1024;                // reductions, biases
+constexpr uint32_t TT_SMEM = TT_OFF_MISC + 512 + 128;              // + alignment slack; 4 CTAs: 4 x (52.6 + 1) KB <= 227 KB
 
 // K-major operand without swizzle: 8-row x 16-byte core matrices; element (r, k) lives at
 // (r / 8) * sbo + (k / 8) * 128 + (r % 8) * 16 + (k % 8) * 2.
-__device__ __forceinline__ uint64_t umma_desc_nosw(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t wgmma_desc_nosw(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
     d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;       // between core matrices along K
-    d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;       // between 8-row groups
-    d |= static_cast<uint64_t>(1) << 46;                    // descriptor version (sm_100); layout type 0 = no swizzle
+    d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;       // between 8-row groups; layout type 0 = no swizzle
     return d;
 }
 __device__ __forceinline__ uint32_t core_off(int r, int kcore, uint32_t sbo) {
     return static_cast<uint32_t>(r >> 3) * sbo + static_cast<uint32_t>(kcore) * 128 + static_cast<uint32_t>(r & 7) * 16;
-}
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&v)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr)
-                 : "memory");
 }
 
 // ---- 8-row statistics with a transposing butterfly: every lane contributes 8 partial sums (one per frame); three
@@ -108,7 +95,7 @@ __device__ __forceinline__ void cta_rowsum8(float (&v)[8], float (*red)[8]) {
 }
 
 // two-pass LayerNorm over the 512 channels of the 8 rows held as x[s][0..3] (biased variance, eps 1e-5); the
-// per-element arithmetic runs on packed fp32 pairs (FADD2 / FMUL2 / FFMA2)
+// per-element arithmetic is written on fp32 pairs
 __device__ __forceinline__ void layernorm8_fast(const float (&x)[8][4], float (&y)[8][4], const float4 g, const float4 b, float (*red)[8]) {
     float m[8], q[8];
 #pragma unroll
@@ -137,13 +124,6 @@ __device__ __forceinline__ void layernorm8_fast(const float (&x)[8][4], float (&
     }
 }
 
-// elect.sync needs the whole warp converged: called at a point where all 128 threads arrive, evaluated in warp 0 only
-__device__ __forceinline__ bool elect_one_in_warp0(int warp) {
-    bool e = false;
-    if (warp == 0) e = elect_one();
-    return e;
-}
-
 __global__ void __launch_bounds__(TT_THREADS, TT_CTAS_PER_SM)
 tokenmix_tc_kernel(float* __restrict__ x, int seqs, const float* __restrict__ ln1_w, const float* __restrict__ ln1_b,
                    const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
@@ -153,17 +133,14 @@ tokenmix_tc_kernel(float* __restrict__ x, int seqs, const float* __restrict__ ln
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~static_cast<uintptr_t>(127));
     const uint32_t sbase = smem_u32(smem);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TT_OFF_MISC);
-    const uint32_t bar_h = smem_u32(bars);                  // GEMM1 of all four tiles done
-    const uint32_t bar_g0 = bar_h + 8;                      // GEMM2 that read G buffer b done (bar_g0 + 8 b)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
-    float (*red)[8] = reinterpret_cast<float (*)[8]>(smem + TT_OFF_MISC + 32);
-    float* s_b1 = reinterpret_cast<float*>(smem + TT_OFF_MISC + 32 + 128);
+    float (*red)[8] = reinterpret_cast<float (*)[8]>(smem + TT_OFF_MISC);
+    float* s_b1 = reinterpret_cast<float*>(smem + TT_OFF_MISC + 128);
     float* s_b2 = s_b1 + 32;
 
-    const int t = threadIdx.x, warp = t >> 5;
+    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+    const int frow = warp * 16 + (lane >> 2), fq = lane & 3;        // fragment row (+8, +64 m) and column pair of this thread
 
-    // ---- one-time setup: weight operands, barriers, TMEM
+    // ---- one-time setup: weight operands
     for (int i = t; i < 32 * 16; i += TT_THREADS) {                 // GEMM1 B operands: row j, k in [0,16)
         const int j = i >> 4, k = i & 15;
         __nv_bfloat16 h, l;
@@ -172,36 +149,19 @@ tokenmix_tc_kernel(float* __restrict__ x, int seqs, const float* __restrict__ ln
         *reinterpret_cast<__nv_bfloat16*>(smem + TT_OFF_B1A + off) = h;                                   // [hi | hi]
         *reinterpret_cast<__nv_bfloat16*>(smem + TT_OFF_B1B + off) = k < 8 ? l : __float2bfloat16_rn(0.f); // [lo | 0]
     }
-    for (int i = t; i < 16 * 64; i += TT_THREADS) {                 // GEMM2 B operands: row s' (8 real of 16), k in [0,64)
+    for (int i = t; i < 8 * 64; i += TT_THREADS) {                  // GEMM2 B operands: row s', k in [0,64)
         const int r = i >> 6, k = i & 63;
-        __nv_bfloat16 h = __float2bfloat16_rn(0.f), l = h;
-        if (r < 8) split_bf16(w2[r * 32 + (k & 31)], h, l);
+        __nv_bfloat16 h, l;
+        split_bf16(w2[r * 32 + (k & 31)], h, l);
         const uint32_t off = core_off(r, k >> 3, 1024) + (k & 7) * 2;
         *reinterpret_cast<__nv_bfloat16*>(smem + TT_OFF_B2A + off) = h;
         *reinterpret_cast<__nv_bfloat16*>(smem + TT_OFF_B2B + off) = k < 32 ? l : __float2bfloat16_rn(0.f);
     }
     if (t < 32) s_b1[t] = b1[t];
     if (t < 8) s_b2[t] = b2[t];
-    if (t == 0) {
-        mbar_init(bar_h, 1);
-        mbar_init(bar_g0, 1);
-        mbar_init(bar_g0 + 8, 1);
-        fence_barrier_init();
-    }
-    if (warp == 0) {
-        tmem_alloc(smem_u32(tmem_slot), TT_TMEM_COLS);
-        tmem_relinquish();
-    }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-    constexpr uint32_t idesc1 = umma_idesc_bf16(128, 32);
-    constexpr uint32_t idesc2 = umma_idesc_bf16(128, 16);
-    const uint64_t d_b1a = umma_desc_nosw(sbase + TT_OFF_B1A, 128, 256), d_b1b = umma_desc_nosw(sbase + TT_OFF_B1B, 128, 256);
-    const bool elected = warp == 0 && elect_one_in_warp0(warp);   // the lane of warp 0 that issues the MMAs
+    const uint64_t d_b1a = wgmma_desc_nosw(sbase + TT_OFF_B1A, 128, 256), d_b1b = wgmma_desc_nosw(sbase + TT_OFF_B1B, 128, 256);
 
     pdl_wait();                                             // x is written by the previous kernel (weights above are constants)
     // x of the track after the current one is fetched into registers while the current track's GELU phase runs; the
@@ -214,9 +174,18 @@ tokenmix_tc_kernel(float* __restrict__ x, int seqs, const float* __restrict__ ln
     }
     const float4 g1 = __ldg(reinterpret_cast<const float4*>(ln1_w + t * 4)), c1 = __ldg(reinterpret_cast<const float4*>(ln1_b + t * 4));
 
-    uint32_t parity = 0;                                    // of bar_h: one completion per track
-    for (int seq = blockIdx.x; seq < seqs; seq += gridDim.x, parity ^= 1) {
+    for (int seq = blockIdx.x; seq < seqs; seq += gridDim.x) {
         const size_t base = static_cast<size_t>(seq) * 8 * 512 + t * 4;
+        {
+            // a copy of this track's x for the residual at the end (cp.async, no registers held) -- re-reading it from L2
+            // there exposed ~500 cycles of latency per track
+            const uint32_t dst = sbase + TT_OFF_X + t * 16;
+            const float* src = x + base;
+#pragma unroll
+            for (int sr = 0; sr < 8; ++sr)
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + sr * 2048), "l"(src + sr * 512) : "memory");
+            asm volatile("cp.async.commit_group;" ::: "memory");
+        }
         {
             float xv[8][4], yv[8][4];
 #pragma unroll
@@ -224,7 +193,7 @@ tokenmix_tc_kernel(float* __restrict__ x, int seqs, const float* __restrict__ ln
             layernorm8_fast(xv, yv, g1, c1, red);
 
             // ---- A1: row t of tile i = [y_hi over the 8 frames | y_lo over the 8 frames] of channel 4t+i
-            // (the tensor cores finished reading the previous track's A1 long ago: its bar_h wait was passed)
+            // (the previous track's MMAs were waited for before its Z was read)
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 uint32_t hw[4], lw[4];
@@ -240,120 +209,106 @@ tokenmix_tc_kernel(float* __restrict__ x, int seqs, const float* __restrict__ ln
             }
         }
         fence_proxy_async_smem();
-        tc_fence_before();
         __syncthreads();
-        if (warp == 0) {                                     // warp-uniform: descriptors in uniform registers, one lane issues
-            tc_fence_after();
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const uint64_t a = umma_desc_nosw(sbase + TT_OFF_A1 + i * TT_A1_TILE, 128, 256);
-                if (elected) {
-                    umma_f16(tmem_base + i * 32, a, d_b1a, idesc1, 0);
-                    umma_f16(tmem_base + i * 32, a, d_b1b, idesc1, 1);
-                }
-            }
-            if (elected) umma_commit(bar_h);
-        }
         if (seq + static_cast<int>(gridDim.x) < seqs) {      // next track's x: in flight during the GELU phase
             const float* src = x + static_cast<size_t>(seq + gridDim.x) * 8 * 512 + t * 4;
 #pragma unroll
             for (int s = 0; s < 8; ++s) nx[s] = *reinterpret_cast<const float4*>(src + s * 512);
         }
-        mbar_wait(bar_h, parity);
-        tc_fence_after();
-        // GEMM1 is done with the A1 tiles: their 16 KB now take a copy of this track's x (cp.async, no registers held)
-        // for the residual at the end -- re-reading it from L2 there exposed ~500 cycles of latency per track
-        {
-            const uint32_t dst = sbase + TT_OFF_A1 + t * 16;
-            const float* src = x + base;
-#pragma unroll
-            for (int sr = 0; sr < 8; ++sr)
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + sr * 2048), "l"(src + sr * 512) : "memory");
-            asm volatile("cp.async.commit_group;" ::: "memory");
-        }
 
-        // ---- per tile: GELU(H_i) -> G buffer (i & 1) -> GEMM2_i (Z_i lands on H_i's first 16 columns) while the
-        // CUDA cores already work on H_{i+1}.  Each G-buffer barrier completes twice per track (parities 0, 1).
-#pragma unroll 1
+        // ---- per tile: GEMM1 -> GELU(H_i) on the fragment -> G -> GEMM2_i (asynchronous: it runs while GEMM1 of tile
+        // i+1 is issued; the wait after that GEMM1 also retires it, which frees G)
+        float z[4][2][4];
+#pragma unroll
         for (int i = 0; i < 4; ++i) {
-            uint32_t v[32];
-            tmem_ld_32x32(lane_addr + i * 32, v);
-            if (i >= 2) mbar_wait(bar_g0 + 8 * (i & 1), 0);  // GEMM2_{i-2} has finished reading this G buffer
-            tmem_ld_wait();
-            uint8_t* row = smem + TT_OFF_G + (i & 1) * TT_G_TILE;
+            float h[2][16];
+            wgmma_fence();
 #pragma unroll
-            for (int p = 0; p < 4; ++p) {
-                uint32_t hw[4], lw[4];
+            for (int m = 0; m < 2; ++m) {
+                const uint64_t a = wgmma_desc_nosw(sbase + TT_OFF_A1 + i * TT_A1_TILE + m * 2048, 128, 256);
+                wgmma_n32(h[m], a, d_b1a, 0);
+                wgmma_n32(h[m], a, d_b1b, 1);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_acc_ready(h[0]);
+            wgmma_acc_ready(h[1]);
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const int j = 8 * p + 2 * e;
-                    const float2 bj = *reinterpret_cast<const float2*>(s_b1 + j);
-                    const float2 g = gelu_fast2_abs(add2(make_float2(__uint_as_float(v[j]), __uint_as_float(v[j + 1])), bj));
-                    hw[e] = cvt_bf16x2(g.x, g.y);
-                    const float2 lo = fma2(make_float2(__uint_as_float(hw[e] << 16), __uint_as_float(hw[e] & 0xffff0000u)),
-                                           bcast2(-1.0f), g);
-                    lw[e] = cvt_bf16x2(lo.x, lo.y);
+            for (int m = 0; m < 2; ++m) {
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    uint8_t* row = smem + TT_OFF_G + core_off(64 * m + frow + 8 * hh, 0, 1024) + fq * 4;
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const float2 bj = *reinterpret_cast<const float2*>(s_b1 + 8 * j + 2 * fq);
+                        const float2 g = gelu_fast2_abs(add2(make_float2(h[m][4 * j + 2 * hh], h[m][4 * j + 2 * hh + 1]), bj));
+                        const uint32_t hw = cvt_bf16x2(g.x, g.y);
+                        const float2 lo = fma2(make_float2(__uint_as_float(hw << 16), __uint_as_float(hw & 0xffff0000u)), bcast2(-1.0f), g);
+                        *reinterpret_cast<uint32_t*>(row + j * 128) = hw;
+                        *reinterpret_cast<uint32_t*>(row + (j + 4) * 128) = cvt_bf16x2(lo.x, lo.y);
+                    }
                 }
-                *reinterpret_cast<uint4*>(row + core_off(t, p, 1024)) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                *reinterpret_cast<uint4*>(row + core_off(t, p + 4, 1024)) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
             }
             fence_proxy_async_smem();
-            tc_fence_before();                               // H_i fully read by this thread before Z_i may overwrite it
             __syncthreads();
-            if (warp == 0) {
-                tc_fence_after();
-                const uint32_t d = tmem_base + i * 32;
-                const uint32_t ga = sbase + TT_OFF_G + (i & 1) * TT_G_TILE;
+            wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {                    // [g_hi | g_lo] . [w2_hi | w2_hi]
-                    const uint64_t da = umma_desc_nosw(ga + k * 256, 128, 1024), db = umma_desc_nosw(sbase + TT_OFF_B2A + k * 256, 128, 1024);
-                    if (elected) umma_f16(d, da, db, idesc2, k != 0);
-                }
+            for (int m = 0; m < 2; ++m) {
+                const uint32_t ga = sbase + TT_OFF_G + m * 8192;
 #pragma unroll
-                for (int k = 0; k < 2; ++k) {                    // g_hi . w2_lo
-                    const uint64_t da = umma_desc_nosw(ga + k * 256, 128, 1024), db = umma_desc_nosw(sbase + TT_OFF_B2B + k * 256, 128, 1024);
-                    if (elected) umma_f16(d, da, db, idesc2, 1);
-                }
-                if (elected) umma_commit(bar_g0 + 8 * (i & 1));
+                for (int k = 0; k < 4; ++k)                      // [g_hi | g_lo] . [w2_hi | w2_hi]
+                    wgmma_n8(z[i][m], wgmma_desc_nosw(ga + k * 256, 128, 1024), wgmma_desc_nosw(sbase + TT_OFF_B2A + k * 256, 128, 1024), k != 0);
+#pragma unroll
+                for (int k = 0; k < 2; ++k)                      // g_hi . w2_lo
+                    wgmma_n8(z[i][m], wgmma_desc_nosw(ga + k * 256, 128, 1024), wgmma_desc_nosw(sbase + TT_OFF_B2B + k * 256, 128, 1024), 1);
             }
+            wgmma_commit();
         }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { wgmma_acc_ready(z[i][0]); wgmma_acc_ready(z[i][1]); }
+        __syncthreads();                                     // every warp's GEMM2 has read G: Z takes its place
+        {
+            float* zs = reinterpret_cast<float*>(smem + TT_OFF_G);         // [tile][row][frame]
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int m = 0; m < 2; ++m)
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh)
+                        *reinterpret_cast<float2*>(zs + (i * 128 + 64 * m + frow + 8 * hh) * 8 + 2 * fq) =
+                            make_float2(z[i][m][2 * hh], z[i][m][2 * hh + 1]);
+        }
+        __syncthreads();
         // ---- residual, LN2, outputs
         float xv[8][4];
         asm volatile("cp.async.wait_group 0;" ::: "memory");
 #pragma unroll
         for (int sr = 0; sr < 8; ++sr) {                     // this thread's own copies: no CTA-wide barrier needed
-            const float4 v = *reinterpret_cast<const float4*>(smem + TT_OFF_A1 + sr * 2048 + t * 16);
+            const float4 v = *reinterpret_cast<const float4*>(smem + TT_OFF_X + sr * 2048 + t * 16);
             xv[sr][0] = v.x; xv[sr][1] = v.y; xv[sr][2] = v.z; xv[sr][3] = v.w;
         }
-        mbar_wait(bar_g0, 1);                                // GEMM2 of tiles 2 and 3 (and therefore of all) done
-        mbar_wait(bar_g0 + 8, 1);
-        tc_fence_after();
         {
-            uint32_t z[4][8];
+            const float* zs = reinterpret_cast<const float*>(smem + TT_OFF_G);
 #pragma unroll
-            for (int i = 0; i < 4; ++i) tmem_ld_32x8(lane_addr + i * 32, z[i]);
-            tmem_ld_wait();
+            for (int i = 0; i < 4; ++i) {
+                const float4 z0 = *reinterpret_cast<const float4*>(zs + (i * 128 + t) * 8), z1 = *reinterpret_cast<const float4*>(zs + (i * 128 + t) * 8 + 4);
+                const float zz[8] = {z0.x, z0.y, z0.z, z0.w, z1.x, z1.y, z1.z, z1.w};
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int s = 0; s < 8; ++s) xv[s][i] += __uint_as_float(z[i][s]) + s_b2[s];
+                for (int s = 0; s < 8; ++s) xv[s][i] += zz[s] + s_b2[s];
+            }
         }
-        tc_fence_before();                                   // Z read before the next track's GEMM1 overwrites the columns
 #pragma unroll
         for (int s = 0; s < 8; ++s)
             *reinterpret_cast<float4*>(x + base + s * 512) = make_float4(xv[s][0], xv[s][1], xv[s][2], xv[s][3]);
         {
             float yv[8][4];
             const float4 g2 = __ldg(reinterpret_cast<const float4*>(ln2_w + t * 4)), c2 = __ldg(reinterpret_cast<const float4*>(ln2_b + t * 4));
-            layernorm8_fast(xv, yv, g2, c2, red);            // its __syncthreads also order the Z reads before the next GEMM1
+            layernorm8_fast(xv, yv, g2, c2, red);            // its __syncthreads also order the Z reads before the next track's G
 #pragma unroll
             for (int s = 0; s < 8; ++s) store_row4(yv[s], base + s * 512, y_hi, y_lo, nullptr);
         }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, TT_TMEM_COLS);
 }
 
 }  // namespace pips

@@ -122,7 +122,7 @@ def fnet_fast(enc: Encoder, x: torch.Tensor) -> torch.Tensor:
 
 
 # --------------------------------------------------------------------------------------------------------------
-# 'tc' path: every 3x3 / 1x1 convolution on the tcgen05 implicit-GEMM kernel (csrc/conv_tc.cu), bf16x3 operands
+# 'tc' path: every 3x3 / 1x1 convolution on the wgmma implicit-GEMM kernel (csrc/conv_tc.cu), bf16x3 operands
 # --------------------------------------------------------------------------------------------------------------
 
 def _pad64(c: int) -> int:
@@ -286,7 +286,7 @@ def adopt_filter(enc: Encoder, name: str, conv: torch.nn.Conv2d, hi: torch.Tenso
 
 def fnet_tc(enc: Encoder, rgb: torch.Tensor) -> torch.Tensor:
     """rgb (N,3,H,W) fp32 or bf16 with values 0..255 (NOT normalised) -> feature maps (N,H/stride,W/stride,128) NHWC.
-    The whole encoder on libpips_b200: the 7x7/2 stem as a 4x1 stride-1 tcgen05 convolution over the unfolded,
+    The whole encoder on libpips_b200: the 7x7/2 stem as a 4x1 stride-1 wgmma convolution over the unfolded,
     normalised image (pips_stem_pack: row pairs x 7 column taps x 3 colours per pixel), residual stages and head on pips_conv_tc, element-wise stages fused."""
     assert rgb.is_cuda and rgb.dtype in (torch.float32, torch.bfloat16)
     from .engine import nvtx_range

@@ -44,7 +44,7 @@ class PackedWeights:
     """Kernel-layout copies of the DeltaBlock / head parameters.
 
     Dense-layer weights are kept as nn.Linear stores them ((out, in) == N x K, K-major), split into a
-    bf16 (hi, lo) pair for the tcgen05 path; the first Linear's K is zero-padded 519 -> 576 and the
+    bf16 (hi, lo) pair for the wgmma path; the first Linear's K is zero-padded 519 -> 576 and the
     last Linear's N 1040 -> 1280 so that TMA boxes never leave the allocation.
 
     ``self.t`` holds every tensor under a stable name ("layer3.fc1_w_hi", "head_b", ...); the names are

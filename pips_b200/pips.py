@@ -3,15 +3,15 @@
 Same constructor, same ``forward(xys, rgbs, coords_init, feat_init, iters, trajs_g, vis_g, valids,
 sw, return_feat, is_train)`` signature and return tuples, same ``state_dict`` keys -- so ``demo.py``,
 ``chain_demo.py``, ``test_on_*.py`` and ``saverloader.load`` work unchanged -- but at inference the
-per-iteration refinement loop (nets/pips.py:459-559) runs in hand-written sm_100a CUDA
+per-iteration refinement loop (nets/pips.py:459-559) runs in hand-written sm_90a CUDA
 (libpips_b200.so) instead of ~150 eager torch ops per iteration, and the all-pairs correlation
 volume is never materialised.
 
 Extra, optional knobs (keyword-only; the reference signature is unchanged):
-  precision   'bf16x3' (default; tcgen05 with hi/lo-split bf16 operands, fp32-class accuracy, meets
+  precision   'bf16x3' (default; wgmma with hi/lo-split bf16 operands, fp32-class accuracy, meets
               the 1e-3 px parity target), 'bf16' (fast, ~1e-2 px), 'fp32' (CUDA-core GEMMs, exact)
   feat_dtype  'fp32' (default) or 'bf16' storage of the correlation pyramid
-  fnet_mode   'tc' (default; residual stages and head as tcgen05 implicit-GEMM convolutions with bf16x3
+  fnet_mode   'tc' (default; residual stages and head as wgmma implicit-GEMM convolutions with bf16x3
               operands, element-wise stages fused, channels-last), 'fast' (cuDNN TF32 tensor-core
               convolutions over hi/lo-split operands instead), 'x3' (the same cuDNN convolutions through
               eager torch ops) or 'plain' (strict fp32 cuDNN)
@@ -113,7 +113,7 @@ class Pips(nn.Module):
         self.shard_fnet = True                  # sharded runs also split the encoder's frames over the ranks
         self.fnet_mode = fnet_mode or os.environ.get("PIPS_B200_FNET", "tc")
         if self.fnet_mode not in ("tc", "fast", "x3", "plain"):
-            raise ValueError("fnet_mode must be 'tc' (tcgen05 implicit-GEMM convolutions, bf16x3), 'fast' (cuDNN 3xTF32 "
+            raise ValueError("fnet_mode must be 'tc' (wgmma implicit-GEMM convolutions, bf16x3), 'fast' (cuDNN 3xTF32 "
                              "convolutions, channels-last, fused element-wise kernels), 'x3' (3xTF32 convolutions through "
                              "eager torch ops) or 'plain' (strict fp32 cuDNN)")
 
@@ -127,9 +127,9 @@ class Pips(nn.Module):
         full copy of the feature pyramid; results are exchanged so each rank returns the full
         result.  Call after ``torch.distributed.init_process_group``.
         ``balance`` (default off; PIPS_B200_BALANCE=1 turns it on): after a few forwards the shares become proportional to
-        each GPU's measured speed (sharding._Balance).  Measured on 8 B200s (profiles/r02_diag_8gpu.txt): under the power
-        cap a GPU's speed drifts by +-3-5 % from step to step and WHICH GPU is slowest changes between runs, so a share
-        fixed from a few samples does not beat equal shares -- kept as an option for boxes with a persistently slow GPU.
+        each GPU's measured speed (sharding._Balance).  Under a power cap a GPU's speed drifts from step to step and WHICH
+        GPU is slowest can change between runs, so a share fixed from a few samples need not beat equal shares -- an
+        option for nodes with a persistently slow GPU (not measured on H100).
         Results do not depend on the shares (tracks are independent): bit-exact either way (tools/check_sharded.py)."""
         import torch.distributed as dist
         self._shard = (dist.get_rank(group), dist.get_world_size(group), group)
@@ -197,7 +197,7 @@ class Pips(nn.Module):
             # nets/pips.py:509 -> RuntimeError; recorded in tests/golden as edge/n0_error): same error type here
             raise RuntimeError("pips_b200.Pips: no particles (xys has N = 0); the reference raises here as well")
         if not rgbs.is_cuda:
-            raise RuntimeError("pips_b200.Pips: the inference path is CUDA-only (sm_100a); move the model and "
+            raise RuntimeError("pips_b200.Pips: the inference path is CUDA-only (sm_90a); move the model and "
                                "inputs to a CUDA device. There is no CPU fallback.")
         with torch.no_grad():
             if self._shard is not None and self._shard[1] > 1 and self.shard_fnet and self.fnet_mode == "tc":
@@ -215,7 +215,7 @@ class Pips(nn.Module):
         reference, without the all-pairs volume.  The reference's own consumers look at one particle
         (``fcps[0:1,:,:,0:1]``, nets/pips.py:572).  Also returns (coord_predictions, vis_e) of the same run."""
         if not rgbs.is_cuda:
-            raise RuntimeError("pips_b200.Pips.score_maps is CUDA-only (sm_100a)")
+            raise RuntimeError("pips_b200.Pips.score_maps is CUDA-only (sm_90a)")
         B, N, D = xys.shape
         assert (D == 2)
         S = rgbs.shape[1]

@@ -102,7 +102,7 @@ def shard_sizes(N: int, weights, quantum: int = 32):
 
 class _Balance:
     """Speed-weighted particle shards.  The GPUs of one box do not run at one clock under the power cap (1.47-1.78 GHz
-    seen on 8 B200s), and every forward ends in an exchange of results, so with equal shards the step time is the
+    seen on a multi-GPU node), and every forward ends in an exchange of results, so with equal shards the step time is the
     SLOWEST GPU's.  After ``warm`` sharded forwards each rank times ``measure`` refinement calls with CUDA events, the
     rates (particles per second) are exchanged once, and from then on rank r gets a share proportional to its rate."""
 

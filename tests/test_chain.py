@@ -1,5 +1,5 @@
 """Chained long-video tracking (chain_demo.py:40-83): threshold sweep logic on CPU, oracle vs the reference's
-recorded chain, and the batched CUDA implementation vs the same recording (B200)."""
+recorded chain, and the batched CUDA implementation vs the same recording (GPU)."""
 import os
 
 import numpy as np

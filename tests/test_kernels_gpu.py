@@ -1,4 +1,4 @@
-"""Per-kernel parity: every C-ABI entry point against the CPU oracle on seeded inputs (B200 only)."""
+"""Per-kernel parity: every C-ABI entry point against the CPU oracle on seeded inputs."""
 import math
 
 import pytest
@@ -186,10 +186,10 @@ def _split(t):
     (1000, 2048, 512, L.EPI_BIAS_GELU),    # FC1
     (1000, 512, 2048, L.EPI_BIAS_RESID),   # FC2
     (300, 1040, 512, L.EPI_BIAS),          # head: partial N tile
-    (40000, 512, 512, L.EPI_BIAS_RESID),   # > 148 tiles: persistent loop + TMEM double buffering
+    (40000, 512, 512, L.EPI_BIAS_RESID),   # more tiles than SMs: persistent loop
 ])
 def test_gemm_tc(terms, M, N, K, epi, pair, monkeypatch):
-    """pair=True: the cta_group::2 kernel (256x256 per CTA pair); False / 128 / 64: the single-CTA kernel with
+    """pair=True: the cluster kernel (256x256 per cluster of two CTAs, W multicast); False / 128 / 64: the single-CTA kernel with
     128 x 256 / 128 / 64 tiles.  The shape is forced -- left alone, pips_gemm_tc picks it from the problem size."""
     lib = L.load()
     torch.manual_seed(7)
@@ -234,9 +234,9 @@ def test_gemm_tc(terms, M, N, K, epi, pair, monkeypatch):
 @pytest.mark.parametrize("terms", [3, 1])
 @pytest.mark.parametrize("M,N,K,epi", [(1000, 2048, 512, L.EPI_BIAS_GELU), (2048, 512, 2048, L.EPI_BIAS_RESID),
                                        (300, 1040, 512, L.EPI_BIAS),
-                                       # partial last wave of the pair kernel -> its 256x128 tail tiles (74 pairs):
-                                       (33000, 512, 512, L.EPI_BIAS_RESID),       # 258 tiles = 3 waves + 36 -> 72 half tiles
-                                       (2400, 2048, 512, L.EPI_BIAS_GELU)])       # 80 tiles = 1 wave + 6 -> 12 half tiles
+                                       # partial last wave of the pair kernel (66 clusters on 132 SMs):
+                                       (33000, 512, 512, L.EPI_BIAS_RESID),       # 258 tiles = 3 waves + 60
+                                       (2400, 2048, 512, L.EPI_BIAS_GELU)])       # 80 tiles = 1 wave + 14
 def test_gemm_tile_shapes_are_bit_identical(terms, M, N, K, epi, monkeypatch):
     """Every tile shape accumulates an output element over K in the same order: the schedule that pips_gemm_tc picks
     from the problem size (pair / 256 / 128 / 64) must not change a single bit -- particle sharding and chunking,

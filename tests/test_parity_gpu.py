@@ -1,5 +1,5 @@
 """End-to-end parity of pips_b200.Pips.forward (CUDA) against the reference's recorded outputs
-(tests/golden) and the CPU oracle, through the public module API (B200 only)."""
+(tests/golden) and the CPU oracle, through the public module API."""
 import os
 
 import numpy as np

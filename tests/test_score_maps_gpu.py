@@ -1,5 +1,5 @@
 """Sparse score maps (SURVEY.md section 8f-3, pips_heatmap) against the reference's recorded fcps and the
-dense torch path (B200 only)."""
+dense torch path."""
 import os
 
 import numpy as np

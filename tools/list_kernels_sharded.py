@@ -39,7 +39,7 @@ if rank == 0:
             cnt[name] += 1
     T = sum(tot.values())
     nccl = [k for k in tot if "nccl" in k.lower()]
-    lines = [f"# one particle-sharded Pips.forward on {world} B200s (rank 0; cfg 2 sizes, 1024 particles per rank, frame-sharded encoder), torch.profiler / CUPTI",
+    lines = [f"# one particle-sharded Pips.forward on {world} H100s (rank 0; cfg 2 sizes, 1024 particles per rank, frame-sharded encoder), torch.profiler / CUPTI",
              f"# {sum(cnt.values())} kernel launches, {T / 1e3:.2f} ms of kernel time; collective-library kernels on the data path: {nccl if nccl else 'none'}"]
     for k, v in tot.most_common():
         lines.append(f"{v / 1e3:9.3f} ms  x{cnt[k]:4d}  {k}")
