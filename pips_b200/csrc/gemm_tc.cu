@@ -11,46 +11,150 @@
 //
 // Structure (one CTA per SM, persistent over 128 x BN output tiles; BN = 256 for large problems, 128 / 64 when
 // 256-wide tiles would leave most SMs without a tile -- few particles: the demo clip, chained windows):
-//   warp 0       TMA producer  : cp.async.bulk.tensor 128B-swizzled K-chunks of A and W -> smem ring
-//   warps 4..7   consumer warpgroup 0: rows 0..63 of the tile   } wgmma m64nNk16 straight from the ring, then the
-//   warps 8..11  consumer warpgroup 1: rows 64..127             } epilogue from registers (bias / GELU / residual / split)
-// The producer runs ahead through the ring while a warpgroup is in its epilogue.
+//   warp 0       TMA producer  : cp.async.bulk.tensor 64B-swizzled 32-wide K-blocks of A and W -> smem ring
+//   warps 4..7   consumer warpgroup 0: rows 0..63 of the tile   } wgmma m64nBNk16 straight from the ring, then the
+//   warps 8..11  consumer warpgroup 1: rows 64..127             } epilogue (below)
+// The ring is 4 (x3, BN = 256) to 8 stages deep, so a slot's TMA has several K-blocks of MMAs to land in, and the
+// producer runs ahead into the next tile while the consumers are in their epilogue.
+//
+// Epilogue: bias / GELU + (hi, lo) split in registers, then 32-column chunks of the warpgroup's 64 rows go through a
+// double-buffered staging area in shared memory to one TMA store per chunk (a TMA add-reduce for the residual).  No
+// thread waits on global memory; the stores of a tile's last chunks drain while the next tile's MMAs run.  TMA clips
+// the boxes at M and N, which covers partial tiles.
 //
 // CLUSTER = 2 ("pair" tiles, 256 x 256 per cluster): the two CTAs of a cluster take the two 128-row halves of the tile
 // and share its W tile -- each loads one 128-row half of W and TMA-multicasts it into both shared memories, which
 // halves the W traffic from L2.  A ring slot is then released by the consumers of BOTH CTAs.
 #include <stdlib.h>
 
+#include <string>
+
 #include "gemm_common.cuh"
 
 namespace pips {
 
 constexpr int BM = 128;
-constexpr int GEMM_THREADS = 384;                 // producer warpgroup + 2 consumer warpgroups
-constexpr uint32_t A_TILE_BYTES = BM * BK * 2;     // 16 KB
+constexpr int KB = 32;                                 // K-block of the ring: 32 bf16 = one 64-byte swizzle row
+constexpr int GEMM_THREADS = 384;                      // producer warpgroup + 2 consumer warpgroups
+constexpr uint32_t A_TILE_BYTES = BM * KB * 2;         // 8 KB
+constexpr int EPI_COLS = 32;                           // epilogue chunk: 32 columns of a warpgroup's 64 rows
+constexpr uint32_t EPI_BUF_BYTES = 64 * EPI_COLS * 4;  // 8 KB: an fp32 chunk, or a bf16 hi chunk + a bf16 lo chunk
+constexpr uint32_t EPI_STAGING_BYTES = 2 * 2 * EPI_BUF_BYTES;   // two buffers per consumer warpgroup
 
 template <int TERMS, int BN>
 struct GemmCfg {
-    static constexpr uint32_t kWTileBytes = BN * BK * 2;                  // 32 / 16 / 8 KB
+    static constexpr uint32_t kWTileBytes = BN * KB * 2;                  // 16 / 8 / 4 KB
     static constexpr int kOperandCopies = TERMS == 3 ? 2 : 1;             // hi (+ lo)
     static constexpr uint32_t kStageBytes = kOperandCopies * (A_TILE_BYTES + kWTileBytes);
-    static constexpr uint32_t kFixedBytes = 1024 /*align*/ + 256 /*barriers*/;
+    static constexpr uint32_t kFixedBytes = 1024 /*align*/ + EPI_STAGING_BYTES + 256 /*barriers*/;
     static constexpr int kFit = static_cast<int>((227u * 1024u - kFixedBytes) / kStageBytes);
-    static constexpr int kStages = kFit > 8 ? 8 : kFit;                   // x3: 2 / 3 / 4 for BN = 256 / 128 / 64
+    static constexpr int kStages = kFit > 8 ? 8 : kFit;                   // x3: 4 / 6 / 8 for BN = 256 / 128 / 64
     static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kFixedBytes;
+    static_assert(kStages >= 4 && kSmemBytes <= 227u * 1024u, "ring + staging must fit in 227 KB");
 };
 
+struct GemmArgs {
+    int M, N, K;                 // valid rows / cols, K multiple of 64
+    const float* bias;           // [N]
+    int epilogue;                // PIPS_EPI_*
+    float* out_f32;              // BIAS / BIAS_RESID target (row stride ldo)
+    int ldo;
+    __nv_bfloat16* out_hi;       // BIAS_GELU target (row stride ldh); out_lo may be null
+    __nv_bfloat16* out_lo;
+    int ldh;
+    int num_tiles;               // output tiles of the launched variant (set by its launcher)
+};
+
+struct GemmMaps {
+    CUtensorMap a_hi, a_lo, w_hi, w_lo;    // operands: {KB, rows} boxes, 64-byte swizzle
+    CUtensorMap out_f32;                   // BIAS / BIAS_RESID target: {32, 64} fp32 boxes, 128-byte swizzle
+    CUtensorMap out_hi, out_lo;            // BIAS_GELU targets: {32, 64} bf16 boxes, 64-byte swizzle
+};
+
+template <int BN>
+__device__ __forceinline__ void gemm_mma(float (&d)[BN / 2], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    if constexpr (BN == 256) wgmma_n256(d, a_desc, b_desc, accumulate);
+    else wgmma_tile<BN>(d, a_desc, b_desc, accumulate);
+}
+
+// Offset of byte `byte` of row `row` in a staging chunk with PITCH-byte rows, swizzled the way TMA reads it with a
+// swizzle span of PITCH (128 B: the 16-byte unit is XORed with row % 8; 64 B: with (row / 2) % 4).  The swizzle also
+// spreads the 8 rows that a warp writes at once over distinct banks.
+template <int PITCH>
+__device__ __forceinline__ uint32_t staged(int row, int byte) {
+    const uint32_t o = static_cast<uint32_t>(row * PITCH + byte);
+    return o ^ (((o >> 7) & (PITCH / 16 - 1)) << 4);
+}
+
+// Epilogue of a warpgroup's 64 x BN accumulator (wgmma fragment layout, ptx.cuh).  `row0` is the first of the
+// warpgroup's rows, `n0` the tile's first column, `staging` its two EPI_BUF_BYTES buffers; `chunk` counts the chunks
+// this warpgroup has staged so far (it picks the buffer and tells when a buffer has had a store issued from it).
+template <int BN>
+__device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArgs& args, const float (&acc)[BN / 2], int row0,
+                                             int n0, uint32_t staging, uint32_t& chunk, int wg) {
+    if (row0 >= args.M) return;                                           // whole warpgroup past M: nothing to store
+    const int lane = threadIdx.x & 31;
+    const int r = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);           // fragment rows r, r + 8 of the 64
+    const int cq = 2 * (lane & 3);                                        // fragment columns cq, cq + 1 of each 8
+    const bool issuer = (threadIdx.x & 127) == 0;
+    const bool gelu = args.epilogue == PIPS_EPI_BIAS_GELU;
+#pragma unroll
+    for (int c = 0; c < BN / EPI_COLS; ++c) {
+        const int col0 = n0 + c * EPI_COLS;
+        if (col0 >= args.N) break;
+        const uint32_t buf = staging + (chunk & 1) * EPI_BUF_BYTES;
+        if (issuer && chunk >= 2) bulk_wait_read<1>();                   // the store issued from buf two chunks ago has read it
+        named_bar_sync(1 + wg, 128);
+#pragma unroll
+        for (int jj = 0; jj < EPI_COLS / 8; ++jj) {
+            const int j = c * (EPI_COLS / 8) + jj;
+            const int col = col0 + 8 * jj + cq;
+            const float2 b = make_float2(col < args.N ? __ldg(args.bias + col) : 0.f, col + 1 < args.N ? __ldg(args.bias + col + 1) : 0.f);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const float2 f = add2(make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]), b);
+                if (gelu) {
+                    const float2 g = gelu_fast2_abs(f);
+                    const uint32_t hw = cvt_bf16x2(g.x, g.y);
+                    const uint32_t o = staged<EPI_COLS * 2>(r + 8 * h, (8 * jj + cq) * 2);
+                    st_shared_u32(buf + o, hw);
+                    if (args.out_lo) {
+                        const float2 lo = fma2(make_float2(__uint_as_float(hw << 16), __uint_as_float(hw & 0xffff0000u)), bcast2(-1.0f), g);   // g - hi, one rounding
+                        st_shared_u32(buf + EPI_BUF_BYTES / 2 + o, cvt_bf16x2(lo.x, lo.y));
+                    }
+                } else {
+                    st_shared_f32x2(buf + staged<EPI_COLS * 4>(r + 8 * h, (8 * jj + cq) * 4), f);
+                }
+            }
+        }
+        fence_proxy_async_smem();                                         // make the writes visible to the TMA unit
+        named_bar_sync(1 + wg, 128);
+        if (issuer) {
+            if (gelu) {
+                tma_store_2d(&maps.out_hi, buf, col0, row0);
+                if (args.out_lo) tma_store_2d(&maps.out_lo, buf + EPI_BUF_BYTES / 2, col0, row0);
+            } else if (args.epilogue == PIPS_EPI_BIAS_RESID) {
+                tma_reduce_add_2d(&maps.out_f32, buf, col0, row0);       // x + (acc + b): the bits of (acc + b) + x
+            } else {
+                tma_store_2d(&maps.out_f32, buf, col0, row0);
+            }
+            bulk_commit();
+        }
+        ++chunk;
+    }
+}
+
 template <int TERMS, int BN, int CLUSTER>
-__device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const CUtensorMap& map_a_lo, const CUtensorMap& map_w_hi,
-                                             const CUtensorMap& map_w_lo, const GemmArgs& args) {
+__device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArgs& args) {
     using Cfg = GemmCfg<TERMS, BN>;
     constexpr int kStages = Cfg::kStages;
     constexpr uint32_t W_TILE_BYTES = Cfg::kWTileBytes;
     static_assert(CLUSTER == 1 || BN == 256, "cluster tiles are 256 columns wide");
     extern __shared__ uint8_t smem_raw[];
-    // 128B swizzle atoms need 1024-byte alignment
+    // the 128-byte-swizzled staging buffers need 1024-byte alignment (the 64-byte-swizzled ring needs 512)
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
+    uint8_t* staging = smem + kStages * Cfg::kStageBytes;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(staging + EPI_STAGING_BYTES);
     const uint32_t full0 = smem_u32(bars);                  // full[kStages], empty[kStages]
     const uint32_t empty0 = full0 + 8 * kStages;
 
@@ -62,15 +166,20 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const 
 
     constexpr int TM = BM * CLUSTER;
     const int tiles_n = (args.N + BN - 1) / BN;
-    const int num_tiles = ((args.M + TM - 1) / TM) * tiles_n;
-    const int num_kb = args.K / BK;
+    const int num_kb = args.K / KB;
 
     if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&map_a_hi);
-        tma_prefetch_desc(&map_w_hi);
+        tma_prefetch_desc(&maps.a_hi);
+        tma_prefetch_desc(&maps.w_hi);
         if (TERMS == 3) {
-            tma_prefetch_desc(&map_a_lo);
-            tma_prefetch_desc(&map_w_lo);
+            tma_prefetch_desc(&maps.a_lo);
+            tma_prefetch_desc(&maps.w_lo);
+        }
+        if (args.epilogue == PIPS_EPI_BIAS_GELU) {
+            tma_prefetch_desc(&maps.out_hi);
+            if (args.out_lo) tma_prefetch_desc(&maps.out_lo);
+        } else {
+            tma_prefetch_desc(&maps.out_f32);
         }
     }
     if (warp == 1 && lane == 0) {
@@ -90,7 +199,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const 
         if (warp == 0 && lane == 0) {
             // ------------------------------------------------------------ TMA producer
             uint32_t stage = 0, phase = 0;
-            for (int t = worker; t < num_tiles; t += num_workers) {
+            for (int t = worker; t < args.num_tiles; t += num_workers) {
                 const int m0 = (t / tiles_n) * TM + static_cast<int>(rank) * BM;
                 const int n0 = (t % tiles_n) * BN;
                 for (int kb = 0; kb < num_kb; ++kb) {
@@ -98,19 +207,19 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const 
                     const uint32_t fb = full0 + 8 * stage;
                     mbar_arrive_expect_tx(fb, Cfg::kStageBytes);
                     const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
-                    const int k0 = kb * BK;
-                    tma_load_2d(base, &map_a_hi, fb, k0, m0);
-                    if (TERMS == 3) tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES, &map_a_lo, fb, k0, m0);
+                    const int k0 = kb * KB;
+                    tma_load_2d(base, &maps.a_hi, fb, k0, m0);
+                    if (TERMS == 3) tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES, &maps.a_lo, fb, k0, m0);
                     if (CLUSTER == 2) {
                         // this CTA's half of the W tile (box = 128 rows), into both CTAs
                         const uint32_t half = rank * (W_TILE_BYTES / 2);
-                        tma_load_2d_multicast(base + A_TILE_BYTES + half, &map_w_hi, fb, k0, n0 + static_cast<int>(rank) * (BN / 2), 3);
+                        tma_load_2d_multicast(base + A_TILE_BYTES + half, &maps.w_hi, fb, k0, n0 + static_cast<int>(rank) * (BN / 2), 3);
                         if (TERMS == 3)
-                            tma_load_2d_multicast(base + 2 * A_TILE_BYTES + W_TILE_BYTES + half, &map_w_lo, fb, k0,
+                            tma_load_2d_multicast(base + 2 * A_TILE_BYTES + W_TILE_BYTES + half, &maps.w_lo, fb, k0,
                                                   n0 + static_cast<int>(rank) * (BN / 2), 3);
                     } else {
-                        tma_load_2d(base + A_TILE_BYTES, &map_w_hi, fb, k0, n0);
-                        if (TERMS == 3) tma_load_2d(base + 2 * A_TILE_BYTES + W_TILE_BYTES, &map_w_lo, fb, k0, n0);
+                        tma_load_2d(base + A_TILE_BYTES, &maps.w_hi, fb, k0, n0);
+                        if (TERMS == 3) tma_load_2d(base + 2 * A_TILE_BYTES + W_TILE_BYTES, &maps.w_lo, fb, k0, n0);
                     }
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
                 }
@@ -121,27 +230,29 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const 
         // ------------------------------------------------------------ consumers: MMA + epilogue, 64 rows each
         const int wg = (warp - 4) >> 2;
         const bool releaser = (threadIdx.x & 127) == 0;
+        const uint32_t my_staging = smem_u32(staging) + wg * 2 * EPI_BUF_BYTES;
+        uint32_t chunk = 0;
         float acc[BN / 2];
         uint32_t stage = 0, phase = 0;
-        for (int t = worker; t < num_tiles; t += num_workers) {
+        for (int t = worker; t < args.num_tiles; t += num_workers) {
             const int m0 = (t / tiles_n) * TM + static_cast<int>(rank) * BM;
             const int n0 = (t % tiles_n) * BN;
             int prev = -1;                                   // ring slot whose MMAs are still in flight
             for (int kb = 0; kb < num_kb; ++kb) {
                 mbar_wait(full0 + 8 * stage, phase);
                 const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
-                const uint64_t a_hi = wgmma_desc_sw128(base + wg * (A_TILE_BYTES / 2));
-                const uint64_t w_hi = wgmma_desc_sw128(base + A_TILE_BYTES);
-                const uint64_t a_lo = wgmma_desc_sw128(base + A_TILE_BYTES + W_TILE_BYTES + wg * (A_TILE_BYTES / 2));
-                const uint64_t w_lo = wgmma_desc_sw128(base + 2 * A_TILE_BYTES + W_TILE_BYTES);
+                const uint64_t a_hi = wgmma_desc_sw64(base + wg * (A_TILE_BYTES / 2));
+                const uint64_t w_hi = wgmma_desc_sw64(base + A_TILE_BYTES);
+                const uint64_t a_lo = wgmma_desc_sw64(base + A_TILE_BYTES + W_TILE_BYTES + wg * (A_TILE_BYTES / 2));
+                const uint64_t w_lo = wgmma_desc_sw64(base + 2 * A_TILE_BYTES + W_TILE_BYTES);
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BK / MMA_K; ++k) {
+                for (int k = 0; k < KB / MMA_K; ++k) {
                     const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);   // 32 B per K=16 step
-                    wgmma_tile<BN>(acc, a_hi + adv, w_hi + adv, (kb | k) != 0);
+                    gemm_mma<BN>(acc, a_hi + adv, w_hi + adv, (kb | k) != 0);
                     if (TERMS == 3) {
-                        wgmma_tile<BN>(acc, a_lo + adv, w_hi + adv, 1);
-                        wgmma_tile<BN>(acc, a_hi + adv, w_lo + adv, 1);
+                        gemm_mma<BN>(acc, a_lo + adv, w_hi + adv, 1);
+                        gemm_mma<BN>(acc, a_hi + adv, w_lo + adv, 1);
                     }
                 }
                 wgmma_commit();
@@ -161,38 +272,67 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const 
                 mbar_arrive(empty0 + 8 * prev);
                 if (CLUSTER == 2) mbar_arrive_cluster(empty0 + 8 * prev, rank ^ 1);
             }
-            epilogue_frag<BN>(args, acc, m0 + wg * 64, n0);
+            epilogue_tma<BN>(maps, args, acc, m0 + wg * 64, n0, my_staging, chunk, wg);
         }
+        if (releaser) bulk_wait<0>();                        // the last stores have finished reading shared memory and writing
     }
     if (CLUSTER == 2) cluster_sync_all();                   // nobody leaves while the peer may still signal or write to us
 }
 
 template <int TERMS, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-               const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-               const GemmArgs args) {
-    gemm_tc_body<TERMS, BN, 1>(map_a_hi, map_a_lo, map_w_hi, map_w_lo, args);
+gemm_tc_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs args) {
+    gemm_tc_body<TERMS, BN, 1>(maps, args);
 }
 
 template <int TERMS>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_tc_pair_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                    const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-                    const GemmArgs args) {
-    gemm_tc_body<TERMS, 256, 2>(map_a_hi, map_a_lo, map_w_hi, map_w_lo, args);
+gemm_tc_pair_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs args) {
+    gemm_tc_body<TERMS, 256, 2>(maps, args);
 }
 
 // ---------------------------------------------------------------------------------- host side
 
 static bool make_operand_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld_elems, int box_rows) {
-    // global tensor (innermost first): {K, rows}, row stride ld_elems*2 bytes; box {64, box_rows}, 128B swizzle
+    // global tensor (innermost first): {K, rows}, row stride ld_elems*2 bytes; box {32, box_rows}, 64B swizzle
     cuuint64_t gdim[2] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(rows)};
     cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ld_elems) * 2};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(BK), static_cast<cuuint32_t>(box_rows)};
+    cuuint32_t box[2] = {static_cast<cuuint32_t>(KB), static_cast<cuuint32_t>(box_rows)};
     cuuint32_t estr[2] = {1, 1};
     return encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_SWIZZLE_128B);
+                        CU_TENSOR_MAP_SWIZZLE_64B);
+}
+
+// Output tensor {N, M} with row stride `ld` elements; box {EPI_COLS, 64} (one warpgroup's chunk), swizzled like the
+// staging buffer.  The bounds are the problem's, so TMA drops the rows and columns of a tile beyond M and N.
+static bool make_output_map(CUtensorMap* map, void* ptr, const GemmArgs& args, int ld, bool f32) {
+    cuuint64_t gdim[2] = {static_cast<cuuint64_t>(args.N), static_cast<cuuint64_t>(args.M)};
+    cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ld) * (f32 ? 4 : 2)};
+    cuuint32_t box[2] = {static_cast<cuuint32_t>(EPI_COLS), 64};
+    cuuint32_t estr[2] = {1, 1};
+    return encode_tiled(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, gdim, gstride, box,
+                        estr, f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
+}
+
+// every map of the problem; W boxes are `w_box_rows` rows (the tile width, or its half in the pair kernel)
+static const char* make_maps(GemmMaps* m, bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi,
+                             const void* w_lo, int ldw, int w_rows, int w_box_rows, const GemmArgs& args) {
+    *m = GemmMaps{};
+    if (!make_operand_map(&m->a_hi, a_hi, a_rows, args.K, lda, BM)) return "tensor map (A hi) failed";
+    if (!make_operand_map(&m->w_hi, w_hi, w_rows, args.K, ldw, w_box_rows)) return "tensor map (W hi) failed";
+    m->a_lo = m->a_hi;
+    m->w_lo = m->w_hi;
+    if (x3) {
+        if (!make_operand_map(&m->a_lo, a_lo, a_rows, args.K, lda, BM)) return "tensor map (A lo) failed";
+        if (!make_operand_map(&m->w_lo, w_lo, w_rows, args.K, ldw, w_box_rows)) return "tensor map (W lo) failed";
+    }
+    if (args.epilogue == PIPS_EPI_BIAS_GELU) {
+        if (!make_output_map(&m->out_hi, args.out_hi, args, args.ldh, false)) return "tensor map (out hi) failed";
+        if (args.out_lo && !make_output_map(&m->out_lo, args.out_lo, args, args.ldh, false)) return "tensor map (out lo) failed";
+    } else if (!make_output_map(&m->out_f32, args.out_f32, args, args.ldo, true)) {
+        return "tensor map (out) failed: out_f32 must be 16-byte aligned";
+    }
+    return nullptr;
 }
 
 // 0: automatic, 1: pair kernel, 64/128/256: single-CTA kernel with that tile width
@@ -242,7 +382,7 @@ extern "C" int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_r
     } else {
         return fail("pips_gemm_tc: unknown epilogue");
     }
-    GemmArgs args;
+    GemmArgs args = {};
     args.M = M; args.N = N; args.K = K; args.bias = bias; args.epilogue = epilogue;
     args.out_f32 = out_f32; args.ldo = ldo;
     args.out_hi = static_cast<__nv_bfloat16*>(out_hi); args.out_lo = static_cast<__nv_bfloat16*>(out_lo); args.ldh = ldh;
@@ -272,77 +412,59 @@ extern "C" int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_r
 namespace pips {
 
 template <int TERMS, int BN>
-static int launch_variant(const CUtensorMap& ma_hi, const CUtensorMap& ma_lo, const CUtensorMap& mw_hi, const CUtensorMap& mw_lo,
-                          const GemmArgs& args, cudaStream_t st) {
+static int launch_variant(const GemmMaps& maps, const GemmArgs& args, cudaStream_t st) {
     using Cfg = GemmCfg<TERMS, BN>;
     static bool attr[kMaxDevices] = {};
     {
         cudaError_t e = ensure_dyn_smem(gemm_tc_kernel<TERMS, BN>, attr, Cfg::kSmemBytes);
         if (e != cudaSuccess) return fail_cuda("pips_gemm_tc: smem attribute", e);
     }
-    const int tiles = ((args.M + BM - 1) / BM) * ((args.N + BN - 1) / BN);
-    const int grid = tiles < sm_count() ? tiles : sm_count();
-    cudaError_t e = launch_pdl(gemm_tc_kernel<TERMS, BN>, dim3(grid), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, ma_hi, ma_lo, mw_hi, mw_lo, args);
+    GemmArgs a = args;
+    a.num_tiles = ((args.M + BM - 1) / BM) * ((args.N + BN - 1) / BN);
+    const int grid = a.num_tiles < sm_count() ? a.num_tiles : sm_count();
+    cudaError_t e = launch_pdl(gemm_tc_kernel<TERMS, BN>, dim3(grid), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, maps, a);
     if (e == cudaSuccess) e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail_cuda("pips_gemm_tc: launch", e);
 }
 
 template <int TERMS>
-static int launch_pair_variant(const CUtensorMap& ma_hi, const CUtensorMap& ma_lo, const CUtensorMap& mw_hi, const CUtensorMap& mw_lo,
-                               const GemmArgs& args, cudaStream_t st) {
+static int launch_pair_variant(const GemmMaps& maps, const GemmArgs& args, cudaStream_t st) {
     using Cfg = GemmCfg<TERMS, 256>;
     static bool attr[kMaxDevices] = {};
     {
         cudaError_t e = ensure_dyn_smem(gemm_tc_pair_kernel<TERMS>, attr, Cfg::kSmemBytes);
         if (e != cudaSuccess) return fail_cuda("pips_gemm_tc (pair): smem attribute", e);
     }
-    const int tiles = ((args.M + 255) / 256) * ((args.N + 255) / 256);
+    GemmArgs a = args;
+    a.num_tiles = ((args.M + 255) / 256) * ((args.N + 255) / 256);
     const int max_pairs = sm_count() / 2;
-    const int pairs = tiles < max_pairs ? tiles : max_pairs;
-    cudaError_t e = launch_pdl(gemm_tc_pair_kernel<TERMS>, dim3(2 * pairs), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, ma_hi, ma_lo, mw_hi,
-                               mw_lo, args);
+    const int pairs = a.num_tiles < max_pairs ? a.num_tiles : max_pairs;
+    cudaError_t e = launch_pdl(gemm_tc_pair_kernel<TERMS>, dim3(2 * pairs), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, maps, a);
     if (e == cudaSuccess) e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail_cuda("pips_gemm_tc (pair): launch", e);
 }
 
 int launch_pair(bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo, int ldw,
                 int w_rows, const GemmArgs& args, cudaStream_t st) {
-    CUtensorMap ma_hi, ma_lo, mw_hi, mw_lo;                  // every box is 128 rows: a CTA's rows of A, its half of the W tile
-    if (!make_operand_map(&ma_hi, a_hi, a_rows, args.K, lda, BM)) return fail("pips_gemm_tc (pair): tensor map (A hi) failed");
-    if (!make_operand_map(&mw_hi, w_hi, w_rows, args.K, ldw, 128)) return fail("pips_gemm_tc (pair): tensor map (W hi) failed");
-    ma_lo = ma_hi;
-    mw_lo = mw_hi;
-    if (x3) {
-        if (!make_operand_map(&ma_lo, a_lo, a_rows, args.K, lda, BM)) return fail("pips_gemm_tc (pair): tensor map (A lo) failed");
-        if (!make_operand_map(&mw_lo, w_lo, w_rows, args.K, ldw, 128)) return fail("pips_gemm_tc (pair): tensor map (W lo) failed");
+    GemmMaps maps;                                           // every operand box is 128 rows: a CTA's rows of A, its half of the W tile
+    if (const char* err = make_maps(&maps, x3, a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, 128, args)) {
+        return fail((std::string("pips_gemm_tc (pair): ") + err).c_str());
     }
-    return x3 ? launch_pair_variant<3>(ma_hi, ma_lo, mw_hi, mw_lo, args, st) : launch_pair_variant<1>(ma_hi, ma_lo, mw_hi, mw_lo, args, st);
+    return x3 ? launch_pair_variant<3>(maps, args, st) : launch_pair_variant<1>(maps, args, st);
 }
 
 int launch_single(int bn, bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo,
                   int ldw, int w_rows, const GemmArgs& args, cudaStream_t st) {
-    const int K = args.K;
-    CUtensorMap ma_hi, ma_lo, mw_hi, mw_lo;
-    if (!make_operand_map(&ma_hi, a_hi, a_rows, K, lda, BM)) return fail("pips_gemm_tc: tensor map (A hi) failed");
-    if (!make_operand_map(&mw_hi, w_hi, w_rows, K, ldw, bn)) return fail("pips_gemm_tc: tensor map (W hi) failed");
-    ma_lo = ma_hi;
-    mw_lo = mw_hi;
-    if (x3) {
-        if (!make_operand_map(&ma_lo, a_lo, a_rows, K, lda, BM)) return fail("pips_gemm_tc: tensor map (A lo) failed");
-        if (!make_operand_map(&mw_lo, w_lo, w_rows, K, ldw, bn)) return fail("pips_gemm_tc: tensor map (W lo) failed");
+    GemmMaps maps;
+    if (const char* err = make_maps(&maps, x3, a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, bn, args)) {
+        return fail((std::string("pips_gemm_tc: ") + err).c_str());
     }
-    int rc;
-    if (x3) rc = bn == 256 ? launch_variant<3, 256>(ma_hi, ma_lo, mw_hi, mw_lo, args, st)
-               : bn == 128 ? launch_variant<3, 128>(ma_hi, ma_lo, mw_hi, mw_lo, args, st)
-                           : launch_variant<3, 64>(ma_hi, ma_lo, mw_hi, mw_lo, args, st);
-    else rc = bn == 256 ? launch_variant<1, 256>(ma_hi, ma_lo, mw_hi, mw_lo, args, st)
-            : bn == 128 ? launch_variant<1, 128>(ma_hi, ma_lo, mw_hi, mw_lo, args, st)
-                        : launch_variant<1, 64>(ma_hi, ma_lo, mw_hi, mw_lo, args, st);
-    if (rc) return rc;
-    cudaError_t e;
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda("pips_gemm_tc: launch", e);
-    return 0;
+    if (x3) return bn == 256 ? launch_variant<3, 256>(maps, args, st)
+                 : bn == 128 ? launch_variant<3, 128>(maps, args, st)
+                             : launch_variant<3, 64>(maps, args, st);
+    return bn == 256 ? launch_variant<1, 256>(maps, args, st)
+         : bn == 128 ? launch_variant<1, 128>(maps, args, st)
+                     : launch_variant<1, 64>(maps, args, st);
 }
 
 }  // namespace pips

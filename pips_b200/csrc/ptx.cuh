@@ -53,6 +53,13 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
 }
 
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float2 v) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
+}
+
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const void* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
@@ -68,6 +75,31 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* map, uint3
         "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
         ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
+}
+
+// shared -> global tensor stores; each issuing thread tracks its own bulk groups
+__device__ __forceinline__ void tma_store_2d(const void* map, uint32_t src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1)
+                 : "memory");
+}
+// global[box] += shared[box], element-wise in the tensor map's data type
+__device__ __forceinline__ void tma_reduce_add_2d(const void* map, uint32_t src, int c0, int c1) {
+    asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's groups are still in flight (writes included)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
+// barrier among `threads` threads of the CTA (a warpgroup: 128) on hardware barrier `id` (0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // ---------------------------------------------------------------- clusters
@@ -156,6 +188,19 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a_desc, uint
         : "l"(a_desc), "l"(b_desc), "r"(accumulate)
         : "memory");
 }
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1, 0, 0;\n\t}"
+        : PIPS_ACC64(d, 0), PIPS_ACC64(d, 64)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
 
 // 64 x BN tile: BN = 256 as two N = 128 instructions on the two 128-row halves of the B tile (128-byte rows)
 template <int BN>
@@ -179,6 +224,16 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     d |= static_cast<uint64_t>(1) << 16;                          // leading byte offset (unused: one swizzle atom along K)
     d |= static_cast<uint64_t>(1024 >> 4) << 32;                  // stride byte offset between 8-row groups
     d |= static_cast<uint64_t>(1) << 62;                          // SWIZZLE_128B
+    return d;
+}
+// K-major, 64-byte-swizzled operand tile (rows of 32 bf16 = 64 B, 8-row groups 512 B apart):
+// the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_64B and a {32, rows} box.
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);      // start address, 16 B units
+    d |= static_cast<uint64_t>(1) << 16;                          // leading byte offset (unused: one swizzle atom along K)
+    d |= static_cast<uint64_t>(512 >> 4) << 32;                   // stride byte offset between 8-row groups
+    d |= static_cast<uint64_t>(2) << 62;                          // SWIZZLE_64B
     return d;
 }
 
