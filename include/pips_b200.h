@@ -148,6 +148,21 @@ size_t pips_heatmap_scratch_floats(int frames, int n_sel, int H8, int W8);
 int pips_heatmap(const void* const* lvl, int feat_dtype, int B, int S, int N, int H8, int W8, const float* ffeats,
                  const int* sel, const int* slot, int n_sel, float* scratch, float* out, size_t out_frame_stride, void* stream);
 
+/* nets/pips.py:58-90 (score_map_loss) without the dense score maps (csrc/scoremap_loss.cu).  The score map of
+ * nets/pips.py:504-511 is fcp[b,s,n,p] = <ffeats[b,s,n], G[b,s,p]> with
+ *   G[b,s,p,:] = sum_l interpolate(fmap_l[b,s], (H8,W8), bilinear, align_corners=True)(p,:) / sqrt(C).
+ * pips_scoremap_basis: G from the fp32 pyramid levels lvl_f32[4] (channels-last) as a bf16 (hi, lo) pair,
+ *   G_hi / G_lo (frames, H8*W8, 128).  Once per forward.
+ * pips_scoremap_loss: one iteration.  ffeats is the loop state ((b*N+n), s, c) at the start of the iteration;
+ *   target (B,S,N) int32 is y*W8 + x of the row's target pixel, or -1 for a row the loss ignores.  For every row
+ *   r = (b*S + s)*N + n it writes pos_part[r] = softplus(-fcp[t]) and neg_part[r, k] = sum of softplus(fcp[p]) over
+ *   the pixels p != t of split k (both 0 for target -1).  The score GEMM runs in bf16x3; scores never reach memory.
+ * pips_scoremap_splits: n_split, the number of pixel splits (columns of neg_part); a function of H8*W8 only. */
+int pips_scoremap_splits(int H8, int W8);
+int pips_scoremap_basis(const float* const* lvl_f32, int frames, int H8, int W8, void* G_hi, void* G_lo, void* stream);
+int pips_scoremap_loss(const void* G_hi, const void* G_lo, const float* ffeats, int B, int S, int N, int H8, int W8,
+                       const int* target, float* neg_part, float* pos_part, void* stream);
+
 /* v -> (hi, lo) bf16 with hi = rn(v), lo = rn(v - hi); lo may be NULL.  Used to pack weights. */
 int pips_split_bf16(const float* src, void* hi, void* lo, size_t n, void* stream);
 

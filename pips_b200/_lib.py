@@ -79,6 +79,9 @@ _SIGNATURES = {
     "pips_update_peer": (_i, [_p] * 9 + [_f, _i, _i, _i, C.POINTER(PeerOut), _p]),
     "pips_heatmap_scratch_floats": (C.c_size_t, [_i, _i, _i, _i]),
     "pips_heatmap": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _i, _p, _p, _p, _i, _p, _p, C.c_size_t, _p]),
+    "pips_scoremap_splits": (_i, [_i, _i]),
+    "pips_scoremap_basis": (_i, [C.POINTER(_p), _i, _i, _i, _p, _p, _p]),
+    "pips_scoremap_loss": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "pips_gemm_tc": (_i, [_p, _p, _i, _i, _p, _p, _i, _i, _i, _i, _i, _p, _i, _p, _i, _p, _p, _i, _p]),
     "pips_gemm_f32": (_i, [_p, _i, _p, _i, _i, _i, _i, _p, _i, _p, _i, _p]),
     "pips_tokenmix": (_i, [_p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),

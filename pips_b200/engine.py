@@ -40,6 +40,15 @@ def _round_up(v: int, m: int) -> int:
     return (v + m - 1) // m * m
 
 
+def _score_map_loss(neg: torch.Tensor, pos: torch.Tensor, target: torch.Tensor, iters: int, P: int) -> torch.Tensor:
+    """nets/pips.py:83-88 from the per-row terms of pips_scoremap_loss: the balanced CE of every kept row's score map
+    against a one-hot at its target, reduce_masked_mean (utils/basic.py:59, eps 1e-6) over the pos and the neg pixels.
+    Rows with target -1 hold zeros.  Fixed-shape fp64 sums: the same bits for the same shape, however it was launched."""
+    k = (target >= 0).sum().double() * iters
+    loss = pos.double().sum() / (1e-6 + k) + neg.double().sum() / (1e-6 + k * (P - 1))
+    return loss.float()
+
+
 class PackedWeights:
     """Kernel-layout copies of the DeltaBlock / head parameters.
 
@@ -276,15 +285,21 @@ class RefineEngine:
     # ------------------------------------------------------------------ the loop
     def _enqueue(self, lib, wc, pyr: Pyramid, ws: Workspace, fmaps2d, c, c0, ffeat, ffeats, feat_init, out, vis,
                  B, S, nc, H8, W8, iters, stride, on_iter=None, build_pyramid=True, frame_base=None, T=0,
-                 heat=None, peer=None, peer_n0=0) -> int:
+                 heat=None, peer=None, peer_n0=0, loss=None) -> int:
         """Enqueue every launch of one forward for ``nc`` particles on the current stream: pyramid, initial
-        features, ``iters`` refinement iterations, visibility head.  Returns the number of kernels launched."""
+        features, ``iters`` refinement iterations, visibility head.  Returns the number of kernels launched.
+        ``loss`` (G_hi, G_lo, target (B,S,nc) int32, neg (iters, B*S*nc, n_split), pos (iters, B*S*nc)): also the
+        score-map loss terms of every iteration (pips_scoremap_loss); the basis G is built with the pyramid."""
         st = self._stream()
         launches = 0
         if build_pyramid:
             with nvtx_range("pips/pyramid"):
                 pyr.build(fmaps2d, st)
             launches += 4
+            if loss is not None:
+                L.check(lib.pips_scoremap_basis(pyr.f32_ptrs, pyr.frames, H8, W8, L.ptr(loss[0]), L.ptr(loss[1]), st),
+                        "pips_scoremap_basis")
+                launches += 1
         c0.copy_(c)
         if feat_init is None:
             L.check(lib.pips_init_gather(L.ptr(pyr.f32[0]), B, S, nc, H8, W8, L.ptr(c), L.ptr(frame_base), T, L.ptr(ffeat),
@@ -319,6 +334,11 @@ class RefineEngine:
                                          sel.numel(), L.ptr(scratch), L.ptr(fcps[0, 0, it]),
                                          fcps.stride(1), st), "pips_heatmap")
                 launches += 1 + (sel.numel() + 31) // 32
+            if loss is not None:                    # plain launch: the iteration's kernels wait until ffeats is read
+                g_hi, g_lo, target, neg, pos = loss
+                L.check(lib.pips_scoremap_loss(L.ptr(g_hi), L.ptr(g_lo), L.ptr(ffeats), B, S, nc, H8, W8, L.ptr(target),
+                                               L.ptr(neg[it]), L.ptr(pos[it]), st), "pips_scoremap_loss")
+                launches += 1
             with nvtx_range(f"pips/iter{it}"):
                 L.check(lib.pips_refine_iter(C.byref(prob), C.byref(wc), C.byref(ws.c), L.ptr(out[it]), st), "pips_refine_iter")
             launches += 1 + (1 + 3 * L.DEPTH + 2) + 1
@@ -331,7 +351,8 @@ class RefineEngine:
     def refine(self, module, fmaps: torch.Tensor, coords: torch.Tensor, feat_init: Optional[torch.Tensor],
                iters: int, stride: float, on_iter=None, frame_base: Optional[torch.Tensor] = None,
                reuse_pyramid: bool = False, heat_sel: Optional[torch.Tensor] = None,
-               heat_out: Optional[torch.Tensor] = None, peer=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+               heat_out: Optional[torch.Tensor] = None, peer=None, loss_target: Optional[torch.Tensor] = None,
+               loss_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """fmaps (B,S,128,H8,W8) fp32, coords (B,S,N,2) fp32 in feature-map pixels.
         Returns preds (iters,B,S,N,2) in input pixels, vis_e (B,S,N) logits, ffeat (B,N,128).
         ``on_iter(it, coords_px)`` (optional) is called once per iteration when the particles fit one
@@ -342,7 +363,10 @@ class RefineEngine:
         ``heat_sel`` (n_sel,) particle indices + ``heat_out`` (B,S,iters,n_sel,H8,W8) fp32: also write the score maps
         of those particles (nets/pips.py:504-511) at the start of every iteration (eager launches, no graph).
         ``peer`` (pips_b200.peer.PeerPlan): this call refines one rank's slice of a particle-sharded run; the update
-        kernel also stores every iteration's prediction into all ranks' slabs (the caller runs the barriers)."""
+        kernel also stores every iteration's prediction into all ranks' slabs (the caller runs the barriers).
+        ``loss_target`` (B,S,N) int32 (y*W8 + x of the ground-truth pixel, -1 for a row the loss ignores) + ``loss_out``
+        (0-dim fp32): also compute the score-map loss of nets/pips.py:58-90 over all iterations into ``loss_out``,
+        without materialising the score maps (pips_scoremap_loss)."""
         lib = L.load()
         B, T, Cc, H8, W8 = fmaps.shape
         S = coords.shape[1]
@@ -366,11 +390,21 @@ class RefineEngine:
             assert n_sel > 0 and int(heat_sel.min()) >= 0 and int(heat_sel.max()) < N, "heat_sel out of range"
             assert heat_out is not None and tuple(heat_out.shape) == (B, S, iters, n_sel, H8, W8) \
                 and heat_out.dtype == torch.float32 and heat_out.is_contiguous() and heat_out.device == dev
+        n_split = 0
+        if loss_target is not None:
+            if frame_base is not None or peer is not None:
+                raise L.PipsCudaError("pips_b200: score-map losses are not defined for chained windows or sharded runs")
+            assert tuple(loss_target.shape) == (B, S, N) and loss_target.dtype == torch.int32 \
+                and loss_target.is_contiguous() and loss_target.device == dev, "loss_target must be (B,S,N) int32"
+            assert loss_out is not None and loss_out.dim() == 0 and loss_out.dtype == torch.float32 and loss_out.device == dev
+            n_split = lib.pips_scoremap_splits(H8, W8)
         if N <= chunk and self.use_graph and iters > 0 and frame_base is None and heat_sel is None:
             plan = self._plan(w, B, S, N, H8, W8, iters, float(stride), feat_init is not None, dev,
-                              nhwc=not fmaps2d.is_contiguous(), peer=peer)
-            preds, vis, ffeat = plan.run(fmaps2d, coords, feat_init)
+                              nhwc=not fmaps2d.is_contiguous(), peer=peer, losses=loss_target is not None)
+            preds, vis, ffeat = plan.run(fmaps2d, coords, feat_init, loss_target)
             self.launches = plan.launches
+            if loss_target is not None:
+                loss_out.copy_(_score_map_loss(plan.neg, plan.pos, loss_target, iters, H8 * W8))
             if on_iter is not None:
                 for it in range(iters):
                     on_iter(it, preds[it])
@@ -380,6 +414,11 @@ class RefineEngine:
         preds = torch.empty(iters, B, S, N, 2, dtype=torch.float32, device=dev)
         vis = torch.empty(B, S, N, dtype=torch.float32, device=dev)
         ffeat_out = torch.empty(B, N, LATENT, dtype=torch.float32, device=dev)
+        if loss_target is not None:
+            g_hi = torch.empty(B * S, H8 * W8, LATENT, dtype=torch.bfloat16, device=dev)
+            g_lo = torch.empty_like(g_hi)
+            neg = torch.empty(iters, B, S, N, n_split, dtype=torch.float32, device=dev)
+            pos = torch.empty(iters, B, S, N, dtype=torch.float32, device=dev)
         self.launches = 0
         for n0 in range(0, N, chunk):
             n1 = min(N, n0 + chunk)
@@ -399,23 +438,35 @@ class RefineEngine:
                 inside = ((heat_sel >= n0) & (heat_sel < n1)).nonzero().flatten()
                 if inside.numel() > 0:
                     heat = ((heat_sel[inside] - n0).to(torch.int32).contiguous(), inside.to(torch.int32).contiguous(), heat_out)
+            loss = None
+            if loss_target is not None:             # a chunk's rows of the shared partial sums, same layout, same bits
+                tn = neg if whole else torch.empty(iters, B, S, nc, n_split, dtype=torch.float32, device=dev)
+                tp = pos if whole else torch.empty(iters, B, S, nc, dtype=torch.float32, device=dev)
+                tg = loss_target if whole else loss_target[:, :, n0:n1].contiguous()
+                loss = (g_hi, g_lo, tg, tn.view(iters, B * S * nc, n_split), tp.view(iters, B * S * nc))
             self.launches += self._enqueue(lib, w.c, pyr, ws, fmaps2d, c, c0, ffeat, ffeats, fi, out, v, B, S, nc, H8, W8,
                                            iters, stride, on_iter if whole else None,
                                            build_pyramid=(n0 == 0 and not reuse_pyramid), frame_base=fb, T=T, heat=heat,
-                                           peer=peer, peer_n0=n0)
+                                           peer=peer, peer_n0=n0, loss=loss)
             if not whole:
                 preds[:, :, :, n0:n1] = out
                 vis[:, :, n0:n1] = v
+                if loss is not None:
+                    neg[:, :, :, n0:n1] = tn
+                    pos[:, :, :, n0:n1] = tp
             ffeat_out[:, n0:n1] = ffeat.reshape(B, nc, LATENT)
+        if loss_target is not None:
+            loss_out.copy_(_score_map_loss(neg, pos, loss_target, iters, H8 * W8))
         return preds, vis, ffeat_out
 
-    def _plan(self, w: PackedWeights, B, S, N, H8, W8, iters, stride, has_feat, dev, nhwc=False, peer=None) -> "_GraphPlan":
-        key = (id(w), B, S, N, H8, W8, iters, stride, has_feat, str(dev), nhwc, None if peer is None else peer.key)
+    def _plan(self, w: PackedWeights, B, S, N, H8, W8, iters, stride, has_feat, dev, nhwc=False, peer=None,
+              losses=False) -> "_GraphPlan":
+        key = (id(w), B, S, N, H8, W8, iters, stride, has_feat, str(dev), nhwc, None if peer is None else peer.key, losses)
         plan = self._plans.get(key)
         if plan is None:
             while len(self._plans) >= 2:                          # each plan owns a full workspace
                 self._plans.pop(next(iter(self._plans)))
-            plan = _GraphPlan(self, w, B, S, N, H8, W8, iters, stride, has_feat, dev, nhwc, peer)
+            plan = _GraphPlan(self, w, B, S, N, H8, W8, iters, stride, has_feat, dev, nhwc, peer, losses)
             self._plans[key] = plan
         else:
             self._plans[key] = self._plans.pop(key)               # LRU order
@@ -497,7 +548,7 @@ class _GraphPlan:
     into one graph launch, which is what matters for small problems (demo / chained windows)."""
 
     def __init__(self, eng: RefineEngine, w: PackedWeights, B, S, N, H8, W8, iters, stride, has_feat, dev, nhwc=False,
-                 peer=None):
+                 peer=None, losses=False):
         lib = L.load()
         self.w = w
         self.peer = peer                              # the captured update kernels store into these slabs
@@ -518,11 +569,20 @@ class _GraphPlan:
         eng.times(dev)
 
         self.nhwc = nhwc
+        loss = None
+        if losses:                                    # score-map loss terms: static targets in, per-row partial sums out
+            n_split = lib.pips_scoremap_splits(H8, W8)
+            self.g_hi = torch.zeros(B * S, H8 * W8, LATENT, dtype=torch.bfloat16, device=dev)
+            self.g_lo = torch.zeros_like(self.g_hi)
+            self.target = torch.full((B, S, N), -1, dtype=torch.int32, device=dev)
+            self.neg = torch.zeros(iters, B * S * N, n_split, **f32)
+            self.pos = torch.zeros(iters, B * S * N, **f32)
+            loss = (self.g_hi, self.g_lo, self.target, self.neg, self.pos)
 
         def enqueue():
             return eng._enqueue(lib, w.c, self.pyr, self.ws, self.fmaps_nhwc if nhwc else self.fmaps_nchw, self.c, self.c0,
                                 self.ffeat, self.ffeats, self.feat_in, self.preds, self.vis, B, S, N, H8, W8, iters, stride,
-                                peer=peer)
+                                peer=peer, loss=loss)
 
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
@@ -534,11 +594,14 @@ class _GraphPlan:
         with torch.cuda.graph(self.graph):
             enqueue()
 
-    def run(self, fmaps2d, coords, feat_init):
+    def run(self, fmaps2d, coords, feat_init, loss_target=None):
+        """Replay with new inputs.  A plan captured with losses leaves the partial sums in ``self.neg`` / ``self.pos``."""
         B, N = self.shape
         (self.fmaps_nhwc if self.nhwc else self.fmaps_nchw).copy_(fmaps2d)
         self.c.copy_(coords)
         if self.feat_in is not None:
             self.feat_in.copy_(feat_init)
+        if loss_target is not None:
+            self.target.copy_(loss_target)
         self.graph.replay()
         return self.preds.clone(), self.vis.clone(), self.ffeat.reshape(B, N, LATENT).clone()

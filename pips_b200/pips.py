@@ -15,7 +15,11 @@ Extra, optional knobs (keyword-only; the reference signature is unchanged):
               operands, element-wise stages fused, channels-last), 'fast' (cuDNN TF32 tensor-core
               convolutions over hi/lo-split operands instead), 'x3' (the same cuDNN convolutions through
               eager torch ops) or 'plain' (strict fp32 cuDNN)
-Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET.
+  loss_path   'torch' (default) or 'cuda': where a call WITH ground truth (trajs_g, vis_g, valids) runs when no
+              gradient is wanted.  'torch' is the dense differentiable path (torch_path.forward_torch); 'cuda' runs
+              the encoder and refinement loop of plain inference and computes the score-map loss with
+              pips_scoremap_loss, which never stores the (B,S,iters,N,H8,W8) score maps
+Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET, PIPS_B200_LOSSES.
 """
 from __future__ import annotations
 
@@ -91,7 +95,7 @@ def _conv_math(allow_tf32: bool):
 
 class Pips(nn.Module):
     def __init__(self, S=8, stride=8, *, precision: Optional[str] = None, feat_dtype: Optional[str] = None,
-                 fnet_mode: Optional[str] = None, max_seqs: int = 32768):
+                 fnet_mode: Optional[str] = None, max_seqs: int = 32768, loss_path: Optional[str] = None):
         super().__init__()
         self.S = S
         self.stride = stride
@@ -116,6 +120,10 @@ class Pips(nn.Module):
             raise ValueError("fnet_mode must be 'tc' (wgmma implicit-GEMM convolutions, bf16x3), 'fast' (cuDNN 3xTF32 "
                              "convolutions, channels-last, fused element-wise kernels), 'x3' (3xTF32 convolutions through "
                              "eager torch ops) or 'plain' (strict fp32 cuDNN)")
+        self.loss_path = loss_path or os.environ.get("PIPS_B200_LOSSES", "torch")
+        if self.loss_path not in ("torch", "cuda"):
+            raise ValueError("loss_path must be 'torch' (dense differentiable score maps) or 'cuda' (fused score-map "
+                             "loss kernel, inference only)")
 
     # ------------------------------------------------------------------ configuration
     @property
@@ -186,7 +194,13 @@ class Pips(nn.Module):
         assert (D == 2)
         B, S, C, H, W = rgbs.shape
 
-        slow = trajs_g is not None or is_train or (sw is not None and getattr(sw, "save_this", False))
+        save_this = sw is not None and getattr(sw, "save_this", False)
+        # evaluation with ground truth (test_on_flt.py:87, test_on_crohd.py:133): no gradient wanted, so the score-map
+        # loss can come from the fused kernel instead of the dense score maps -- when loss_path asks for it
+        cuda_losses = (trajs_g is not None and self.loss_path == "cuda" and not is_train and not save_this
+                       and all(t is not None and t.is_cuda for t in (rgbs, trajs_g, vis_g, valids))
+                       and not torch.is_grad_enabled() and (self._shard is None or self._shard[1] == 1))
+        slow = not cuda_losses and (trajs_g is not None or is_train or save_this)
         if slow:
             from .torch_path import forward_torch
             return forward_torch(self, xys, rgbs, coords_init=coords_init, feat_init=feat_init, iters=iters,
@@ -205,6 +219,9 @@ class Pips(nn.Module):
                 fmaps = encode_sharded(self, rgbs)
             else:
                 fmaps = self.encode(rgbs)
+            if cuda_losses:
+                return self.refine(xys, fmaps, coords_init=coords_init, feat_init=feat_init, iters=iters,
+                                   return_feat=return_feat, trajs_g=trajs_g, vis_g=vis_g, valids=valids)
             return self.refine(xys, fmaps, coords_init=coords_init, feat_init=feat_init, iters=iters,
                                return_feat=return_feat)
 
@@ -233,11 +250,25 @@ class Pips(nn.Module):
                                               heat_sel=sel, heat_out=fcps)
         return fcps, [preds[i] for i in range(iters)], vis_e
 
-    def refine(self, xys, fmaps, coords_init=None, feat_init=None, iters=3, return_feat=False):
-        """Everything after fnet (nets/pips.py:450-611) given precomputed feature maps."""
+    def refine(self, xys, fmaps, coords_init=None, feat_init=None, iters=3, return_feat=False, trajs_g=None, vis_g=None,
+               valids=None):
+        """Everything after fnet (nets/pips.py:450-611) given precomputed feature maps.  With ground truth
+        (trajs_g (B,S,N,2) in input pixels, vis_g and valids (B,S,N)) ``losses`` is the reference's
+        (seq_loss, vis_loss, ce_loss) as 0-dim fp32 tensors (nets/pips.py:600-606), without gradients; the score-map
+        loss comes from pips_scoremap_loss.  Not for particle-sharded models."""
         B, N, _ = xys.shape
         S = fmaps.shape[1]
         stride = float(self.stride)
+        loss_target = score = None
+        if trajs_g is not None:
+            from .torch_path import score_map_targets
+            assert tuple(trajs_g.shape) == (B, S, N, 2), "trajs_g must be (B,S,N,2)"
+            assert tuple(vis_g.shape) == (B, S, N) and tuple(valids.shape) == (B, S, N), "vis_g, valids must be (B,S,N)"
+            if self._shard is not None and self._shard[1] > 1:
+                raise RuntimeError("pips_b200.Pips: losses on the CUDA path are not available for particle-sharded models")
+            H8, W8 = fmaps.shape[-2:]
+            loss_target = score_map_targets(trajs_g / stride, vis_g, valids, H8, W8)      # :603
+            score = torch.empty((), dtype=torch.float32, device=fmaps.device)
         xys_ = xys.detach().float() / stride                                            # :450
         if coords_init is None:
             coords = xys_.reshape(B, 1, N, 2).repeat(1, S, 1, 1)                        # :453
@@ -247,7 +278,8 @@ class Pips(nn.Module):
             feat_init = feat_init.detach().float()
 
         if self._shard is None or self._shard[1] == 1:
-            preds, vis_e, ffeat = self._engine.refine(self, fmaps.float(), coords, feat_init, iters, stride)
+            preds, vis_e, ffeat = self._engine.refine(self, fmaps.float(), coords, feat_init, iters, stride,
+                                                      loss_target=loss_target, loss_out=score)
         else:
             from .sharding import refine_sharded
             preds, vis_e, ffeat = refine_sharded(self, fmaps.float(), coords, feat_init, iters, stride)
@@ -257,6 +289,10 @@ class Pips(nn.Module):
         last = coord_predictions[-1] if iters > 0 else start
         coord_predictions2 = [start, start] + coord_predictions + [last, last]          # :474-475, :562-563
         losses = None
+        if trajs_g is not None:                                                         # :600-604
+            from .torch_path import balanced_ce_loss, sequence_loss
+            losses = (sequence_loss(coord_predictions, trajs_g, vis_g, valids, 0.8),
+                      balanced_ce_loss(vis_e, vis_g, valids)[0], score)
         if return_feat:
             return coord_predictions, coord_predictions2, vis_e, ffeat, losses
         return coord_predictions, coord_predictions2, vis_e, losses

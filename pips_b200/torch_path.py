@@ -56,6 +56,17 @@ def score_map_loss(fcps, trajs_g, vis_g, valids):
     return loss
 
 
+def score_map_targets(trajs_g, vis_g, valids, H8, W8):
+    """The rows score_map_loss keeps (nets/pips.py:63-67: rounded half to even, inside the map, valid and visible) and
+    their target pixel y*W8 + x, -1 for every other row: the (B,S,N) int32 targets of pips_scoremap_loss.  trajs_g is
+    in feature-map pixels."""
+    B, S, N, _ = trajs_g.shape
+    xy = trajs_g.reshape(B * S * N, 2).round().long()
+    x, y = xy[:, 0], xy[:, 1]
+    keep = (x >= 0) & (x <= W8 - 1) & (y >= 0) & (y <= H8 - 1) & (valids.reshape(-1) > 0) & (vis_g.reshape(-1) > 0)
+    return torch.where(keep, y * W8 + x, torch.full_like(x, -1)).to(torch.int32).reshape(B, S, N).contiguous()
+
+
 def sample_clamped(im, x, y):
     """utils/samp.py:5-78: bilinear sample with clamped indices and unclamped weights -> (B,N,C)."""
     B, C, H, W = im.shape
