@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define PIPS_B200_ABI_VERSION 3
+#define PIPS_B200_ABI_VERSION 4
 
 enum { PIPS_S = 8, PIPS_C = 128, PIPS_LEVELS = 4, PIPS_RADIUS = 3 };
 enum { PIPS_KITCHEN = 519, PIPS_KITCHEN_PAD = 576, PIPS_DIM = 512, PIPS_HIDDEN = 2048, PIPS_DEPTH = 12, PIPS_HEAD = 1040 };
@@ -167,7 +167,7 @@ int pips_scoremap_loss(const void* G_hi, const void* G_lo, const float* ffeats, 
 int pips_split_bf16(const float* src, void* hi, void* lo, size_t n, void* stream);
 
 /* ---- channels-last element-wise stages of fnet (BasicEncoder, nets/pips.py:131-281; upstream of the loop) ----
- * InstanceNorm2d statistics of y (N, HW, C) NHWC: stats = [N][2][C] (mean, rstd); partial is [N][chunks][2][C] scratch. */
+ * InstanceNorm2d statistics of y (N, HW, C) NHWC: stats = [N][2][C] (mean, rstd); partial is [N][chunks][3][C] scratch. */
 int pips_inorm_stats(const float* y, int N, int HW, int C, float* partial, int chunks, float* stats, void* stream);
 /* out = relu_out?( relu_main?( norm(y) ) + norm?(r) ); written as plain fp32 and/or as the [hi|lo|hi] TF32 split
  * (3*C channels at row stride split_ld) that conv2d_3xtf32 consumes.  stats_y / r / stats_r may be NULL. */
@@ -195,20 +195,22 @@ int pips_conv_tc(const void* x_hi, const void* x_lo, int N, int H, int W, int Cp
 /* 3x3 / stride 1 / pad 1 convolution with 64 input and 64 output channels (BasicEncoder layer1, nets/pips.py:135-136):
  * every input row is loaded once into a ring of row buffers and serves all 9 filter taps (csrc/conv_rows.cu).
  * x_hi/x_lo (N,H,W,64) bf16, w_hi/w_lo (64, 9*64) bf16 [k = (r*3+s)*64 + ci], out (N,H,W,64) fp32.  partial (optional):
- * (N, pips_conv_rows_chunks(H,W), 2, 64) per-chunk (sum, sum of squares) of `out` per channel -- the InstanceNorm
- * statistics (nets/pips.py:154-157), reduced by pips_inorm_finalize. */
+ * (N, pips_conv_rows_chunks(H,W), 3, 64) per-chunk (mean, M2, count) of `out` per channel -- the InstanceNorm
+ * statistics (nets/pips.py:154-157), merged by pips_inorm_finalize. */
 int pips_conv_rows_chunks(int H, int W);
 int pips_conv_rows(const void* x_hi, const void* x_lo, int N, int H, int W, const void* w_hi, const void* w_lo, float* out,
                    float* partial, void* stream);
-/* (mean, 1/sqrt(var + 1e-5)) per (image, channel) from `chunks` partial (sum, sum of squares) rows per image. */
+/* (mean, 1/sqrt(var + 1e-5)) per (image, channel) from `chunks` partial rows per image.  A partial row is three vectors of
+ * C floats: the chunk's mean, M2 (sum of squared deviations from that mean) and pixel count; the counts of an image add up
+ * to HW.  (ABI 4; ABI 3 stored (sum, sum of squares), which cancels catastrophically on flat images.) */
 int pips_inorm_finalize(const float* partial, int N, int chunks, int HW, int C, float* stats, void* stream);
 
 int pips_conv_tc_aniso(const void* x_hi, const void* x_lo, int N, int H, int W, int Cp, const void* w_hi, const void* w_lo,
                        int Cout, int R, int S, int stride_y, int stride_x, int pad_y, int pad_x, const float* bias, float* out,
                        void* stream);
 /* pips_conv_tc_aniso that also accumulates, in its epilogue, the InstanceNorm partial statistics of its output
- * (nets/pips.py:154-157): partial (N, pips_conv_tc_chunks(geometry), 2, Cout) fp32 per-chunk (sum, sum of squares) per
- * channel; the chunking depends on the image geometry only.  Reduce with pips_inorm_finalize. */
+ * (nets/pips.py:154-157): partial (N, pips_conv_tc_chunks(geometry), 3, Cout) fp32 per-chunk (mean, M2, count) per
+ * channel; the chunking depends on the image geometry only.  Merge with pips_inorm_finalize. */
 int pips_conv_tc_chunks(int H, int W, int R, int S, int stride_y, int stride_x, int pad_y, int pad_x);
 int pips_conv_tc_stats(const void* x_hi, const void* x_lo, int N, int H, int W, int Cp, const void* w_hi, const void* w_lo,
                        int Cout, int R, int S, int stride_y, int stride_x, int pad_y, int pad_x, const float* bias, float* out,

@@ -10,7 +10,7 @@ import os
 
 from . import _build
 
-ABI_VERSION = 3            # PIPS_B200_ABI_VERSION of include/pips_b200.h
+ABI_VERSION = 4            # PIPS_B200_ABI_VERSION of include/pips_b200.h
 DEPTH = 12
 LEVELS = 4
 KPAD = 576

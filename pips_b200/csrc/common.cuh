@@ -68,6 +68,21 @@ __device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bflo
     lo = __float2bfloat16_rn(v - __bfloat162float(hi));
 }
 
+// InstanceNorm partial statistics are (count, mean, M2 = sum of squared deviations from the mean): sums of squares
+// about zero cancel catastrophically in q/n - mean^2 when the mean is large against the spread (flat frames), while
+// every term of this pairwise update (Chan, Golub & LeVeque) is non-negative.  (mean, m2) of n values absorbs (mb, m2b)
+// of nb values, with f = nb / (n + nb) and g = n * f (callers that merge many columns of equal counts compute them once).
+__device__ __forceinline__ void chan_merge(float f, float g, float& mean, float& m2, float mb, float m2b) {
+    const float d = mb - mean;
+    mean = fmaf(d, f, mean);
+    m2 += m2b + d * d * g;
+}
+
+__device__ __forceinline__ void chan_merge_n(float n, float& mean, float& m2, float nb, float mb, float m2b) {
+    const float f = nb / (n + nb);
+    chan_merge(f, n * f, mean, m2, mb, m2b);
+}
+
 // two floats -> packed bf16x2 (round to nearest even), `lo_elem` in the low half
 __device__ __forceinline__ uint32_t cvt_bf16x2(float lo_elem, float hi_elem) {
     uint32_t r;

@@ -12,8 +12,8 @@
 //   * all 9 taps' weights (144 KB, hi and lo) are loaded once per CTA and stay resident;
 //   * one consumer warpgroup (wgmma m64n64k16, accumulator in registers) per CTA; a work item is (image, 256-pixel column
 //     block, 8 rows, 128-pixel half "rank"), done as two 64-pixel strips;
-//   * InstanceNorm statistics (nets/pips.py:154-157) are accumulated in the epilogue: per work item one partial (sum, sum
-//     of squares) per channel -- the layout pips_inorm_finalize reduces in fp64, deterministic and independent of the
+//   * InstanceNorm statistics (nets/pips.py:154-157) are accumulated in the epilogue: per work item one partial (mean,
+//     M2, count) per channel -- the layout pips_inorm_finalize merges in fp64, deterministic and independent of the
 //     batch size; the separate statistics pass over the layer-1 activations disappears.
 // Same bf16x3 products (hi*hi + lo*hi + hi*lo, fp32 accumulation) and K order (tap-major, then channel) as conv_tc.cu.
 #include "gemm_common.cuh"
@@ -30,7 +30,7 @@ constexpr uint32_t R_ROW_BYTES = 9 * 1024;           // slot stride (1 KB aligne
 constexpr uint32_t R_W_HALF = 64 * 128, R_W_TAP = 2 * R_W_HALF;   // per tap: [w_hi 64 rows x 128 B | w_lo]
 constexpr uint32_t R_OFF_W = R_RING * 2 * R_ROW_BYTES;            // 72 KB
 constexpr uint32_t R_OFF_COMB = R_OFF_W + 9 * R_W_TAP;            // +144 KB
-constexpr uint32_t R_OFF_BARS = R_OFF_COMB + 4 * 64 * 2 * 4;      // 4 consumer warps x 64 channels x (sum, sum of squares)
+constexpr uint32_t R_OFF_BARS = R_OFF_COMB + 4 * 64 * 2 * 4;      // 4 consumer warps x 64 channels x (mean, M2)
 constexpr uint32_t R_SMEM_BYTES = R_OFF_BARS + 256 + 1024;
 
 struct RowsArgs {
@@ -38,7 +38,7 @@ struct RowsArgs {
     int px_blocks;              // ceil(W / 256)
     int row_chunks;             // ceil(H / R_ROWS_PER_ITEM)
     float* out;                 // (N, H, W, 64) fp32
-    float* partial;             // optional (N, px_blocks * row_chunks * 2, 2, 64)
+    float* partial;             // optional (N, px_blocks * row_chunks * 2, 3, 64)
 };
 
 __global__ void __launch_bounds__(R_THREADS, 1)
@@ -49,6 +49,7 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     float* comb = reinterpret_cast<float*>(smem + R_OFF_COMB);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + R_OFF_BARS);
+    float* counts = reinterpret_cast<float*>(smem + R_OFF_BARS + 128);   // valid pixels per consumer warp and item
     const uint32_t wfull = smem_u32(bars);                 // all 9 taps loaded
     const uint32_t rfull0 = wfull + 8;                     // ring slot filled
     const uint32_t rempty0 = rfull0 + 8 * R_RING;          // ring slot free
@@ -115,8 +116,9 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
             const int img = item / items_img, rem = item - img * items_img;
             const int px = rem / a.row_chunks, chunk = rem - px * a.row_chunks;
             const int y0 = chunk * R_ROWS_PER_ITEM, ntiles = min(a.H, y0 + R_ROWS_PER_ITEM) - y0;
-            // statistics of this thread's columns 8j + 2(lane%4), +1
-            float ssum[8][2], ssq[8][2];
+            // statistics of this thread's columns 8j + 2(lane%4), +1 over its tcount pixels of the item: sums of the
+            // deviations from the first value it sees (a pixel of the same 8-row block, so sums of squares stay small)
+            float shift[8][2], ssum[8][2], ssq[8][2], tcount = 0.f;
 #pragma unroll
             for (int j = 0; j < 8; ++j) { ssum[j][0] = ssum[j][1] = 0.f; ssq[j][0] = ssq[j][1] = 0.f; }
             for (int strip = 0; strip < 2; ++strip) {
@@ -165,12 +167,18 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
                         const int x = xs + w4 * 16 + (lane >> 2) + 8 * h;
                         if (x < a.W) {
                             float* orow = a.out + ((static_cast<size_t>(img) * a.H + (y0 + j)) * a.W + x) * 64 + 2 * (lane & 3);
+                            if (tcount == 0.f) {
+#pragma unroll
+                                for (int c = 0; c < 8; ++c) { shift[c][0] = acc[4 * c + 2 * h]; shift[c][1] = acc[4 * c + 2 * h + 1]; }
+                            }
+                            tcount += 1.f;
 #pragma unroll
                             for (int c = 0; c < 8; ++c) {
                                 const float2 o = make_float2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]);
                                 *reinterpret_cast<float2*>(orow + 8 * c) = o;
-                                ssum[c][0] += o.x; ssum[c][1] += o.y;
-                                ssq[c][0] = fmaf(o.x, o.x, ssq[c][0]); ssq[c][1] = fmaf(o.y, o.y, ssq[c][1]);
+                                const float dx = o.x - shift[c][0], dy = o.y - shift[c][1];
+                                ssum[c][0] += dx; ssum[c][1] += dy;
+                                ssq[c][0] = fmaf(dx, dx, ssq[c][0]); ssq[c][1] = fmaf(dy, dy, ssq[c][1]);
                             }
                         }
                     }
@@ -178,31 +186,57 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
                 base_ld += ntiles + 2;
             }
             if (a.partial) {
-                // totals over the pixels a warp's lanes hold (lanes with equal lane % 4 share columns), then over the
-                // four warps in a fixed order
-                float* mine = comb + w4 * 128;               // [column][sum, squares]
+                // (count, mean, M2) per thread, merged over the 8 lanes that hold the same columns (lane 0..3 keep the
+                // result, always merged in the same order), then over the four warps in a fixed order
+                float* mine = comb + w4 * 128;               // [column][mean, M2]
+                const float inv = tcount > 0.f ? 1.f / tcount : 0.f;
+                float n = tcount;
 #pragma unroll
-                for (int c = 0; c < 8; ++c) {
+                for (int w = 4; w <= 16; w <<= 1) {
+                    const float nb = __shfl_xor_sync(0xffffffffu, n, w);
+                    const float f = n + nb > 0.f ? nb / (n + nb) : 0.f, g = n * f;
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        float s = ssum[c][e], q = ssq[c][e];
+                    for (int c = 0; c < 8; ++c) {
 #pragma unroll
-                        for (int w = 4; w <= 16; w <<= 1) {
-                            s += __shfl_xor_sync(0xffffffffu, s, w);
-                            q += __shfl_xor_sync(0xffffffffu, q, w);
+                        for (int e = 0; e < 2; ++e) {
+                            if (w == 4) {                    // the thread's own (mean, M2) from its shifted sums
+                                const float s = ssum[c][e];
+                                ssum[c][e] = tcount > 0.f ? fmaf(s, inv, shift[c][e]) : 0.f;
+                                ssq[c][e] = fmaxf(ssq[c][e] - s * s * inv, 0.f);
+                            }
+                            const float mb = __shfl_xor_sync(0xffffffffu, ssum[c][e], w);
+                            const float m2b = __shfl_xor_sync(0xffffffffu, ssq[c][e], w);
+                            chan_merge(f, g, ssum[c][e], ssq[c][e], mb, m2b);
                         }
-                        if (lane < 4) {
+                    }
+                    n += nb;
+                }
+                if (lane < 4) {
+#pragma unroll
+                    for (int c = 0; c < 8; ++c) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
                             const int col = 8 * c + 2 * lane + e;
-                            mine[col * 2] = s; mine[col * 2 + 1] = q;
+                            mine[col * 2] = ssum[c][e]; mine[col * 2 + 1] = ssq[c][e];
                         }
                     }
                 }
+                if (lane == 0) counts[w4] = n;
                 asm volatile("bar.sync 1, 128;" ::: "memory");
                 const int col = threadIdx.x - 128;
                 if (col < 64) {
-                    float* p = a.partial + ((static_cast<size_t>(img) * items_img + rem) * 2 + rank) * 128;
-                    p[col] = ((comb[col * 2] + comb[128 + col * 2]) + comb[256 + col * 2]) + comb[384 + col * 2];
-                    p[64 + col] = ((comb[col * 2 + 1] + comb[128 + col * 2 + 1]) + comb[256 + col * 2 + 1]) + comb[384 + col * 2 + 1];
+                    float n = 0.f, mean = 0.f, m2 = 0.f;
+#pragma unroll
+                    for (int w = 0; w < 4; ++w) {
+                        if (counts[w] > 0.f) {
+                            chan_merge_n(n, mean, m2, counts[w], comb[w * 128 + col * 2], comb[w * 128 + col * 2 + 1]);
+                            n += counts[w];
+                        }
+                    }
+                    float* p = a.partial + ((static_cast<size_t>(img) * items_img + rem) * 2 + rank) * 192;
+                    p[col] = mean;
+                    p[64 + col] = m2;
+                    p[128 + col] = n;
                 }
                 asm volatile("bar.sync 1, 128;" ::: "memory");  // comb is rewritten by the next item
             }
@@ -220,7 +254,7 @@ extern "C" int pips_conv_rows_chunks(int H, int W) {
 }
 
 // x_hi/x_lo: (N, H, W, 64) bf16; w_hi/w_lo: (64, 9*64) bf16, k = (r*3 + s)*64 + ci; out: (N, H, W, 64) fp32;
-// partial (optional): (N, pips_conv_rows_chunks(H, W), 2, 64) fp32 per-chunk (sum, sum of squares) of `out` per channel.
+// partial (optional): (N, pips_conv_rows_chunks(H, W), 3, 64) fp32 per-chunk (mean, M2, count) of `out` per channel.
 extern "C" int pips_conv_rows(const void* x_hi, const void* x_lo, int N, int H, int W, const void* w_hi, const void* w_lo,
                               float* out, float* partial, void* stream) {
     if (!x_hi || !x_lo || !w_hi || !w_lo || !out) return fail("pips_conv_rows: null pointer");

@@ -22,8 +22,8 @@ constexpr int C_THREADS = 384;
 constexpr uint32_t C_A_BYTES = 128 * BK * 2;          // 128 pixels x 64 channels bf16
 constexpr int C_MAX_STAGES = 8;
 constexpr uint32_t C_RING_BYTES = 200 * 1024;         // smem ring: stage = A_hi | A_lo | W_hi | W_lo, 2*(16 KB + BN*128 B)
-constexpr uint32_t C_COMB_BYTES = 8 * 8 * 64 * 4;      // statistics exchange: 8 consumer warps x 8 column quarters x (sum, squares) x 32
-constexpr uint32_t C_SMEM_BYTES = C_RING_BYTES + C_COMB_BYTES + 1024 + 256;
+constexpr uint32_t C_COMB_BYTES = 8 * 8 * 64 * 4;      // statistics exchange: 8 consumer warps x 256 columns x (mean, M2)
+constexpr uint32_t C_SMEM_BYTES = C_RING_BYTES + C_COMB_BYTES + 1024 + 256;   // + alignment, barriers and 8 warp counts
 
 struct ConvArgs {
     int N, Ho, Wo, Cout;        // output (NHWC fp32, row stride Cout)
@@ -37,9 +37,9 @@ struct ConvArgs {
     float* out;
     // Work items: the tiles of ONE image in groups of G consecutive pair tiles (pt_img pair tiles per image, groups_img
     // groups).  A group is the unit of the InstanceNorm partial statistics (nets/pips.py:154-157): with `partial` set, the
-    // epilogue accumulates (sum, sum of squares) per output channel over the group's valid pixels and every CTA writes one
-    // row partial[(img * groups_img + g) * 2 + rank][2][Cout] -- a layout fixed by the image geometry alone (never by the
-    // batch), reduced in fp64 by pips_inorm_finalize.
+    // epilogue accumulates (mean, M2, count) per output channel over the group's valid pixels and every CTA writes one
+    // row partial[(img * groups_img + g) * 2 + rank][3][Cout] -- a layout fixed by the image geometry alone (never by the
+    // batch), merged in fp64 by pips_inorm_finalize.
     int G, groups_img, pt_img;
     float* partial;             // optional
 };
@@ -53,6 +53,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     float* comb = reinterpret_cast<float*>(smem + C_RING_BYTES);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_RING_BYTES + C_COMB_BYTES);
+    float* counts = reinterpret_cast<float*>(bars + 2 * C_MAX_STAGES);      // valid pixels per consumer warp and item
     const uint32_t full0 = smem_u32(bars);
     const uint32_t empty0 = full0 + 8 * C_MAX_STAGES;
     const int C_STAGES = a.stages;
@@ -125,8 +126,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
         for (int item = pair; item < num_items; item += num_pairs) {
             const int img = item / a.groups_img, grp = item - img * a.groups_img;
             const int p0 = grp * a.G, p1 = min(a.pt_img, p0 + a.G);
-            // per-warp statistics of the item: mine[column] = (sum, sum of squares) over the warp's pixels
+            // per-warp statistics of the item: mine[column] = (mean, M2) over the warp's wcount valid pixels
             float* mine = comb + (warp - 4) * (BN * 2);
+            float wcount = 0.f;
             if (a.partial) {
                 for (int i = lane; i < BN * 2; i += 32) mine[i] = 0.f;
                 __syncwarp();
@@ -171,46 +173,66 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
                     ok[h] = rem < tiles_img && oy < a.Ho && ox < a.Wo;
                     orow[h] = a.out + ((static_cast<size_t>(img) * a.Ho + oy) * a.Wo + ox) * a.Cout;
                 }
+                // valid pixels among the warp's 16 (each pixel is held by the 4 lanes of a lane / 4 group)
+                const int n16 = (__popc(__ballot_sync(0xffffffffu, ok[0])) + __popc(__ballot_sync(0xffffffffu, ok[1]))) >> 2;
+                const float inv16 = n16 > 0 ? 1.f / n16 : 0.f;
+                const float mf = n16 * (1.f / (wcount + n16)), mg = wcount * mf;    // merge weights, the same for every column
 #pragma unroll
                 for (int j = 0; j < NJ; ++j) {
                     const int col = 8 * j + 2 * (lane & 3);
                     const bool cok = col < a.Cout;                    // Cout is a multiple of 4: column pairs are whole
                     float2 b = make_float2(0.f, 0.f);
                     if (a.bias && cok) b = __ldg(reinterpret_cast<const float2*>(a.bias + col));
-                    float2 s = make_float2(0.f, 0.f), q = make_float2(0.f, 0.f);
+                    float2 o[2], s = make_float2(0.f, 0.f);
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
+                        o[h] = make_float2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
                         if (ok[h] && cok) {
-                            const float2 o = make_float2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
-                            *reinterpret_cast<float2*>(orow[h] + col) = o;
-                            s.x += o.x; s.y += o.y;
-                            q.x = fmaf(o.x, o.x, q.x); q.y = fmaf(o.y, o.y, q.y);
+                            *reinterpret_cast<float2*>(orow[h] + col) = o[h];
+                            s.x += o[h].x; s.y += o[h].y;
                         }
                     }
-                    if (a.partial) {
-                        // totals over the warp's 16 pixels: lanes with equal lane % 4 hold the same columns
+                    if (a.partial && n16 > 0) {
+                        // (mean, M2) over the warp's valid pixels, two passes in registers, merged into the warp's
+                        // running statistics of the item; lanes with equal lane % 4 hold the same columns
 #pragma unroll
-                        for (int w = 4; w <= 16; w <<= 1) {
-                            s.x += __shfl_xor_sync(0xffffffffu, s.x, w); s.y += __shfl_xor_sync(0xffffffffu, s.y, w);
-                            q.x += __shfl_xor_sync(0xffffffffu, q.x, w); q.y += __shfl_xor_sync(0xffffffffu, q.y, w);
+                        for (int w = 4; w <= 16; w <<= 1) { s.x += __shfl_xor_sync(0xffffffffu, s.x, w); s.y += __shfl_xor_sync(0xffffffffu, s.y, w); }
+                        const float2 m = make_float2(s.x * inv16, s.y * inv16);
+                        float2 q = make_float2(0.f, 0.f);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            if (ok[h]) {
+                                const float dx = o[h].x - m.x, dy = o[h].y - m.y;
+                                q.x = fmaf(dx, dx, q.x); q.y = fmaf(dy, dy, q.y);
+                            }
                         }
+#pragma unroll
+                        for (int w = 4; w <= 16; w <<= 1) { q.x += __shfl_xor_sync(0xffffffffu, q.x, w); q.y += __shfl_xor_sync(0xffffffffu, q.y, w); }
                         if (lane < 4 && cok) {
-                            mine[col * 2] += s.x; mine[col * 2 + 1] += q.x;
-                            mine[col * 2 + 2] += s.y; mine[col * 2 + 3] += q.y;
+                            chan_merge(mf, mg, mine[col * 2], mine[col * 2 + 1], m.x, q.x);
+                            chan_merge(mf, mg, mine[col * 2 + 2], mine[col * 2 + 3], m.y, q.y);
                         }
                     }
                 }
+                wcount += static_cast<float>(n16);
             }
             if (a.partial) {
-                // the 8 consumer warps' totals in a fixed order
+                // the 8 consumer warps' statistics merged in a fixed order
+                if (lane == 0) counts[warp - 4] = wcount;
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-                float* p = a.partial + ((static_cast<size_t>(img) * a.groups_img + grp) * 2 + rank) * 2 * a.Cout;
+                float* p = a.partial + ((static_cast<size_t>(img) * a.groups_img + grp) * 2 + rank) * 3 * a.Cout;
                 for (int col = threadIdx.x - 128; col < a.Cout; col += 256) {
-                    float s = 0.f, q = 0.f;
+                    float n = 0.f, mean = 0.f, m2 = 0.f;
 #pragma unroll
-                    for (int w = 0; w < 8; ++w) { s += comb[w * (BN * 2) + col * 2]; q += comb[w * (BN * 2) + col * 2 + 1]; }
-                    p[col] = s;
-                    p[a.Cout + col] = q;
+                    for (int w = 0; w < 8; ++w) {
+                        if (counts[w] > 0.f) {
+                            chan_merge_n(n, mean, m2, counts[w], comb[w * (BN * 2) + col * 2], comb[w * (BN * 2) + col * 2 + 1]);
+                            n += counts[w];
+                        }
+                    }
+                    p[col] = mean;
+                    p[a.Cout + col] = m2;
+                    p[2 * a.Cout + col] = n;
                 }
                 asm volatile("bar.sync 1, 256;" ::: "memory");    // comb is rewritten by the next item
             }
@@ -325,7 +347,7 @@ extern "C" int pips_conv_tc_chunks(int H, int W, int R, int S, int stride_y, int
 }
 
 // pips_conv_tc_aniso that also accumulates the InstanceNorm partial statistics of its output in the epilogue:
-// partial (N, pips_conv_tc_chunks(...), 2, Cout) fp32 = per chunk (sum, sum of squares) per channel, for pips_inorm_finalize.
+// partial (N, pips_conv_tc_chunks(...), 3, Cout) fp32 = per chunk (mean, M2, count) per channel, for pips_inorm_finalize.
 extern "C" int pips_conv_tc_stats(const void* x_hi, const void* x_lo, int N, int H, int W, int Cp, const void* w_hi, const void* w_lo,
                                   int Cout, int R, int S, int stride_y, int stride_x, int pad_y, int pad_x, const float* bias,
                                   float* out, float* partial, void* stream) {

@@ -14,50 +14,65 @@ namespace pips {
 __device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
 
 // ---------------------------------------------------------------------------------------- statistics
-// grid (chunks, N); block 256 threads = (C/4 float4 lanes) x rows; every thread sums its pixels in fp32,
-// rows are combined through smem in a fixed order, chunks by the finalize kernel in fp64: deterministic.
+// Partial statistics: per (image, chunk) three rows of C floats, (mean, M2, count) of the chunk's pixels (chan_merge).
+// grid (chunks, N); block 256 threads = (C/4 float4 lanes) x rows; every thread runs Welford's update over its pixels
+// in fp32, rows are merged through smem in a fixed order, chunks by the finalize kernel in fp64: deterministic.
+__device__ __forceinline__ void welford(float n, float v, float& mean, float& m2) {
+    const float d = v - mean;
+    mean += d / n;
+    m2 = fmaf(d, v - mean, m2);
+}
+
 __global__ void __launch_bounds__(256)
 inorm_partial_kernel(const float* __restrict__ y, int HW, int C, int chunk_px, float* __restrict__ partial) {
-    extern __shared__ float sm[];                       // [rows][2][C]
+    extern __shared__ float sm[];                       // [rows][2][C]: (mean, M2)
     pdl_trigger();
     pdl_wait();
     const int c4n = C >> 2;
     const int lane_c = threadIdx.x % c4n, row = threadIdx.x / c4n, rows = blockDim.x / c4n;
     const int n = blockIdx.y, chunk = blockIdx.x;
     const int p0 = chunk * chunk_px, p1 = min(HW, p0 + chunk_px);
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
     if (row < rows) {
+        float4 m = make_float4(0.f, 0.f, 0.f, 0.f), q = m;
+        float cnt = 0.f;
         const float4* base = reinterpret_cast<const float4*>(y + (static_cast<size_t>(n) * HW) * C) + lane_c;
         for (int p = p0 + row; p < p1; p += rows) {
             const float4 v = base[static_cast<size_t>(p) * c4n];
-            s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-            q.x += v.x * v.x; q.y += v.y * v.y; q.z += v.z * v.z; q.w += v.w * v.w;
+            cnt += 1.f;
+            welford(cnt, v.x, m.x, q.x); welford(cnt, v.y, m.y, q.y); welford(cnt, v.z, m.z, q.z); welford(cnt, v.w, m.w, q.w);
         }
         float* d = sm + (row * 2) * C + lane_c * 4;
-        d[0] = s.x; d[1] = s.y; d[2] = s.z; d[3] = s.w;
+        d[0] = m.x; d[1] = m.y; d[2] = m.z; d[3] = m.w;
         d[C + 0] = q.x; d[C + 1] = q.y; d[C + 2] = q.z; d[C + 3] = q.w;
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
-        float a = 0.f;
-        for (int r = 0; r < rows; ++r) a += sm[r * 2 * C + i];
-        partial[(static_cast<size_t>(n) * gridDim.x + chunk) * 2 * C + i] = a;
+    float* out = partial + (static_cast<size_t>(n) * gridDim.x + chunk) * 3 * C;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        float cnt = 0.f, mean = 0.f, m2 = 0.f;
+        for (int r = 0; r < rows; ++r) {
+            const float nr = static_cast<float>(p1 - p0 - r > 0 ? (p1 - p0 - r + rows - 1) / rows : 0);   // pixels of row r
+            if (nr > 0.f) { chan_merge_n(cnt, mean, m2, nr, sm[r * 2 * C + c], sm[r * 2 * C + C + c]); cnt += nr; }
+        }
+        out[c] = mean; out[C + c] = m2; out[2 * C + c] = cnt;
     }
 }
 
+// (mean, rstd) per (image, channel) from the chunks' (mean, M2, count), merged in fp64
 __global__ void inorm_finalize_kernel(const float* __restrict__ partial, int chunks, int HW, int C, float* __restrict__ stats) {
     const int n = blockIdx.x;
     pdl_trigger();
     pdl_wait();
+    const float* pn = partial + static_cast<size_t>(n) * chunks * 3 * C;
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        double s = 0.0, q = 0.0;
-        for (int k = 0; k < chunks; ++k) {
-            const float* p = partial + (static_cast<size_t>(n) * chunks + k) * 2 * C;
-            s += p[c]; q += p[C + c];
-        }
+        double s = 0.0;
+        for (int k = 0; k < chunks; ++k) s += static_cast<double>(pn[k * 3 * C + 2 * C + c]) * pn[k * 3 * C + c];
         const double mean = s / HW;
-        double var = q / HW - mean * mean;              // biased variance, as InstanceNorm uses for normalisation
-        if (var < 0.0) var = 0.0;
+        double m2 = 0.0;
+        for (int k = 0; k < chunks; ++k) {
+            const double d = static_cast<double>(pn[k * 3 * C + c]) - mean;
+            m2 += pn[k * 3 * C + C + c] + pn[k * 3 * C + 2 * C + c] * d * d;
+        }
+        const double var = m2 / HW;                     // biased variance, as InstanceNorm uses for normalisation
         stats[(static_cast<size_t>(n) * 2) * C + c] = static_cast<float>(mean);
         stats[(static_cast<size_t>(n) * 2 + 1) * C + c] = static_cast<float>(1.0 / sqrt(var + 1e-5));
     }

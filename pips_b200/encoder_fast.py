@@ -62,7 +62,7 @@ class _Ops:
         # partial sums per image: by image size only (never by N: a rank's share of a frame-sharded batch must give
         # the bits of the whole batch); 64 chunks keep even an 8-frame clip at 512 CTAs
         chunks = max(1, min(64, hw // 256))
-        partial = torch.empty(N, chunks, 2, C, dtype=torch.float32, device=self.dev)
+        partial = torch.empty(N, chunks, 3, C, dtype=torch.float32, device=self.dev)
         st = torch.empty(N, 2, C, dtype=torch.float32, device=self.dev)
         L.check(self.lib.pips_inorm_stats(L.ptr(y), N, hw, C, L.ptr(partial), chunks, L.ptr(st), _st()), "pips_inorm_stats")
         LAUNCHES[0] += 2
@@ -178,7 +178,7 @@ def conv_tc(x: _Pair, conv: torch.nn.Conv2d, bias: bool = False, stats: bool = F
         LAUNCHES[0] += 1
         return out
     chunks = lib.pips_conv_tc_chunks(H, W, R, S, st, st, pad, pad)
-    partial = torch.empty(N, chunks, 2, cout, dtype=torch.float32, device=dev)
+    partial = torch.empty(N, chunks, 3, cout, dtype=torch.float32, device=dev)
     stt = torch.empty(N, 2, cout, dtype=torch.float32, device=dev)
     L.check(lib.pips_conv_tc_stats(L.ptr(x.hi), L.ptr(x.lo), N, H, W, x.Cp, L.ptr(w_hi), L.ptr(w_lo), cout, R, S, st, st, pad, pad,
                                    L.ptr(b), L.ptr(out), L.ptr(partial), _st()), "pips_conv_tc_stats")
@@ -206,7 +206,7 @@ def conv_rows(x: _Pair, conv: torch.nn.Conv2d):
     dev = x.hi.device
     out = torch.empty(N, H, W, 64, dtype=torch.float32, device=dev)
     chunks = lib.pips_conv_rows_chunks(H, W)
-    partial = torch.empty(N, chunks, 2, 64, dtype=torch.float32, device=dev)
+    partial = torch.empty(N, chunks, 3, 64, dtype=torch.float32, device=dev)
     st = torch.empty(N, 2, 64, dtype=torch.float32, device=dev)
     L.check(lib.pips_conv_rows(L.ptr(x.hi), L.ptr(x.lo), N, H, W, L.ptr(w_hi), L.ptr(w_lo), L.ptr(out), L.ptr(partial), _st()),
             "pips_conv_rows")
@@ -310,7 +310,7 @@ def _fnet_tc(enc: Encoder, rgb: torch.Tensor) -> torch.Tensor:
     w_hi, w_lo = _packed_stem_weight(enc.conv1)
     y = torch.empty(N, Ho, Wo, 64, dtype=torch.float32, device=rgb.device)
     chunks = lib.pips_conv_tc_chunks(Ho + 3, Wo, 4, 1, 1, 1, 0, 0)
-    partial = torch.empty(N, chunks, 2, 64, dtype=torch.float32, device=rgb.device)
+    partial = torch.empty(N, chunks, 3, 64, dtype=torch.float32, device=rgb.device)
     s_stem = torch.empty(N, 2, 64, dtype=torch.float32, device=rgb.device)
     L.check(lib.pips_conv_tc_stats(L.ptr(unf.hi), L.ptr(unf.lo), N, Ho + 3, Wo, 64, L.ptr(w_hi), L.ptr(w_lo), 64, 4, 1, 1, 1, 0, 0,
                                    None, L.ptr(y), L.ptr(partial), _st()), "pips_conv_tc_stats")

@@ -19,7 +19,7 @@ def test_header_symbols_are_exported():
     for name in declared:
         assert hasattr(lib, name)
     macro = int(re.search(r"#define PIPS_B200_ABI_VERSION (\d+)", hdr).group(1))
-    assert lib.pips_abi_version() == macro == L.ABI_VERSION == 3
+    assert lib.pips_abi_version() == macro == L.ABI_VERSION == 4
 
 
 def test_argument_validation_without_gpu():
