@@ -163,6 +163,22 @@ int pips_scoremap_basis(const float* const* lvl_f32, int frames, int H8, int W8,
 int pips_scoremap_loss(const void* G_hi, const void* G_lo, const float* ffeats, int B, int S, int N, int H8, int W8,
                        const int* target, float* neg_part, float* pos_part, void* stream);
 
+/* Backward of the score-map loss over `iters` iterations (csrc/scoremap_grad.cu), without the dense score maps.
+ * coef (device, 2 floats) holds g/(eps+K) and g/(eps+K(P-1)): g the upstream gradient, K the kept rows times iters,
+ * P = H8*W8, eps = 1e-6.  target is that of pips_scoremap_loss; G_hi / G_lo that of pips_scoremap_basis.  Each output
+ * element is summed in a fixed order (deterministic, no atomics); the score GEMMs run in bf16x3.
+ * pips_scoremap_grad_feats: dffeats = dloss/dffeats, both (iters, B*S, N, 128) fp32 frame-major
+ *   (ffeats[i, b*S+s, n] is the ffeats of track (b, n) in frame s at the start of iteration i).
+ * pips_scoremap_grad_basis: dG = dloss/dG (B*S, H8*W8, 128) fp32, from F_hi / F_lo, the bf16 (hi, lo) split of those
+ *   ffeats (iters, B*S, N, 128).
+ * pips_scoremap_basis_grad: the adjoint of pips_scoremap_basis: dG -> the fp32 channels-last level gradients
+ *   dlvl_f32[l] (B*S, H8>>l, W8>>l, 128). */
+int pips_scoremap_grad_feats(const void* G_hi, const void* G_lo, const float* ffeats, int iters, int B, int S, int N,
+                             int H8, int W8, const int* target, const float* coef, float* dffeats, void* stream);
+int pips_scoremap_grad_basis(const void* G_hi, const void* G_lo, const void* F_hi, const void* F_lo, int iters, int B,
+                             int S, int N, int H8, int W8, const int* target, const float* coef, float* dG, void* stream);
+int pips_scoremap_basis_grad(const float* dG, int frames, int H8, int W8, float* const* dlvl_f32, void* stream);
+
 /* v -> (hi, lo) bf16 with hi = rn(v), lo = rn(v - hi); lo may be NULL.  Used to pack weights. */
 int pips_split_bf16(const float* src, void* hi, void* lo, size_t n, void* stream);
 

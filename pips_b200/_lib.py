@@ -82,6 +82,9 @@ _SIGNATURES = {
     "pips_scoremap_splits": (_i, [_i, _i]),
     "pips_scoremap_basis": (_i, [C.POINTER(_p), _i, _i, _i, _p, _p, _p]),
     "pips_scoremap_loss": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "pips_scoremap_grad_feats": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "pips_scoremap_grad_basis": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "pips_scoremap_basis_grad": (_i, [_p, _i, _i, _i, C.POINTER(_p), _p]),
     "pips_gemm_tc": (_i, [_p, _p, _i, _i, _p, _p, _i, _i, _i, _i, _i, _p, _i, _p, _i, _p, _p, _i, _p]),
     "pips_gemm_f32": (_i, [_p, _i, _p, _i, _i, _i, _i, _p, _i, _p, _i, _p]),
     "pips_tokenmix": (_i, [_p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),

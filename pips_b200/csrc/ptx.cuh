@@ -202,6 +202,22 @@ __device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t a_desc, uin
         : "memory");
 }
 
+// D[64 x 128] (+)= A[64 x 16, registers] * B[16 x 128, smem desc, MN-major], bf16 inputs, fp32 accumulation.  A is held
+// like the mma.m16n8k16 A fragment per warp (rows 16w..16w+15 of the warpgroup): a[0] = (row l/4, columns 2(l%4), +1),
+// a[1] = row + 8, a[2] = columns + 8, a[3] = both -- so the accumulator columns 16k..16k+15 of an earlier wgmma,
+// {d[8k], d[8k+1]}, {d[8k+2], d[8k+3]}, {d[8k+4], d[8k+5]}, {d[8k+6], d[8k+7]} packed to bf16x2, are an A fragment as they are.
+__device__ __forceinline__ void wgmma_n128_rA_tb(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                                 uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, 1;\n\t}"
+        : PIPS_ACC64(d, 0)
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
+
 // 64 x BN tile: BN = 256 as two N = 128 instructions on the two 128-row halves of the B tile (128-byte rows)
 template <int BN>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
@@ -233,6 +249,17 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr) {
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);      // start address, 16 B units
     d |= static_cast<uint64_t>(1) << 16;                          // leading byte offset (unused: one swizzle atom along K)
     d |= static_cast<uint64_t>(512 >> 4) << 32;                   // stride byte offset between 8-row groups
+    d |= static_cast<uint64_t>(2) << 62;                          // SWIZZLE_64B
+    return d;
+}
+// MN-major, 64-byte-swizzled operand (transposed B): the same 64-byte rows as wgmma_desc_sw64, read with the row index as
+// K and the 32 elements of a row as MN.  Each 8-row group of a buffer is one MN-major SW64 atom (32 MN x 8 K); atoms
+// along K are 512 B apart (stride byte offset) and the 32-wide MN blocks are `mn_block_bytes` apart (leading byte offset).
+__device__ __forceinline__ uint64_t wgmma_desc_sw64_mn(uint32_t smem_addr, uint32_t mn_block_bytes) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);      // start address, 16 B units
+    d |= static_cast<uint64_t>((mn_block_bytes >> 4) & 0x3FFF) << 16;   // leading byte offset: next 32 MN elements
+    d |= static_cast<uint64_t>(512 >> 4) << 32;                   // stride byte offset: next 8 K rows
     d |= static_cast<uint64_t>(2) << 62;                          // SWIZZLE_64B
     return d;
 }

@@ -15,10 +15,13 @@ Extra, optional knobs (keyword-only; the reference signature is unchanged):
               operands, element-wise stages fused, channels-last), 'fast' (cuDNN TF32 tensor-core
               convolutions over hi/lo-split operands instead), 'x3' (the same cuDNN convolutions through
               eager torch ops) or 'plain' (strict fp32 cuDNN)
-  loss_path   'torch' (default) or 'cuda': where a call WITH ground truth (trajs_g, vis_g, valids) runs when no
+  loss_path   'torch' (default), 'cuda' or 'fused': where a call WITH ground truth (trajs_g, vis_g, valids) runs when no
               gradient is wanted.  'torch' is the dense differentiable path (torch_path.forward_torch); 'cuda' runs
               the encoder and refinement loop of plain inference and computes the score-map loss with
-              pips_scoremap_loss, which never stores the (B,S,iters,N,H8,W8) score maps
+              pips_scoremap_loss, which never stores the (B,S,iters,N,H8,W8) score maps.  'fused' does what 'cuda' does,
+              and every other call with ground truth (gradients on, is_train=True: train.py) runs the differentiable
+              path with torch_path.fused_score_map_loss, whose forward and backward are CUDA kernels that never build
+              the score maps either (CPU tensors keep the dense loss)
 Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET, PIPS_B200_LOSSES.
 """
 from __future__ import annotations
@@ -121,9 +124,10 @@ class Pips(nn.Module):
                              "convolutions, channels-last, fused element-wise kernels), 'x3' (3xTF32 convolutions through "
                              "eager torch ops) or 'plain' (strict fp32 cuDNN)")
         self.loss_path = loss_path or os.environ.get("PIPS_B200_LOSSES", "torch")
-        if self.loss_path not in ("torch", "cuda"):
-            raise ValueError("loss_path must be 'torch' (dense differentiable score maps) or 'cuda' (fused score-map "
-                             "loss kernel, inference only)")
+        if self.loss_path not in ("torch", "cuda", "fused"):
+            raise ValueError("loss_path must be 'torch' (dense differentiable score maps), 'cuda' (fused score-map "
+                             "loss kernel, inference only) or 'fused' ('cuda', and the fused loss with its CUDA backward "
+                             "on the differentiable path)")
 
     # ------------------------------------------------------------------ configuration
     @property
@@ -197,7 +201,7 @@ class Pips(nn.Module):
         save_this = sw is not None and getattr(sw, "save_this", False)
         # evaluation with ground truth (test_on_flt.py:87, test_on_crohd.py:133): no gradient wanted, so the score-map
         # loss can come from the fused kernel instead of the dense score maps -- when loss_path asks for it
-        cuda_losses = (trajs_g is not None and self.loss_path == "cuda" and not is_train and not save_this
+        cuda_losses = (trajs_g is not None and self.loss_path in ("cuda", "fused") and not is_train and not save_this
                        and all(t is not None and t.is_cuda for t in (rgbs, trajs_g, vis_g, valids))
                        and not torch.is_grad_enabled() and (self._shard is None or self._shard[1] == 1))
         slow = not cuda_losses and (trajs_g is not None or is_train or save_this)

@@ -2,7 +2,9 @@
 cover: ground truth given (losses requested, nets/pips.py:600-606), ``is_train=True`` (no frame-0
 lock, gradients needed) or a summary writer that wants to log this step.  It runs wherever the
 tensors live (it is what ``train.py`` / ``test_on_flt.py`` exercise) and keeps the reference's
-semantics, including the dense score map ``fcps`` that only the score-map loss consumes.
+semantics, including the dense score map ``fcps`` that only the score-map loss consumes -- except with
+``model.loss_path == 'fused'`` on CUDA tensors, where ``fused_score_map_loss`` computes that loss and its gradients
+without ``fcps``.
 
 Not used -- and not a fallback -- for plain inference: that path is CUDA-only (pips.py).
 """
@@ -67,6 +69,95 @@ def score_map_targets(trajs_g, vis_g, valids, H8, W8):
     return torch.where(keep, y * W8 + x, torch.full_like(x, -1)).to(torch.int32).reshape(B, S, N).contiguous()
 
 
+class _FusedScoreMapLoss(torch.autograd.Function):
+    """score_map_loss from the per-iteration ffeats and the pyramid, without the dense score maps, forward and backward
+    on the CUDA kernels of csrc/scoremap_loss.cu and csrc/scoremap_grad.cu.  Saves G (hi, lo), the targets and the
+    ffeats; the backward recomputes the scores tile by tile."""
+
+    @staticmethod
+    def forward(ctx, target, n_iters, *tensors):
+        from . import _lib as L
+        from .engine import _score_map_loss
+        lib = L.load()
+        ffeats, levels = tensors[:n_iters], tensors[n_iters:]
+        B, S, N, C = ffeats[0].shape
+        H8, W8 = levels[0].shape[-2:]
+        P, dev = H8 * W8, ffeats[0].device
+        st = torch.cuda.current_stream(dev).cuda_stream
+        lvls = [lv.detach().float().permute(0, 1, 3, 4, 2).contiguous() for lv in levels]       # channels-last
+        g_hi = torch.empty(B * S, P, C, dtype=torch.bfloat16, device=dev)
+        g_lo = torch.empty_like(g_hi)
+        L.check(lib.pips_scoremap_basis(L.ptr_array(lvls), B * S, H8, W8, L.ptr(g_hi), L.ptr(g_lo), st), "pips_scoremap_basis")
+        del lvls
+        n_split = lib.pips_scoremap_splits(H8, W8)
+        neg = torch.empty(n_iters, B * S * N, n_split, device=dev)
+        pos = torch.empty(n_iters, B * S * N, device=dev)
+        for i, f in enumerate(ffeats):
+            fi = f.detach().float().permute(0, 2, 1, 3).contiguous()        # ((b*N + n), s, c): free for the loop's state
+            L.check(lib.pips_scoremap_loss(L.ptr(g_hi), L.ptr(g_lo), L.ptr(fi), B, S, N, H8, W8, L.ptr(target),
+                                           L.ptr(neg[i]), L.ptr(pos[i]), st), "pips_scoremap_loss")
+        ctx.save_for_backward(g_hi, g_lo, target, *ffeats)
+        ctx.n_iters, ctx.level_shapes = n_iters, [lv.shape for lv in levels]
+        return _score_map_loss(neg, pos, target, n_iters, P)
+
+    @staticmethod
+    def backward(ctx, grad):
+        from . import _lib as L
+        lib = L.load()
+        g_hi, g_lo, target, *ffeats = ctx.saved_tensors
+        I = ctx.n_iters
+        B, S, N, C = ffeats[0].shape
+        H8, W8 = ctx.level_shapes[0][-2:]
+        P, dev = H8 * W8, g_hi.device
+        st = torch.cuda.current_stream(dev).cuda_stream
+        # dloss/dpos and dloss/dneg of engine._score_map_loss, on the device
+        k = (target >= 0).sum().double() * I
+        g = grad.detach().double()
+        coef = torch.stack([g / (1e-6 + k), g / (1e-6 + k * (P - 1))]).float()
+        F_ = torch.stack([f.detach().float() for f in ffeats])            # (I, B, S, N, C): frame-major
+        need_f = any(ctx.needs_input_grad[2:2 + I])
+        need_l = any(ctx.needs_input_grad[2 + I:])
+        dF = None
+        if need_f:
+            dF = torch.empty_like(F_)
+            L.check(lib.pips_scoremap_grad_feats(L.ptr(g_hi), L.ptr(g_lo), L.ptr(F_), I, B, S, N, H8, W8, L.ptr(target),
+                                                 L.ptr(coef), L.ptr(dF), st), "pips_scoremap_grad_feats")
+        dls = [None] * len(ctx.level_shapes)
+        if need_l:
+            f_hi = torch.empty(F_.shape, dtype=torch.bfloat16, device=dev)
+            f_lo = torch.empty_like(f_hi)
+            L.check(lib.pips_split_bf16(L.ptr(F_), L.ptr(f_hi), L.ptr(f_lo), F_.numel(), st), "pips_split_bf16")
+            del F_
+            dG = torch.empty(B * S, P, C, device=dev)
+            L.check(lib.pips_scoremap_grad_basis(L.ptr(g_hi), L.ptr(g_lo), L.ptr(f_hi), L.ptr(f_lo), I, B, S, N, H8, W8,
+                                                 L.ptr(target), L.ptr(coef), L.ptr(dG), st), "pips_scoremap_grad_basis")
+            del f_hi, f_lo
+            dl = [torch.empty(B * S, sh[-2], sh[-1], C, device=dev) for sh in ctx.level_shapes]
+            L.check(lib.pips_scoremap_basis_grad(L.ptr(dG), B * S, H8, W8, L.ptr_array(dl), st), "pips_scoremap_basis_grad")
+            dls = [d.view(B, S, d.shape[1], d.shape[2], C).permute(0, 1, 4, 2, 3) for d in dl]   # logical (B,S,C,h,w)
+        dFs = [None] * I if dF is None else list(dF.unbind(0))
+        return (None, None, *dFs, *dls)
+
+
+def fused_score_map_loss(ffeats_per_iter, pyramid, trajs_g, vis_g, valids):
+    """score_map_loss (nets/pips.py:58-90) of the score maps <ffeats_i, G> without building them, differentiable in the
+    ffeats and the pyramid.  ffeats_per_iter: the I (B,S,N,128) ffeats at the start of each iteration; pyramid: the 4
+    (B,S,128,H8>>l,W8>>l) levels; trajs_g (B,S,N,2) in feature-map pixels, vis_g and valids (B,S,N).  CUDA tensors only.
+    Returns the same 0-dim fp32 loss as score_map_loss, summed in fp64 in a fixed order."""
+    ffeats_per_iter, pyramid = list(ffeats_per_iter), list(pyramid)
+    if not ffeats_per_iter:
+        raise ValueError("fused_score_map_loss: no iterations")
+    if not all(t.is_cuda for t in ffeats_per_iter + pyramid + [trajs_g, vis_g, valids]):
+        raise RuntimeError("fused_score_map_loss runs on the CUDA kernels only; use score_map_loss for CPU tensors")
+    B, S, N, C = ffeats_per_iter[0].shape
+    H8, W8 = pyramid[0].shape[-2:]
+    assert all(tuple(f.shape) == (B, S, N, C) for f in ffeats_per_iter), "every iteration's ffeats must be (B,S,N,128)"
+    assert len(pyramid) == 4 and all(tuple(lv.shape) == (B, S, C, H8 >> l, W8 >> l) for l, lv in enumerate(pyramid)), \
+        "pyramid must be the 4 avg-pooled levels (B,S,128,H8>>l,W8>>l)"
+    target = score_map_targets(trajs_g, vis_g, valids, H8, W8)
+    return _FusedScoreMapLoss.apply(target, len(ffeats_per_iter), *ffeats_per_iter, *pyramid)
+
+
 def sample_clamped(im, x, y):
     """utils/samp.py:5-78: bilinear sample with clamped indices and unclamped weights -> (B,N,C)."""
     B, C, H, W = im.shape
@@ -118,14 +209,21 @@ def forward_torch(model, xys, rgbs, coords_init=None, feat_init=None, iters=3, t
     window = torch.stack(torch.meshgrid(offs, offs, indexing="ij"), dim=-1).view(1, 2 * r + 1, 2 * r + 1, 2)
     times = torch.linspace(0, S, S, device=coords.device).reshape(1, S, 1)
 
-    preds, anim, fcps = [], [coords.detach() * stride] * 2, []
+    # loss_path='fused': the score-map loss comes from fused_score_map_loss over each iteration's starting ffeats, so the
+    # dense score maps fcps (B,S,iters,N,H8,W8) are never built
+    fused = (trajs_g is not None and getattr(model, "loss_path", "torch") == "fused"
+             and all(t.is_cuda for t in (rgbs, trajs_g, vis_g, valids)))
+    preds, anim, fcps, ffeats_per_iter = [], [coords.detach() * stride] * 2, [], []
     for _ in range(iters):
         coords = coords.detach()
         vols = [torch.matmul(ffeats, f.flatten(3)).reshape(B, S, N, *f.shape[-2:]) / torch.sqrt(torch.tensor(float(f.shape[2])))
                 for f in pyramid]                                               # :384-398
-        fcp = sum(F.interpolate(v.flatten(0, 1), (H8, W8), mode="bilinear", align_corners=True).reshape(B, S, N, H8, W8)
-                  for v in vols)                                                # :504-511
-        fcps.append(fcp)
+        if fused:
+            ffeats_per_iter.append(ffeats)
+        else:
+            fcp = sum(F.interpolate(v.flatten(0, 1), (H8, W8), mode="bilinear", align_corners=True).reshape(B, S, N, H8, W8)
+                      for v in vols)                                            # :504-511
+            fcps.append(fcp)
         taps = []
         for i, v in enumerate(vols):                                            # :355-382
             h, w = v.shape[-2:]
@@ -149,7 +247,10 @@ def forward_torch(model, xys, rgbs, coords_init=None, feat_init=None, iters=3, t
     anim += [coords * stride] * 2
 
     losses = None
-    if trajs_g is not None:
+    if fused:
+        losses = (sequence_loss(preds, trajs_g, vis_g, valids, 0.8), balanced_ce_loss(vis_e, vis_g, valids)[0],
+                  fused_score_map_loss(ffeats_per_iter, pyramid, trajs_g / float(stride), vis_g, valids))
+    elif trajs_g is not None:
         fcps_t = torch.stack(fcps, dim=2)
         losses = (sequence_loss(preds, trajs_g, vis_g, valids, 0.8), balanced_ce_loss(vis_e, vis_g, valids)[0],
                   score_map_loss(fcps_t, trajs_g / float(stride), vis_g, valids))
