@@ -41,7 +41,9 @@ enum { PIPS_PREC_F32 = 0,      /* fp32 CUDA-core GEMMs (exact; validation / smal
 /* GEMM epilogues */
 enum { PIPS_EPI_BIAS = 0,        /* out_f32 = acc + bias                                              */
        PIPS_EPI_BIAS_GELU = 1,   /* out    = gelu_erf(acc + bias)  (bf16 hi[/lo] or fp32)             */
-       PIPS_EPI_BIAS_RESID = 2 };/* out_f32 += acc + bias                                             */
+       PIPS_EPI_BIAS_RESID = 2,  /* out_f32 += acc + bias                                             */
+       PIPS_EPI_BIAS_GELU_PRE = 3, /* BIAS_GELU into bf16 hi[/lo], and aux = acc + bias (fp32)         */
+       PIPS_EPI_GELU_GRAD = 4 }; /* out = (acc + bias) * gelu_erf'(aux), bf16 hi[/lo]                 */
 
 int pips_abi_version(void);
 const char* pips_last_error(void);
@@ -77,6 +79,46 @@ int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_rows,
                  const void* w_hi, const void* w_lo, int ldw, int w_rows,
                  int M, int N, int K, const float* bias, int epilogue,
                  float* out_f32, int ldo, void* out_hi, void* out_lo, int ldh, void* stream);
+
+/* pips_gemm_tc with an fp32 side tensor aux (row stride ld_aux) for the two pre-activation epilogues: BIAS_GELU_PRE
+ * also writes the pre-activation acc + bias there (what the GELU backward needs); GELU_GRAD reads it and writes
+ * (acc + bias) * GELU'(aux) with the exact-erf derivative -- the FC2 input gradient of the mixer's backward.  Both need
+ * N % 8 == 0 and an 8-byte aligned aux; the other epilogues ignore aux (may be NULL). */
+int pips_gemm_tc_aux(const void* a_hi, const void* a_lo, int lda, int a_rows,
+                     const void* w_hi, const void* w_lo, int ldw, int w_rows,
+                     int M, int N, int K, const float* bias, int epilogue,
+                     float* out_f32, int ldo, void* out_hi, void* out_lo, int ldh,
+                     float* aux, int ld_aux, void* stream);
+
+/* ---- backward of the DeltaBlock mixer (csrc/gemm_tc.cu, csrc/mixer_grad.cu).  Every sum runs in a fixed order that
+ * depends on the shape only: no atomics, the same bits on any GPU. ----
+ * Weight gradient of a dense layer on the tensor cores, bf16x3: dw[n,k] = sum_m G[m,n] X[m,k] for m < M, with
+ * G (M, N) row stride ldg and X (M, K) row stride ldx as bf16 (hi, lo) pairs; dw (N, K) fp32, dense.  N, K, ldg, ldx
+ * multiples of 8, every pointer 16-byte aligned.  M is split into chunks whose partial sums go to scratch
+ * (pips_wgrad_scratch_floats(M, N, K) floats; may be NULL when that is 0). */
+size_t pips_wgrad_scratch_floats(int M, int N, int K);
+int pips_wgrad(const void* g_hi, const void* g_lo, int ldg, const void* x_hi, const void* x_lo, int ldx, int M, int N, int K,
+               float* scratch, float* dw, void* stream);
+/* column sums out[n] = sum_{m < M} g[m*ld + n]: of fp32 g, or (g == NULL) of the bf16 pair g_hi + g_lo.  The bias
+ * gradients of the dense layers.  scratch: pips_colsum_scratch_floats(M, N) floats (may be NULL when that is 0). */
+size_t pips_colsum_scratch_floats(int M, int N);
+int pips_colsum(const float* g, const void* g_hi, const void* g_lo, size_t ld, int M, int N, float* scratch, float* out,
+                void* stream);
+/* Backward of pips_tokenmix for one mixer block (nets/pips.py:117-118), one sequence of 8 rows x 512 per CTA:
+ * x_in, the block input; x_mid, the residual stream after token mixing (what pips_tokenmix leaves in x); dy, the
+ * gradient of LN2's output.  dx (seqs*8, 512) holds the gradient of the block output on entry and that of the block input
+ * on return (the FC branch's residual included).  grads (2600 floats) receives the parameter gradients:
+ *   ln1_w[512] ln1_b[512] tok_w1[32*8] tok_b1[32] tok_w2[8*32] tok_b2[8] ln2_w[512] ln2_b[512].
+ * scratch: pips_tokenmix_grad_scratch_floats(seqs) floats. */
+size_t pips_tokenmix_grad_scratch_floats(int seqs);
+int pips_tokenmix_grad(const float* x_in, const float* x_mid, const float* dy, float* dx, int seqs, const float* ln1_w,
+                       const float* ln1_b, const float* w1, const float* b1, const float* w2, const float* b2,
+                       const float* ln2_w, const float* ln2_b, float* scratch, float* grads, void* stream);
+/* Backward of pips_ln_pool: dp (seqs, 512), the gradient of the pooled rows -> dx (seqs*8, 512), and the LayerNorm's
+ * parameter gradients grads = ln_w[512] ln_b[512].  scratch: pips_ln_pool_grad_scratch_floats(seqs) floats. */
+size_t pips_ln_pool_grad_scratch_floats(int seqs);
+int pips_ln_pool_grad(const float* x, const float* dp, int seqs, const float* ln_w, const float* ln_b, float* dx,
+                      float* scratch, float* grads, void* stream);
 
 /* the same contract in fp32 on CUDA cores (PIPS_PREC_F32) */
 int pips_gemm_f32(const float* a, int lda, const float* w, int ldw, int M, int N, int K,

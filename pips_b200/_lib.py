@@ -21,7 +21,7 @@ HEAD_PAD = 1280
 
 FEAT_F32, FEAT_BF16 = 0, 1
 PREC_F32, PREC_BF16X3, PREC_BF16 = 0, 1, 2
-EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_RESID = 0, 1, 2
+EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_RESID, EPI_BIAS_GELU_PRE, EPI_GELU_GRAD = 0, 1, 2, 3, 4
 
 PRECISIONS = {"fp32": PREC_F32, "bf16x3": PREC_BF16X3, "bf16": PREC_BF16}
 FEAT_DTYPES = {"fp32": FEAT_F32, "bf16": FEAT_BF16}
@@ -86,6 +86,15 @@ _SIGNATURES = {
     "pips_scoremap_grad_basis": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "pips_scoremap_basis_grad": (_i, [_p, _i, _i, _i, C.POINTER(_p), _p]),
     "pips_gemm_tc": (_i, [_p, _p, _i, _i, _p, _p, _i, _i, _i, _i, _i, _p, _i, _p, _i, _p, _p, _i, _p]),
+    "pips_gemm_tc_aux": (_i, [_p, _p, _i, _i, _p, _p, _i, _i, _i, _i, _i, _p, _i, _p, _i, _p, _p, _i, _p, _i, _p]),
+    "pips_wgrad_scratch_floats": (C.c_size_t, [_i, _i, _i]),
+    "pips_wgrad": (_i, [_p, _p, _i, _p, _p, _i, _i, _i, _i, _p, _p, _p]),
+    "pips_colsum_scratch_floats": (C.c_size_t, [_i, _i]),
+    "pips_colsum": (_i, [_p, _p, _p, C.c_size_t, _i, _i, _p, _p, _p]),
+    "pips_tokenmix_grad_scratch_floats": (C.c_size_t, [_i]),
+    "pips_tokenmix_grad": (_i, [_p, _p, _p, _p, _i] + [_p] * 8 + [_p, _p, _p]),
+    "pips_ln_pool_grad_scratch_floats": (C.c_size_t, [_i]),
+    "pips_ln_pool_grad": (_i, [_p, _p, _i, _p, _p, _p, _p, _p, _p]),
     "pips_gemm_f32": (_i, [_p, _i, _p, _i, _i, _i, _i, _p, _i, _p, _i, _p]),
     "pips_tokenmix": (_i, [_p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "pips_tokenmix_tc": (_i, [_p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),

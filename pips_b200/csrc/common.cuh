@@ -95,6 +95,11 @@ __device__ __forceinline__ float gelu_exact(float v) {
     return 0.5f * v * (1.0f + erff(v * 0.70710678118654752440f));
 }
 
+// d/dx of the exact GELU: Phi(x) + x phi(x), with erfc so that the negative tail keeps its relative accuracy
+__device__ __forceinline__ float gelu_grad_exact(float v) {
+    return 0.5f * erfcf(-v * 0.70710678118654752440f) + v * 0.39894228040143267794f * expf(-0.5f * v * v);
+}
+
 // GELU(x) = x * Phi(x) with Phi(-|x|) = 0.5 erfc(|x|/sqrt2) ~= 0.5 (a1 t + ... + a6 t^6) exp(-x^2/2),
 // t = 1/(1 + p |x|/sqrt2): a 6-term Abramowitz-Stegun-form fit (max error of the fit 7.8e-9, about
 // 4e-7 relative after fp32 evaluation -- the same class as an erff-based evaluation, ~12 instructions

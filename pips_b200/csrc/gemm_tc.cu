@@ -59,11 +59,19 @@ struct GemmArgs {
     int epilogue;                // PIPS_EPI_*
     float* out_f32;              // BIAS / BIAS_RESID target (row stride ldo)
     int ldo;
-    __nv_bfloat16* out_hi;       // BIAS_GELU target (row stride ldh); out_lo may be null
+    __nv_bfloat16* out_hi;       // BIAS_GELU / _PRE / GELU_GRAD target (row stride ldh); out_lo may be null
     __nv_bfloat16* out_lo;
     int ldh;
     int num_tiles;               // output tiles of the launched variant (set by its launcher)
+    // the fields below are read by the aux and weight-gradient variants only
+    float* aux;                  // BIAS_GELU_PRE: pre-activation out; GELU_GRAD: pre-activation in (row stride ld_aux)
+    int ld_aux;
+    int kb_per_split;            // weight-gradient variant: K-blocks (32 rows of M) per split of M
 };
+
+__host__ __device__ __forceinline__ bool bf16_epilogue(int epi) {
+    return epi == PIPS_EPI_BIAS_GELU || epi == PIPS_EPI_BIAS_GELU_PRE || epi == PIPS_EPI_GELU_GRAD;
+}
 
 struct GemmMaps {
     CUtensorMap a_hi, a_lo, w_hi, w_lo;    // operands: {KB, rows} boxes, 64-byte swizzle
@@ -89,7 +97,9 @@ __device__ __forceinline__ uint32_t staged(int row, int byte) {
 // Epilogue of a warpgroup's 64 x BN accumulator (wgmma fragment layout, ptx.cuh).  `row0` is the first of the
 // warpgroup's rows, `n0` the tile's first column, `staging` its two EPI_BUF_BYTES buffers; `chunk` counts the chunks
 // this warpgroup has staged so far (it picks the buffer and tells when a buffer has had a store issued from it).
-template <int BN>
+// AUX: the pre-activation epilogues (BIAS_GELU_PRE, GELU_GRAD) -- a separate instantiation, so the plain ones keep
+// their registers.
+template <int BN, bool AUX = false>
 __device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArgs& args, const float (&acc)[BN / 2], int row0,
                                              int n0, uint32_t staging, uint32_t& chunk, int wg) {
     if (row0 >= args.M) return;                                           // whole warpgroup past M: nothing to store
@@ -97,7 +107,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArg
     const int r = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);           // fragment rows r, r + 8 of the 64
     const int cq = 2 * (lane & 3);                                        // fragment columns cq, cq + 1 of each 8
     const bool issuer = (threadIdx.x & 127) == 0;
-    const bool gelu = args.epilogue == PIPS_EPI_BIAS_GELU;
+    const bool gelu = AUX ? bf16_epilogue(args.epilogue) : args.epilogue == PIPS_EPI_BIAS_GELU;
 #pragma unroll
     for (int c = 0; c < BN / EPI_COLS; ++c) {
         const int col0 = n0 + c * EPI_COLS;
@@ -114,7 +124,22 @@ __device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArg
             for (int h = 0; h < 2; ++h) {
                 const float2 f = add2(make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]), b);
                 if (gelu) {
-                    const float2 g = gelu_fast2_abs(f);
+                    float2 g;
+                    if constexpr (AUX) {
+                        // the aux epilogues require N % 8 == 0, so col < N covers col + 1
+                        const int row = row0 + r + 8 * h;
+                        const bool inside = row < args.M && col < args.N;
+                        float* aux = args.aux + static_cast<size_t>(row) * args.ld_aux + col;
+                        if (args.epilogue == PIPS_EPI_GELU_GRAD) {
+                            const float2 pre = inside ? __ldg(reinterpret_cast<const float2*>(aux)) : make_float2(0.f, 0.f);
+                            g = mul2(f, make_float2(gelu_grad_exact(pre.x), gelu_grad_exact(pre.y)));
+                        } else {
+                            g = gelu_fast2_abs(f);
+                            if (inside) *reinterpret_cast<float2*>(aux) = f;
+                        }
+                    } else {
+                        g = gelu_fast2_abs(f);
+                    }
                     const uint32_t hw = cvt_bf16x2(g.x, g.y);
                     const uint32_t o = staged<EPI_COLS * 2>(r + 8 * h, (8 * jj + cq) * 2);
                     st_shared_u32(buf + o, hw);
@@ -144,12 +169,38 @@ __device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArg
     }
 }
 
-template <int TERMS, int BN, int CLUSTER>
+// Weight-gradient epilogue: the warpgroup's 64 x 128 fp32 partial sum of one split of M goes straight from registers to
+// its slice of the output (rows n, columns k, row stride args.ldo); rows >= N and columns >= K are not stored.
+__device__ __forceinline__ void epilogue_wgrad(const GemmArgs& args, const float (&acc)[64], float* out, int row0, int k0) {
+    const int lane = threadIdx.x & 31;
+    const int r = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int n = row0 + r + 8 * h;
+        if (n >= args.N) continue;
+        float* o = out + static_cast<size_t>(n) * args.ldo;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const int k = k0 + 8 * j + cq;                                // K % 8 == 0: k < K covers k + 1
+            if (k < args.K) *reinterpret_cast<float2*>(o + k) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
+    }
+}
+
+// WGRAD = false: C = epi(A . W^T + bias), K-major operands (above).
+// WGRAD = true:  the weight gradient dW[N,K] = sum_m G[m,n] X[m,k] (maps a_* over G, w_* over X; both row-major with m as
+// the row, so both are read MN-major).  A ring stage holds 32 rows of m: the 128 n of the tile as four {32 n, 32 m}
+// boxes and the 128 k as four more, each box one stack of MN-major SW64 atoms.  A tile is (n block, k block, split of M);
+// each split's partial sum goes to its own slice of args.out_f32 (N*K floats apart) and is summed in a fixed order later.
+template <int TERMS, int BN, int CLUSTER, bool WGRAD = false, bool AUX = false>
 __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArgs& args) {
     using Cfg = GemmCfg<TERMS, BN>;
     constexpr int kStages = Cfg::kStages;
     constexpr uint32_t W_TILE_BYTES = Cfg::kWTileBytes;
+    constexpr uint32_t BOX_BYTES = 32 * KB * 2;                    // WGRAD: one {32, 32} box, 2 KB
     static_assert(CLUSTER == 1 || BN == 256, "cluster tiles are 256 columns wide");
+    static_assert(!WGRAD || (BN == 128 && CLUSTER == 1 && TERMS == 3), "the weight-gradient variant is bf16x3, 128 x 128");
     extern __shared__ uint8_t smem_raw[];
     // the 128-byte-swizzled staging buffers need 1024-byte alignment (the 64-byte-swizzled ring needs 512)
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -165,8 +216,24 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
     pdl_trigger();
 
     constexpr int TM = BM * CLUSTER;
-    const int tiles_n = (args.N + BN - 1) / BN;
-    const int num_kb = args.K / KB;
+    // C = A . W^T: tiles (m block, n block), all of K.  WGRAD: tiles (n block, k block, split of M), the split's K-blocks.
+    const int tiles_n = WGRAD ? (args.K + BN - 1) / BN : (args.N + BN - 1) / BN;
+    const int total_kb = WGRAD ? (args.M + KB - 1) / KB : args.K / KB;
+    const int splits = WGRAD ? (total_kb + args.kb_per_split - 1) / args.kb_per_split : 1;
+    // tile t -> first output row (m, or n), first output column (n, or k), K-block range
+    auto tile_coords = [&](int t, int& row0, int& col0, int& kb0, int& kb1) {
+        if constexpr (WGRAD) {
+            const int s = t % splits;
+            t /= splits;
+            kb0 = s * args.kb_per_split;
+            kb1 = min(total_kb, kb0 + args.kb_per_split);
+        } else {
+            kb0 = 0;
+            kb1 = total_kb;
+        }
+        row0 = (t / tiles_n) * TM + static_cast<int>(rank) * BM;
+        col0 = (t % tiles_n) * BN;
+    };
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&maps.a_hi);
@@ -175,7 +242,8 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
             tma_prefetch_desc(&maps.a_lo);
             tma_prefetch_desc(&maps.w_lo);
         }
-        if (args.epilogue == PIPS_EPI_BIAS_GELU) {
+        if (WGRAD) {
+        } else if (AUX ? bf16_epilogue(args.epilogue) : args.epilogue == PIPS_EPI_BIAS_GELU) {
             tma_prefetch_desc(&maps.out_hi);
             if (args.out_lo) tma_prefetch_desc(&maps.out_lo);
         } else {
@@ -200,14 +268,25 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
             // ------------------------------------------------------------ TMA producer
             uint32_t stage = 0, phase = 0;
             for (int t = worker; t < args.num_tiles; t += num_workers) {
-                const int m0 = (t / tiles_n) * TM + static_cast<int>(rank) * BM;
-                const int n0 = (t % tiles_n) * BN;
-                for (int kb = 0; kb < num_kb; ++kb) {
+                int m0, n0, kb0, kb1;
+                tile_coords(t, m0, n0, kb0, kb1);
+                for (int kb = kb0; kb < kb1; ++kb) {
                     mbar_wait(empty0 + 8 * stage, phase ^ 1);
                     const uint32_t fb = full0 + 8 * stage;
                     mbar_arrive_expect_tx(fb, Cfg::kStageBytes);
                     const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
                     const int k0 = kb * KB;
+                    if constexpr (WGRAD) {                    // m0: first n of the tile, n0: first k, k0: first m
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            tma_load_2d(base + i * BOX_BYTES, &maps.a_hi, fb, m0 + 32 * i, k0);
+                            tma_load_2d(base + A_TILE_BYTES + i * BOX_BYTES, &maps.w_hi, fb, n0 + 32 * i, k0);
+                            tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES + i * BOX_BYTES, &maps.a_lo, fb, m0 + 32 * i, k0);
+                            tma_load_2d(base + 2 * A_TILE_BYTES + W_TILE_BYTES + i * BOX_BYTES, &maps.w_lo, fb, n0 + 32 * i, k0);
+                        }
+                        if (++stage == kStages) { stage = 0; phase ^= 1; }
+                        continue;
+                    }
                     tma_load_2d(base, &maps.a_hi, fb, k0, m0);
                     if (TERMS == 3) tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES, &maps.a_lo, fb, k0, m0);
                     if (CLUSTER == 2) {
@@ -235,24 +314,41 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
         float acc[BN / 2];
         uint32_t stage = 0, phase = 0;
         for (int t = worker; t < args.num_tiles; t += num_workers) {
-            const int m0 = (t / tiles_n) * TM + static_cast<int>(rank) * BM;
-            const int n0 = (t % tiles_n) * BN;
+            int m0, n0, kb0, kb1;
+            tile_coords(t, m0, n0, kb0, kb1);
             int prev = -1;                                   // ring slot whose MMAs are still in flight
-            for (int kb = 0; kb < num_kb; ++kb) {
+            for (int kb = kb0; kb < kb1; ++kb) {
                 mbar_wait(full0 + 8 * stage, phase);
                 const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
-                const uint64_t a_hi = wgmma_desc_sw64(base + wg * (A_TILE_BYTES / 2));
-                const uint64_t w_hi = wgmma_desc_sw64(base + A_TILE_BYTES);
-                const uint64_t a_lo = wgmma_desc_sw64(base + A_TILE_BYTES + W_TILE_BYTES + wg * (A_TILE_BYTES / 2));
-                const uint64_t w_lo = wgmma_desc_sw64(base + 2 * A_TILE_BYTES + W_TILE_BYTES);
-                wgmma_fence();
+                if constexpr (WGRAD) {
+                    wgmma_fence();
+                    // the warpgroup's 64 n are the boxes 2wg, 2wg + 1; a K=16 step is 16 rows of m = 1 KB into every box
+                    const uint32_t a_hi = base + wg * 2 * BOX_BYTES, w_hi = base + A_TILE_BYTES;
+                    const uint32_t a_lo = a_hi + A_TILE_BYTES + W_TILE_BYTES, w_lo = w_hi + A_TILE_BYTES + W_TILE_BYTES;
 #pragma unroll
-                for (int k = 0; k < KB / MMA_K; ++k) {
-                    const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);   // 32 B per K=16 step
-                    gemm_mma<BN>(acc, a_hi + adv, w_hi + adv, (kb | k) != 0);
-                    if (TERMS == 3) {
-                        gemm_mma<BN>(acc, a_lo + adv, w_hi + adv, 1);
-                        gemm_mma<BN>(acc, a_hi + adv, w_lo + adv, 1);
+                    for (int k = 0; k < KB / MMA_K; ++k) {
+                        const uint64_t ah = wgmma_desc_sw64_mn(a_hi + k * 1024, BOX_BYTES);
+                        const uint64_t al = wgmma_desc_sw64_mn(a_lo + k * 1024, BOX_BYTES);
+                        const uint64_t wh = wgmma_desc_sw64_mn(w_hi + k * 1024, BOX_BYTES);
+                        const uint64_t wl = wgmma_desc_sw64_mn(w_lo + k * 1024, BOX_BYTES);
+                        wgmma_n128_tt(*reinterpret_cast<float(*)[64]>(&acc[0]), ah, wh, (kb != kb0) | k);
+                        wgmma_n128_tt(*reinterpret_cast<float(*)[64]>(&acc[0]), al, wh, 1);
+                        wgmma_n128_tt(*reinterpret_cast<float(*)[64]>(&acc[0]), ah, wl, 1);
+                    }
+                } else {
+                    const uint64_t a_hi = wgmma_desc_sw64(base + wg * (A_TILE_BYTES / 2));
+                    const uint64_t w_hi = wgmma_desc_sw64(base + A_TILE_BYTES);
+                    const uint64_t a_lo = wgmma_desc_sw64(base + A_TILE_BYTES + W_TILE_BYTES + wg * (A_TILE_BYTES / 2));
+                    const uint64_t w_lo = wgmma_desc_sw64(base + 2 * A_TILE_BYTES + W_TILE_BYTES);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < KB / MMA_K; ++k) {
+                        const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);   // 32 B per K=16 step
+                        gemm_mma<BN>(acc, a_hi + adv, w_hi + adv, (kb | k) != 0);
+                        if (TERMS == 3) {
+                            gemm_mma<BN>(acc, a_lo + adv, w_hi + adv, 1);
+                            gemm_mma<BN>(acc, a_hi + adv, w_lo + adv, 1);
+                        }
                     }
                 }
                 wgmma_commit();
@@ -272,7 +368,13 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
                 mbar_arrive(empty0 + 8 * prev);
                 if (CLUSTER == 2) mbar_arrive_cluster(empty0 + 8 * prev, rank ^ 1);
             }
-            epilogue_tma<BN>(maps, args, acc, m0 + wg * 64, n0, my_staging, chunk, wg);
+            if constexpr (WGRAD) {
+                const int split = t % splits;
+                float* out = args.out_f32 + static_cast<size_t>(split) * args.N * args.ldo;
+                epilogue_wgrad(args, *reinterpret_cast<const float(*)[64]>(&acc[0]), out, m0 + wg * 64, n0);
+            } else {
+                epilogue_tma<BN, AUX>(maps, args, acc, m0 + wg * 64, n0, my_staging, chunk, wg);
+            }
         }
         if (releaser) bulk_wait<0>();                        // the last stores have finished reading shared memory and writing
     }
@@ -290,6 +392,20 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_pair_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs args) {
     gemm_tc_body<TERMS, 256, 2>(maps, args);
 }
+
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_tc_aux_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs args) {
+    gemm_tc_body<3, 128, 1, false, true>(maps, args);
+}
+
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+wgrad_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs args) {
+    gemm_tc_body<3, 128, 1, true>(maps, args);
+}
+
+// Rows of M per split of the weight-gradient GEMM.  The layer shapes give 20..64 output tiles of 128 x 128, too few for the
+// SMs; splitting M fills them.  A constant, so the partial sums -- and the bits -- depend on the shape only.
+constexpr int WG_SPLIT_ROWS = 2048;
 
 // ---------------------------------------------------------------------------------- host side
 
@@ -326,7 +442,7 @@ static const char* make_maps(GemmMaps* m, bool x3, const void* a_hi, const void*
         if (!make_operand_map(&m->a_lo, a_lo, a_rows, args.K, lda, BM)) return "tensor map (A lo) failed";
         if (!make_operand_map(&m->w_lo, w_lo, w_rows, args.K, ldw, w_box_rows)) return "tensor map (W lo) failed";
     }
-    if (args.epilogue == PIPS_EPI_BIAS_GELU) {
+    if (bf16_epilogue(args.epilogue)) {
         if (!make_output_map(&m->out_hi, args.out_hi, args, args.ldh, false)) return "tensor map (out hi) failed";
         if (args.out_lo && !make_output_map(&m->out_lo, args.out_lo, args, args.ldh, false)) return "tensor map (out lo) failed";
     } else if (!make_output_map(&m->out_f32, args.out_f32, args, args.ldo, true)) {
@@ -350,6 +466,9 @@ int launch_single(int bn, bool x3, const void* a_hi, const void* a_lo, int lda, 
 int launch_pair(bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo, int ldw,
                 int w_rows, const GemmArgs& args, cudaStream_t st);
 
+int launch_aux(const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo, int ldw, int w_rows,
+               const GemmArgs& args, cudaStream_t st);
+
 static bool use_pair_kernel() {
     static int v = -1;
     if (v < 0) {
@@ -368,6 +487,15 @@ extern "C" int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_r
                             int M, int N, int K, const float* bias, int epilogue,
                             float* out_f32, int ldo, void* out_hi, void* out_lo, int ldh,
                             void* stream) {
+    return pips_gemm_tc_aux(a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, M, N, K, bias, epilogue, out_f32, ldo, out_hi,
+                            out_lo, ldh, nullptr, 0, stream);
+}
+
+extern "C" int pips_gemm_tc_aux(const void* a_hi, const void* a_lo, int lda, int a_rows,
+                                const void* w_hi, const void* w_lo, int ldw, int w_rows,
+                                int M, int N, int K, const float* bias, int epilogue,
+                                float* out_f32, int ldo, void* out_hi, void* out_lo, int ldh,
+                                float* aux, int ld_aux, void* stream) {
     if (K % BK != 0 || K <= 0) return fail("pips_gemm_tc: K must be a positive multiple of 64");
     if (M <= 0 || N <= 0) return fail("pips_gemm_tc: empty problem");
     if (a_rows < M || w_rows < N) return fail("pips_gemm_tc: operand allocations smaller than the problem");
@@ -375,8 +503,14 @@ extern "C" int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_r
     if (!bias) return fail("pips_gemm_tc: bias is required");
     const bool x3 = a_lo != nullptr && w_lo != nullptr;
     if ((a_lo != nullptr) != (w_lo != nullptr)) return fail("pips_gemm_tc: need both or neither lo operands");
-    if (epilogue == PIPS_EPI_BIAS_GELU) {
+    if (bf16_epilogue(epilogue)) {
         if (!out_hi || (ldh % 8)) return fail("pips_gemm_tc: GELU epilogue needs out_hi with ldh % 8 == 0");
+        if (epilogue != PIPS_EPI_BIAS_GELU) {
+            if (!aux || (reinterpret_cast<uintptr_t>(aux) & 7) || ld_aux < N || (ld_aux % 2) || (N % 8))
+                return fail("pips_gemm_tc: the pre-activation epilogues need an 8-byte aligned aux with ld_aux >= N, "
+                            "ld_aux % 2 == 0, and N % 8 == 0");
+            if (!x3) return fail("pips_gemm_tc: the pre-activation epilogues are bf16x3 only (a_lo and w_lo required)");
+        }
     } else if (epilogue == PIPS_EPI_BIAS || epilogue == PIPS_EPI_BIAS_RESID) {
         if (!out_f32 || (ldo % 4)) return fail("pips_gemm_tc: fp32 epilogue needs out_f32 with ldo % 4 == 0");
     } else {
@@ -386,11 +520,14 @@ extern "C" int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_r
     args.M = M; args.N = N; args.K = K; args.bias = bias; args.epilogue = epilogue;
     args.out_f32 = out_f32; args.ldo = ldo;
     args.out_hi = static_cast<__nv_bfloat16*>(out_hi); args.out_lo = static_cast<__nv_bfloat16*>(out_lo); args.ldh = ldh;
+    args.aux = aux; args.ld_aux = ld_aux;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // Tile shape.  Every variant accumulates each output element over K in the same order (same MMA K-steps, same
     // hi/lo term order), so the choice changes the schedule, not the bits (tests/test_kernels_gpu.py).
     //   pair  256x256 per cluster of two CTAs (W multicast): least operand traffic; needs enough pair tiles to fill the GPU
     //   128 x {256,128,64} single CTA: when 256-wide tiles would leave most SMs idle (few particles)
+    if (epilogue == PIPS_EPI_BIAS_GELU_PRE || epilogue == PIPS_EPI_GELU_GRAD)
+        return launch_aux(a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, args, st);
     const int force = forced_tile();                  // PIPS_B200_GEMM_TILE = pair | 256 | 128 | 64 (tests, profiling)
     const bool pair_ok = use_pair_kernel() && M > 128 && (a_rows % 256) == 0 && (w_rows % 256) == 0;
     const int pair_tiles = ((M + 255) / 256) * ((N + 255) / 256);
@@ -407,6 +544,53 @@ extern "C" int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_r
     if (pair)
         return launch_pair(x3, a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, args, st);
     return launch_single(bn, x3, a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, args, st);
+}
+
+namespace pips {
+int colsum_launch(const float* g, const void* g_hi, const void* g_lo, size_t ld, int M, int N, float* scratch, float* out,
+                  cudaStream_t st);   // mixer_grad.cu
+}  // namespace pips
+
+extern "C" size_t pips_wgrad_scratch_floats(int M, int N, int K) {
+    if (M <= 0 || N <= 0 || K <= 0) return 0;
+    const size_t splits = (static_cast<size_t>(M) + WG_SPLIT_ROWS - 1) / WG_SPLIT_ROWS;
+    return splits > 1 ? splits * N * K : 0;
+}
+
+extern "C" int pips_wgrad(const void* g_hi, const void* g_lo, int ldg, const void* x_hi, const void* x_lo, int ldx, int M, int N,
+                          int K, float* scratch, float* dw, void* stream) {
+    if (!g_hi || !g_lo || !x_hi || !x_lo || !dw) return fail("pips_wgrad: null pointer");
+    if (M <= 0 || N <= 0 || K <= 0) return fail("pips_wgrad: empty problem");
+    if ((N % 8) || (K % 8) || ldg < N || ldx < K || (ldg % 8) || (ldx % 8))
+        return fail("pips_wgrad: N and K must be multiples of 8, ldg >= N and ldx >= K multiples of 8");
+    if ((reinterpret_cast<uintptr_t>(g_hi) | reinterpret_cast<uintptr_t>(g_lo) | reinterpret_cast<uintptr_t>(x_hi)
+         | reinterpret_cast<uintptr_t>(x_lo) | reinterpret_cast<uintptr_t>(dw) | reinterpret_cast<uintptr_t>(scratch)) & 15)
+        return fail("pips_wgrad: operands, scratch and dw must be 16-byte aligned");
+    const int splits = (M + WG_SPLIT_ROWS - 1) / WG_SPLIT_ROWS;
+    if (static_cast<long long>(N) * K > 0x7fffffffLL || splits > 256) return fail("pips_wgrad: problem too large");
+    if (splits > 1 && !scratch) return fail("pips_wgrad: scratch of pips_wgrad_scratch_floats(M, N, K) floats is required");
+    GemmMaps maps = {};
+    if (!make_operand_map(&maps.a_hi, g_hi, M, N, ldg, 32) || !make_operand_map(&maps.a_lo, g_lo, M, N, ldg, 32)
+        || !make_operand_map(&maps.w_hi, x_hi, M, K, ldx, 32) || !make_operand_map(&maps.w_lo, x_lo, M, K, ldx, 32))
+        return fail("pips_wgrad: tensor map failed");
+    GemmArgs a = {};
+    a.M = M; a.N = N; a.K = K; a.epilogue = PIPS_EPI_BIAS;
+    a.out_f32 = splits > 1 ? scratch : dw; a.ldo = K;
+    a.kb_per_split = WG_SPLIT_ROWS / KB;
+    a.num_tiles = ((N + BM - 1) / BM) * ((K + 127) / 128) * splits;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    using Cfg = GemmCfg<3, 128>;
+    static bool attr[kMaxDevices] = {};
+    cudaError_t e = ensure_dyn_smem(wgrad_kernel, attr, Cfg::kSmemBytes);
+    if (e != cudaSuccess) return fail_cuda("pips_wgrad: smem attribute", e);
+    const int grid = a.num_tiles < sm_count() ? a.num_tiles : sm_count();
+    e = launch_pdl(wgrad_kernel, dim3(grid), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, maps, a);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e != cudaSuccess) return fail_cuda("pips_wgrad: launch", e);
+    if (splits == 1) return 0;
+    // the splits' partial sums, in split order
+    const size_t nk = static_cast<size_t>(N) * K;
+    return colsum_launch(scratch, nullptr, nullptr, nk, splits, static_cast<int>(nk), nullptr, dw, st);
 }
 
 namespace pips {
@@ -451,6 +635,27 @@ int launch_pair(bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows
         return fail((std::string("pips_gemm_tc (pair): ") + err).c_str());
     }
     return x3 ? launch_pair_variant<3>(maps, args, st) : launch_pair_variant<1>(maps, args, st);
+}
+
+// the pre-activation epilogues: bf16x3, 128 x 128 tiles (the FC1 / FC2 backward shapes have thousands of them)
+int launch_aux(const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo, int ldw, int w_rows,
+               const GemmArgs& args, cudaStream_t st) {
+    GemmMaps maps;
+    if (const char* err = make_maps(&maps, true, a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, 128, args)) {
+        return fail((std::string("pips_gemm_tc: ") + err).c_str());
+    }
+    using Cfg = GemmCfg<3, 128>;
+    static bool attr[kMaxDevices] = {};
+    {
+        cudaError_t e = ensure_dyn_smem(gemm_tc_aux_kernel, attr, Cfg::kSmemBytes);
+        if (e != cudaSuccess) return fail_cuda("pips_gemm_tc (aux): smem attribute", e);
+    }
+    GemmArgs a = args;
+    a.num_tiles = ((args.M + BM - 1) / BM) * ((args.N + 127) / 128);
+    const int grid = a.num_tiles < sm_count() ? a.num_tiles : sm_count();
+    cudaError_t e = launch_pdl(gemm_tc_aux_kernel, dim3(grid), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, maps, a);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail_cuda("pips_gemm_tc (aux): launch", e);
 }
 
 int launch_single(int bn, bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo,

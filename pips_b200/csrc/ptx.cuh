@@ -218,6 +218,19 @@ __device__ __forceinline__ void wgmma_n128_rA_tb(float (&d)[64], uint32_t a0, ui
         : "memory");
 }
 
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128], both from shared memory MN-major (wgmma_desc_sw64_mn): the weight-gradient
+// GEMM, whose two operands are stored with the contraction index as the row.
+__device__ __forceinline__ void wgmma_n128_tt(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 1, 1;\n\t}"
+        : PIPS_ACC64(d, 0)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
+
 // 64 x BN tile: BN = 256 as two N = 128 instructions on the two 128-row halves of the B tile (128-byte rows)
 template <int BN>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {

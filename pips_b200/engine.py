@@ -75,9 +75,20 @@ class PackedWeights:
 
     @staticmethod
     def _pack(module, stream) -> Dict[str, torch.Tensor]:
+        return PackedWeights.pack_mapping({k: v.detach() for k, v in module.state_dict().items()}, stream)
+
+    @staticmethod
+    def pack_mapping(sd: Dict[str, torch.Tensor], stream, transposed: bool = False,
+                     f32_copies: bool = True) -> Dict[str, torch.Tensor]:
+        """The kernel-layout tensors from a name -> tensor mapping with the module's state_dict keys.  The DeltaBlock's
+        entries ("delta_block.to_delta.*") are required; the update and visibility heads' are packed when present.
+        ``transposed``: also (hi, lo) pairs of in_w^T (768 x 512, rows >= 576 zero), fc1_w^T, fc2_w^T and head_w^T
+        (512 x 1280, columns >= 1040 zero) as "in_wT_hi", "layer3.fc1_wT_lo", ...: the W operands of the mixer's
+        input-gradient GEMMs (torch_path.delta_block_cuda).  ``f32_copies=False``: no "<weight>_f32" copies of the split
+        weights (only the fp32-precision inference path reads them)."""
         lib = L.load()
-        sd = {k: v.detach() for k, v in module.state_dict().items()}
-        dev = sd["norm.weight"].device
+        td = "delta_block.to_delta"
+        dev = sd[f"{td}.0.weight"].device
         if dev.type != "cuda":
             raise L.PipsCudaError("pips_b200: the refinement path needs the module on a CUDA device")
         t: Dict[str, torch.Tensor] = {}
@@ -85,15 +96,16 @@ class PackedWeights:
         def f32(name, v):
             t[name] = v.to(torch.float32).contiguous().clone()
 
-        def split(name, v):
-            f32(name + "_f32", v)
-            src = t[name + "_f32"]
+        def split(name, v, keep_f32=f32_copies):
+            src = v.to(torch.float32).contiguous()
+            if keep_f32:
+                f32(name + "_f32", src)
+                src = t[name + "_f32"]
             hi = torch.empty(src.shape, dtype=torch.bfloat16, device=dev)
             lo = torch.empty(src.shape, dtype=torch.bfloat16, device=dev)
             L.check(lib.pips_split_bf16(L.ptr(src), L.ptr(hi), L.ptr(lo), src.numel(), stream), "pips_split_bf16")
             t[name + "_hi"], t[name + "_lo"] = hi, lo
 
-        td = "delta_block.to_delta"
         w0 = torch.zeros(L.DIM, L.KPAD, dtype=torch.float32, device=dev)
         w0[:, :519] = sd[f"{td}.0.weight"]
         split("in_w", w0)
@@ -112,18 +124,27 @@ class PackedWeights:
             f32(q + "fc1_b", sd[p + ".1.fn.0.bias"])
             split(q + "fc2_w", sd[p + ".1.fn.3.weight"])
             f32(q + "fc2_b", sd[p + ".1.fn.3.bias"])
+            if transposed:
+                split(q + "fc1_wT", sd[p + ".1.fn.0.weight"].t(), keep_f32=False)
+                split(q + "fc2_wT", sd[p + ".1.fn.3.weight"].t(), keep_f32=False)
         f32("out_ln_w", sd[f"{td}.13.weight"])
         f32("out_ln_b", sd[f"{td}.13.bias"])
         wh = torch.zeros(L.HEAD_PAD, L.DIM, dtype=torch.float32, device=dev)
         wh[:L.HEAD] = sd[f"{td}.15.weight"]
         split("head_w", wh)
         f32("head_b", sd[f"{td}.15.bias"])
-        f32("gn_w", sd["norm.weight"])
-        f32("gn_b", sd["norm.bias"])
-        f32("upd_w", sd["ffeat_updater.0.weight"])
-        f32("upd_b", sd["ffeat_updater.0.bias"])
-        f32("vis_w", sd["vis_predictor.0.weight"].reshape(-1))
-        f32("vis_b", sd["vis_predictor.0.bias"])
+        if transposed:
+            w0t = torch.zeros(768, L.DIM, dtype=torch.float32, device=dev)
+            w0t[:L.KPAD] = w0.t()
+            split("in_wT", w0t, keep_f32=False)
+            split("head_wT", wh.t(), keep_f32=False)
+        if "norm.weight" in sd:
+            f32("gn_w", sd["norm.weight"])
+            f32("gn_b", sd["norm.bias"])
+            f32("upd_w", sd["ffeat_updater.0.weight"])
+            f32("upd_b", sd["ffeat_updater.0.bias"])
+            f32("vis_w", sd["vis_predictor.0.weight"].reshape(-1))
+            f32("vis_b", sd["vis_predictor.0.bias"])
         return t
 
     LAYER_FIELDS = ("ln1_w", "ln1_b", "tok_w1", "tok_b1", "tok_w2", "tok_b2", "ln2_w", "ln2_b",

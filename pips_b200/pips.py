@@ -22,7 +22,13 @@ Extra, optional knobs (keyword-only; the reference signature is unchanged):
               and every other call with ground truth (gradients on, is_train=True: train.py) runs the differentiable
               path with torch_path.fused_score_map_loss, whose forward and backward are CUDA kernels that never build
               the score maps either (CPU tensors keep the dense loss)
-Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET, PIPS_B200_LOSSES.
+  mixer_path  'torch' (default) or 'cuda': where the differentiable path (torch_path.forward_torch: ground truth,
+              is_train=True, train.py) runs the DeltaBlock mixer.  'torch' is the nn.Module under autograd, which keeps
+              every intermediate of every block; 'cuda' is torch_path.delta_block_cuda, one autograd node whose forward
+              and backward run on sm_90a kernels (wgmma GEMMs, recompute per block from the saved block inputs) in
+              bf16x3 arithmetic -- always, since PIPS_B200_PRECISION is an inference knob.  CPU tensors keep the module.
+              Independent of loss_path; loss_path='fused', mixer_path='cuda' puts both on the CUDA kernels
+Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET, PIPS_B200_LOSSES, PIPS_B200_MIXER.
 """
 from __future__ import annotations
 
@@ -98,7 +104,8 @@ def _conv_math(allow_tf32: bool):
 
 class Pips(nn.Module):
     def __init__(self, S=8, stride=8, *, precision: Optional[str] = None, feat_dtype: Optional[str] = None,
-                 fnet_mode: Optional[str] = None, max_seqs: int = 32768, loss_path: Optional[str] = None):
+                 fnet_mode: Optional[str] = None, max_seqs: int = 32768, loss_path: Optional[str] = None,
+                 mixer_path: Optional[str] = None):
         super().__init__()
         self.S = S
         self.stride = stride
@@ -128,6 +135,10 @@ class Pips(nn.Module):
             raise ValueError("loss_path must be 'torch' (dense differentiable score maps), 'cuda' (fused score-map "
                              "loss kernel, inference only) or 'fused' ('cuda', and the fused loss with its CUDA backward "
                              "on the differentiable path)")
+        self.mixer_path = mixer_path or os.environ.get("PIPS_B200_MIXER", "torch")
+        if self.mixer_path not in ("torch", "cuda"):
+            raise ValueError("mixer_path must be 'torch' (the DeltaBlock module under autograd) or 'cuda' (its forward and "
+                             "backward on the sm_90a kernels, bf16x3)")
 
     # ------------------------------------------------------------------ configuration
     @property

@@ -4,7 +4,8 @@ lock, gradients needed) or a summary writer that wants to log this step.  It run
 tensors live (it is what ``train.py`` / ``test_on_flt.py`` exercise) and keeps the reference's
 semantics, including the dense score map ``fcps`` that only the score-map loss consumes -- except with
 ``model.loss_path == 'fused'`` on CUDA tensors, where ``fused_score_map_loss`` computes that loss and its gradients
-without ``fcps``.
+without ``fcps``, and with ``model.mixer_path == 'cuda'`` on CUDA tensors, where ``delta_block_cuda`` runs the
+DeltaBlock mixer forward and backward on the sm_90a kernels.
 
 Not used -- and not a fallback -- for plain inference: that path is CUDA-only (pips.py).
 """
@@ -158,6 +159,260 @@ def fused_score_map_loss(ffeats_per_iter, pyramid, trajs_g, vis_g, valids):
     return _FusedScoreMapLoss.apply(target, len(ffeats_per_iter), *ffeats_per_iter, *pyramid)
 
 
+def _round_up(v, m):
+    return (v + m - 1) // m * m
+
+
+class _MixerRun:
+    """Launch helpers of one delta_block_cuda call: its packs, device, stream and row counts.  Row buffers are allocated
+    with whole 256-row tiles (the pair GEMM kernel's condition) from torch's caching allocator on the call's device."""
+
+    def __init__(self, packs, R, dev):
+        from . import _lib as L
+        self.L, self.lib, self.w, self.dev = L, L.load(), packs, dev
+        self.st = torch.cuda.current_stream(dev).cuda_stream
+        self.R, self.M = R, R * 8
+        self.Ra, self.Ma = _round_up(R, 256), _round_up(R * 8, 256)
+        self.zero = torch.zeros(L.HIDDEN, device=dev)                 # the bias of the input-gradient GEMMs
+
+    def rows(self, n, cols, dtype=torch.float32):
+        return torch.empty(n, cols, dtype=dtype, device=self.dev)
+
+    def pair(self, n, cols):
+        return self.rows(n, cols, torch.bfloat16), self.rows(n, cols, torch.bfloat16)
+
+    def split(self, src, n_rows=None):
+        """(hi, lo) of the fp32 rows src (n, cols), in buffers of whole tiles"""
+        hi, lo = self.pair(_round_up(src.shape[0], 256), src.shape[1])
+        self.L.check(self.lib.pips_split_bf16(self.L.ptr(src), self.L.ptr(hi), self.L.ptr(lo), src.numel(), self.st),
+                     "pips_split_bf16")
+        return hi, lo
+
+    def gemm(self, a, M, K, wname, N, bias, epi, out=None, ldo=0, oh=(None, None), ldh=0, aux=None):
+        L, w = self.L, self.w
+        self.L.check(self.lib.pips_gemm_tc_aux(
+            L.ptr(a[0]), L.ptr(a[1]), a[0].shape[1], a[0].shape[0], L.ptr(w[wname + "_hi"]), L.ptr(w[wname + "_lo"]),
+            w[wname + "_hi"].shape[1], w[wname + "_hi"].shape[0], M, N, K, L.ptr(bias), epi, L.ptr(out), ldo,
+            L.ptr(oh[0]), L.ptr(oh[1]), ldh, L.ptr(aux), 0 if aux is None else aux.shape[1], self.st), "pips_gemm_tc")
+
+    def wgrad(self, g, N, x, K, M):
+        L = self.L
+        dw = torch.empty(N, K, device=self.dev)
+        n = self.lib.pips_wgrad_scratch_floats(M, N, K)
+        scratch = torch.empty(n, device=self.dev) if n else None
+        L.check(self.lib.pips_wgrad(L.ptr(g[0]), L.ptr(g[1]), g[0].shape[1], L.ptr(x[0]), L.ptr(x[1]), x[0].shape[1], M, N, K,
+                                    L.ptr(scratch), L.ptr(dw), self.st), "pips_wgrad")
+        return dw
+
+    def colsum(self, g32=None, pair=(None, None), N=0, M=0):
+        L = self.L
+        out = torch.empty(N, device=self.dev)
+        n = self.lib.pips_colsum_scratch_floats(M, N)
+        scratch = torch.empty(n, device=self.dev) if n else None
+        ld = (g32 if g32 is not None else pair[0]).shape[1]
+        L.check(self.lib.pips_colsum(L.ptr(g32), L.ptr(pair[0]), L.ptr(pair[1]), ld, M, N, L.ptr(scratch), L.ptr(out), self.st),
+                "pips_colsum")
+        return out
+
+    def block_forward(self, l, x, y, h):
+        """block l in place on the residual stream x (Ma, 512); y, h: (hi, lo) buffers of LN2's output and FC1's"""
+        L, w, q = self.L, self.w, f"layer{l}."
+        L.check(self.lib.pips_tokenmix(L.ptr(x), self.R, *(L.ptr(w[q + n]) for n in
+                                                          ("ln1_w", "ln1_b", "tok_w1", "tok_b1", "tok_w2", "tok_b2", "ln2_w", "ln2_b")),
+                                       L.ptr(y[0]), L.ptr(y[1]), None, self.st), "pips_tokenmix")
+        self.gemm(y, self.M, L.DIM, q + "fc1_w", L.HIDDEN, w[q + "fc1_b"], L.EPI_BIAS_GELU, oh=h, ldh=L.HIDDEN)
+        self.gemm(h, self.M, L.HIDDEN, q + "fc2_w", L.DIM, w[q + "fc2_b"], L.EPI_BIAS_RESID, out=x, ldo=L.DIM)
+
+
+# DeltaBlock parameter names in named_parameters order: the order of delta_block_cuda's inputs and gradients
+def _delta_param_names(depth=12):
+    names = ["to_delta.0.weight", "to_delta.0.bias"]
+    for l in range(depth):
+        p = f"to_delta.{l + 1}"
+        for half in (0, 1):                 # PreNormResidual registers fn before norm
+            names += [f"{p}.{half}.fn.0.weight", f"{p}.{half}.fn.0.bias", f"{p}.{half}.fn.3.weight", f"{p}.{half}.fn.3.bias",
+                      f"{p}.{half}.norm.weight", f"{p}.{half}.norm.bias"]
+    return names + ["to_delta.13.weight", "to_delta.13.bias", "to_delta.15.weight", "to_delta.15.bias"]
+
+
+DELTA_PARAMS = tuple(_delta_param_names())
+
+
+def _delta_shapes():
+    """the parameter shapes of a DeltaBlock(), by name (built on the meta device: no memory, no initialisation)"""
+    global _DELTA_SHAPES
+    if _DELTA_SHAPES is None:
+        from .pips import DeltaBlock
+        with torch.device("meta"):
+            _DELTA_SHAPES = {n: tuple(p.shape) for n, p in DeltaBlock().named_parameters()}
+    return _DELTA_SHAPES
+
+
+_DELTA_SHAPES = None
+
+
+def _delta_block_params(delta_block):
+    """The 150 parameter tensors of ``delta_block`` in DELTA_PARAMS order, found by attribute lookup along each dotted
+    name.  named_parameters() would not do: an nn.DataParallel replica (torch.nn.parallel.replicate) keeps its broadcast
+    parameters as plain attributes and lists none."""
+    params = []
+    for n in DELTA_PARAMS:
+        mod_name, attr = n.rsplit(".", 1)
+        try:
+            t = getattr(delta_block.get_submodule(mod_name), attr)
+        except AttributeError:
+            t = None
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != _delta_shapes()[n]:
+            raise ValueError(f"delta_block_cuda: the module is not a 12-block DeltaBlock(dim=512, S=8) (at {n})")
+        params.append(t)
+    return params
+
+
+# pack entries only the forward reads: dropped before the pack is kept for the backward
+_FORWARD_ONLY = ("in_w_hi", "in_w_lo", "head_w_hi", "head_w_lo") + tuple(
+    f"layer{l}.fc2_w_{part}" for l in range(12) for part in ("hi", "lo"))
+
+
+class _DeltaBlockFn(torch.autograd.Function):
+    """DeltaBlock.forward on the sm_90a kernels, bf16x3 throughout, with the parameters as explicit inputs (so gradients
+    reach nn.DataParallel replicas' broadcast parameters).  The forward saves the block boundaries only: the (hi, lo)
+    input rows, the residual stream at the entry of each of the 12 blocks and before the final LayerNorm.  The backward
+    recomputes each block from its entry with the forward's kernels, so the recomputed activations are the forward's
+    bits, and runs the block's backward: FC1 recompute (keeping the pre-activation), FC2 weight / input gradients (the
+    GELU derivative in the GEMM epilogue), FC1 weight / input gradients, then one CUDA-core kernel for the LayerNorms and
+    the token mixing."""
+
+    @staticmethod
+    def forward(ctx, save, x, *params):
+        from .engine import PackedWeights
+        R = x.shape[0]
+        dev = x.device
+        with torch.cuda.device(dev):
+            sd = {"delta_block." + n: p.detach() for n, p in zip(DELTA_PARAMS, params)}
+            run = _MixerRun(None, R, dev)
+            L = run.L
+            run.w = PackedWeights.pack_mapping(sd, run.st, transposed=save, f32_copies=False)
+            M, Ma = run.M, run.Ma
+            xin = torch.zeros(M, L.KPAD, device=dev)
+            xin[:, :519] = x.detach().reshape(M, 519)
+            x0 = run.split(xin)
+            del xin
+            xs = torch.empty(L.DEPTH + 1 if save else 1, Ma, L.DIM, device=dev)
+            run.gemm(x0, M, L.KPAD, "in_w", L.DIM, run.w["in_b"], L.EPI_BIAS, out=xs[0], ldo=L.DIM)
+            y, h = run.pair(Ma, L.DIM), run.pair(Ma, L.HIDDEN)
+            for l in range(L.DEPTH):
+                cur = xs[l + 1] if save else xs[0]
+                if save:
+                    cur.copy_(xs[l])
+                run.block_forward(l, cur, y, h)
+            del y, h
+            xf = xs[-1]
+            p = run.pair(run.Ra, L.DIM)
+            L.check(run.lib.pips_ln_pool(L.ptr(xf), R, L.ptr(run.w["out_ln_w"]), L.ptr(run.w["out_ln_b"]), L.ptr(p[0]),
+                                         L.ptr(p[1]), None, run.st), "pips_ln_pool")
+            delta = torch.empty(R, L.HEAD, device=dev)
+            run.gemm(p, R, L.DIM, "head_w", L.HEAD, run.w["head_b"], L.EPI_BIAS, out=delta, ldo=L.HEAD)
+        if save:
+            ctx.save_for_backward(x0[0], x0[1], xs)
+            ctx.packs = {k: v for k, v in run.w.items() if k not in _FORWARD_ONLY}
+            ctx.shapes = [p.shape for p in params]
+        return delta.view(R, 8, L.HEAD // 8)
+
+    @staticmethod
+    def backward(ctx, grad):
+        from . import _lib as L
+        x0_hi, x0_lo, xs = ctx.saved_tensors
+        dev = xs.device
+        R = grad.shape[0]
+        with torch.cuda.device(dev):
+            run = _MixerRun(ctx.packs, R, dev)
+            w, lib, M, Ma, Ra = run.w, run.lib, run.M, run.Ma, run.Ra
+            g = {}
+            # head: delta = p . head_w^T + head_b over the R pooled rows; K padded to 1280 with zeros
+            dd = torch.zeros(R, L.HEAD_PAD, device=dev)
+            dd[:, :L.HEAD] = grad.reshape(R, L.HEAD)
+            ddp = run.split(dd)
+            p = run.pair(Ra, L.DIM)
+            L.check(lib.pips_ln_pool(L.ptr(xs[-1]), R, L.ptr(w["out_ln_w"]), L.ptr(w["out_ln_b"]), L.ptr(p[0]), L.ptr(p[1]), None,
+                                     run.st), "pips_ln_pool")
+            g["to_delta.15.weight"] = run.wgrad(ddp, L.HEAD, p, L.DIM, R)
+            g["to_delta.15.bias"] = run.colsum(g32=dd, N=L.HEAD, M=R)
+            del p
+            dp = run.rows(Ra, L.DIM)
+            run.gemm(ddp, R, L.HEAD_PAD, "head_wT", L.DIM, run.zero, L.EPI_BIAS, out=dp, ldo=L.DIM)
+            del dd, ddp
+            dX = run.rows(Ma, L.DIM)
+            lp = torch.empty(lib.pips_ln_pool_grad_scratch_floats(R), device=dev)
+            lpg = torch.empty(2 * L.DIM, device=dev)
+            L.check(lib.pips_ln_pool_grad(L.ptr(xs[-1]), L.ptr(dp), R, L.ptr(w["out_ln_w"]), L.ptr(w["out_ln_b"]), L.ptr(dX),
+                                          L.ptr(lp), L.ptr(lpg), run.st), "pips_ln_pool_grad")
+            g["to_delta.13.weight"], g["to_delta.13.bias"] = lpg[:L.DIM], lpg[L.DIM:]
+            del dp, lp
+            # the 12 blocks, last first
+            work = run.rows(Ma, L.DIM)
+            y, gh = run.pair(Ma, L.DIM), run.pair(Ma, L.HIDDEN)
+            dh = run.pair(Ma, L.HIDDEN)
+            hpre = run.rows(Ma, L.HIDDEN)
+            dy = run.rows(Ma, L.DIM)
+            tg = torch.empty(lib.pips_tokenmix_grad_scratch_floats(R), device=dev)
+            for l in reversed(range(L.DEPTH)):
+                q, pn = f"layer{l}.", f"to_delta.{l + 1}"
+                work.copy_(xs[l])
+                L.check(lib.pips_tokenmix(L.ptr(work), R, *(L.ptr(w[q + n]) for n in
+                                                           ("ln1_w", "ln1_b", "tok_w1", "tok_b1", "tok_w2", "tok_b2", "ln2_w", "ln2_b")),
+                                          L.ptr(y[0]), L.ptr(y[1]), None, run.st), "pips_tokenmix")
+                run.gemm(y, M, L.DIM, q + "fc1_w", L.HIDDEN, w[q + "fc1_b"], L.EPI_BIAS_GELU_PRE, oh=gh, ldh=L.HIDDEN, aux=hpre)
+                dXp = run.split(dX[:M])
+                g[pn + ".1.fn.3.weight"] = run.wgrad(dXp, L.DIM, gh, L.HIDDEN, M)
+                g[pn + ".1.fn.3.bias"] = run.colsum(g32=dX, N=L.DIM, M=M)
+                run.gemm(dXp, M, L.DIM, q + "fc2_wT", L.HIDDEN, run.zero, L.EPI_GELU_GRAD, oh=dh, ldh=L.HIDDEN, aux=hpre)
+                del dXp
+                g[pn + ".1.fn.0.weight"] = run.wgrad(dh, L.HIDDEN, y, L.DIM, M)
+                g[pn + ".1.fn.0.bias"] = run.colsum(pair=dh, N=L.HIDDEN, M=M)
+                run.gemm(dh, M, L.HIDDEN, q + "fc1_wT", L.DIM, run.zero, L.EPI_BIAS, out=dy, ldo=L.DIM)
+                tk = torch.empty(2600, device=dev)
+                L.check(lib.pips_tokenmix_grad(L.ptr(xs[l]), L.ptr(work), L.ptr(dy), L.ptr(dX), R,
+                                               *(L.ptr(w[q + n]) for n in ("ln1_w", "ln1_b", "tok_w1", "tok_b1", "tok_w2",
+                                                                           "tok_b2", "ln2_w", "ln2_b")),
+                                               L.ptr(tg), L.ptr(tk), run.st), "pips_tokenmix_grad")
+                for name, a, b in ((".0.norm.weight", 0, 512), (".0.norm.bias", 512, 1024), (".0.fn.0.weight", 1024, 1280),
+                                   (".0.fn.0.bias", 1280, 1312), (".0.fn.3.weight", 1312, 1568), (".0.fn.3.bias", 1568, 1576),
+                                   (".1.norm.weight", 1576, 2088), (".1.norm.bias", 2088, 2600)):
+                    g[pn + name] = tk[a:b]
+            del work, y, gh, dh, hpre, dy, tg
+            # input layer: x = x0 . in_w^T + in_b
+            dXp = run.split(dX[:M])
+            dx0 = run.rows(Ma, L.KPAD)
+            run.gemm(dXp, M, L.DIM, "in_wT", L.KPAD, run.zero, L.EPI_BIAS, out=dx0, ldo=L.KPAD)
+            g["to_delta.0.weight"] = run.wgrad(dXp, L.DIM, (x0_hi, x0_lo), L.KPAD, M)[:, :519].contiguous()
+            g["to_delta.0.bias"] = run.colsum(g32=dX, N=L.DIM, M=M)
+            dx = dx0[:M, :519].reshape(R, 8, 519)
+        grads = [g[n].reshape(sh) for n, sh in zip(DELTA_PARAMS, ctx.shapes)]
+        return (None, dx if ctx.needs_input_grad[1] else None, *grads)
+
+
+def delta_block_cuda(delta_block, x):
+    """``DeltaBlock.forward`` (nets/pips.py:304-311) on the sm_90a kernels, differentiable in ``x`` and in every one of
+    the block's 150 parameters: x (R, 8, 519) fp32 CUDA -> (R, 8, 130).  The arithmetic is bf16x3 (fp32-class) whatever
+    PIPS_B200_PRECISION says.  Allocates through torch's caching allocator on x's device and runs on its current stream;
+    the weights are packed from the parameters on every call (nn.DataParallel replicas hold new tensors each step).
+    ``delta_block`` may be a DeltaBlock or an nn.DataParallel replica of one; the gradients flow to whatever tensors its
+    parameter attributes hold (a replica's broadcast copies, and through them the original parameters)."""
+    if not isinstance(x, torch.Tensor) or not x.is_cuda:
+        raise RuntimeError("delta_block_cuda runs on the CUDA kernels only; use the DeltaBlock module for CPU tensors")
+    if x.dim() != 3 or x.shape[1] != 8 or x.shape[2] != 519:
+        raise ValueError(f"delta_block_cuda: x must be (R, 8, 519) (S = 8 frames); got {tuple(x.shape)}")
+    if x.dtype != torch.float32:
+        raise ValueError(f"delta_block_cuda: x must be float32; got {x.dtype}")
+    if x.shape[0] == 0:
+        raise ValueError("delta_block_cuda: no rows")
+    params = _delta_block_params(delta_block)
+    if any(p.device != x.device or p.dtype != torch.float32 for p in params):
+        raise ValueError("delta_block_cuda: the parameters must be float32 on x's device")
+    save = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
+    return _DeltaBlockFn.apply(save, x.contiguous(), *params)
+
+
 def sample_clamped(im, x, y):
     """utils/samp.py:5-78: bilinear sample with clamped indices and unclamped weights -> (B,N,C)."""
     B, C, H, W = im.shape
@@ -234,7 +489,11 @@ def forward_torch(model, xys, rgbs, coords_init=None, feat_init=None, iters=3, t
         flow = (coords - coords[:, 0:1]).permute(0, 2, 1, 3).reshape(B * N, S, 2)
         flow = torch.cat([flow, times.expand(B * N, -1, -1)], dim=2)
         feats_ = ffeats.permute(0, 2, 1, 3).reshape(B * N, S, -1)
-        delta = model.delta_block(torch.cat([feats_, fcorr, motion_embedding(flow)], dim=2))      # :524
+        x_mix = torch.cat([feats_, fcorr, motion_embedding(flow)], dim=2)
+        if getattr(model, "mixer_path", "torch") == "cuda" and x_mix.is_cuda:
+            delta = delta_block_cuda(model.delta_block, x_mix)                                      # :524 on sm_90a
+        else:
+            delta = model.delta_block(x_mix)                                                        # :524
         dfeat = delta[:, :, 2:].reshape(B * N * S, -1)
         feats_ = model.ffeat_updater(model.norm(dfeat)) + feats_.reshape(B * N * S, -1)             # :530
         ffeats = feats_.reshape(B, N, S, -1).permute(0, 2, 1, 3)

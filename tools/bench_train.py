@@ -1,0 +1,190 @@
+"""Training-path timings on one GPU: the DeltaBlock mixer's forward + backward on the torch module against
+torch_path.delta_block_cuda, each new backward kernel alone, and a whole training step (is_train=True, the backward of the
+three losses) with loss_path='fused' and mixer_path 'torch' against 'cuda'.
+
+    python tools/bench_train.py [--reps 5] [--skip-step]
+
+Shapes: train.py's per-GPU shape (B=4, N=768, 4 iterations, 8 x 384 x 512, stride 8: R = 3072 tracks, M = 24576 mixer
+rows) and BASELINE cfg 2 (N=1024, 6 iterations: M = 32768).  Medians of --reps timed runs after two warm-ups, CUDA
+events; peaks from torch.cuda.max_memory_allocated.  Rates count useful FLOPs (2 M N K per GEMM); the share of 989
+TFLOP/s (H100 SXM dense BF16) counts the three MMAs of every bf16x3 product."""
+import argparse
+import os
+import statistics
+import subprocess
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from oracle import pips_oracle as po  # noqa: E402
+from pips_b200 import Pips, _lib as L, torch_path  # noqa: E402
+from pips_b200.pips import DeltaBlock  # noqa: E402
+
+DEV = "cuda:0"
+PEAK = 989e12
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    return q[0] if q else torch.cuda.get_device_name()
+
+
+def timed(fn, reps, warm=2):
+    for _ in range(warm):
+        fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(reps):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        fn()
+        b.record()
+        torch.cuda.synchronize()
+        ts.append(a.elapsed_time(b))
+    return statistics.median(ts)
+
+
+def peak_of(fn):
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()
+    torch.cuda.reset_peak_memory_stats()
+    base = torch.cuda.memory_allocated()
+    fn()
+    torch.cuda.synchronize()
+    return (torch.cuda.max_memory_allocated() - base) / 2**30
+
+
+def delta_block(seed=3):
+    sd = po.init_state_dict(seed=seed, head_scale=0.05)
+    m = DeltaBlock().to(DEV)
+    m.load_state_dict({k[len("delta_block."):]: v for k, v in sd.items() if k.startswith("delta_block.")})
+    return m
+
+
+def strict_fp32():
+    """Strict fp32 for the torch module, the accuracy class of the bf16x3 kernels: cuDNN on (the token-mixing Conv1d
+    layers), TF32 off for its convolutions and for matmul (off by default).  Returns the previous settings."""
+    old = (torch.backends.cudnn.enabled, torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
+    torch.backends.cudnn.enabled = True
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    return old
+
+
+def bench_mixer(reps):
+    m = delta_block()
+    old = strict_fp32()
+    try:
+        _bench_mixer(m, reps)
+    finally:
+        torch.backends.cudnn.enabled, torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
+
+
+def _bench_mixer(m, reps):
+    for R in (3072, 4096):
+        x = torch.randn(R, 8, 519, device=DEV)
+        dy = torch.randn(R, 8, 130, device=DEV)
+        for name in ("torch", "cuda"):
+            def step():
+                m.zero_grad(set_to_none=True)
+                xr = x.clone().requires_grad_(True)
+                out = torch_path.delta_block_cuda(m, xr) if name == "cuda" else m(xr)
+                (out * dy).sum().backward()
+            try:
+                ms = timed(step, reps)
+                gib = peak_of(step)
+                print(f"mixer fwd+bwd M={8 * R} {name:5s}: {ms:8.2f} ms, peak {gib:6.2f} GiB above inputs")
+            except torch.cuda.OutOfMemoryError:
+                print(f"mixer fwd+bwd M={8 * R} {name:5s}: out of memory")
+            torch.cuda.empty_cache()
+
+
+def split(v):
+    hi = torch.empty(v.shape, dtype=torch.bfloat16, device=DEV)
+    lo = torch.empty_like(hi)
+    L.check(L.load().pips_split_bf16(L.ptr(v), L.ptr(hi), L.ptr(lo), v.numel(), torch.cuda.current_stream().cuda_stream))
+    return hi, lo
+
+
+def bench_kernels(reps):
+    lib = L.load()
+    st = torch.cuda.current_stream().cuda_stream
+    M, R = 24576, 3072
+
+    def report(name, ms, flop, mmas=3):
+        print(f"{name:34s}: {ms * 1e3:8.1f} us, {flop / ms / 1e9:6.1f} TFLOP/s useful, {mmas * flop / (ms * 1e-3) / PEAK:.2f} of "
+              f"989 TFLOP/s in issued MMAs" if flop else f"{name:34s}: {ms * 1e3:8.1f} us")
+
+    for (Mv, N, K, what) in ((M, 512, 2048, "wgrad FC2 (512x2048)"), (M, 2048, 512, "wgrad FC1 (2048x512)"),
+                             (M, 512, 576, "wgrad input (512x576)"), (R, 1040, 512, "wgrad head (1040x512)")):
+        g, x = split(torch.randn(Mv, N, device=DEV)), split(torch.randn(Mv, K, device=DEV))
+        dw = torch.empty(N, K, device=DEV)
+        sc = torch.empty(max(1, lib.pips_wgrad_scratch_floats(Mv, N, K)), device=DEV)
+        fn = lambda: L.check(lib.pips_wgrad(L.ptr(g[0]), L.ptr(g[1]), N, L.ptr(x[0]), L.ptr(x[1]), K, Mv, N, K, L.ptr(sc),
+                                            L.ptr(dw), st))
+        report(f"{what} M={Mv}", timed(fn, 20, 3), 2.0 * Mv * N * K)
+    a, w = split(torch.randn(M, 512, device=DEV)), split(torch.randn(2048, 512, device=DEV) / 23)
+    b = torch.randn(2048, device=DEV)
+    hi, lo = torch.empty(M, 2048, dtype=torch.bfloat16, device=DEV), torch.empty(M, 2048, dtype=torch.bfloat16, device=DEV)
+    pre = torch.empty(M, 2048, device=DEV)
+    for epi, name in ((L.EPI_BIAS_GELU, "FC1 forward (BIAS_GELU)"), (L.EPI_BIAS_GELU_PRE, "FC1 recompute (BIAS_GELU_PRE)"),
+                      (L.EPI_GELU_GRAD, "FC2 dgrad (GELU_GRAD)")):
+        fn = lambda: L.check(lib.pips_gemm_tc_aux(L.ptr(a[0]), L.ptr(a[1]), 512, M, L.ptr(w[0]), L.ptr(w[1]), 512, 2048, M, 2048, 512,
+                                                  L.ptr(b), epi, None, 0, L.ptr(hi), L.ptr(lo), 2048, L.ptr(pre), 2048, st))
+        report(f"{name} M={M}", timed(fn, 20, 3), 2.0 * M * 2048 * 512)
+    x = torch.randn(M, 512, device=DEV)
+    dxb = torch.randn(M, 512, device=DEV)
+    P = [torch.randn(n, device=DEV) for n in (512, 512, 256, 32, 256, 8, 512, 512)]
+    sc = torch.empty(lib.pips_tokenmix_grad_scratch_floats(R), device=DEV)
+    gr = torch.empty(2600, device=DEV)
+    fn = lambda: L.check(lib.pips_tokenmix_grad(L.ptr(x), L.ptr(x), L.ptr(x), L.ptr(dxb), R, *(L.ptr(p) for p in P), L.ptr(sc),
+                                                L.ptr(gr), st))
+    report(f"tokenmix_grad {R} sequences", timed(fn, 20, 3), 0)
+
+
+def bench_step(reps):
+    for label, B, N, iters in (("train.py shape", 4, 768, 4), ("cfg 2", 4, 1024, 6)):
+        rgbs = po.smooth_video(B, 8, 384, 512, seed=1).to(DEV)
+        xys = po.random_queries(B, N, 384, 512, seed=2).to(DEV)
+        g = torch.Generator().manual_seed(3)
+        tg = (xys.cpu()[:, None] + torch.cumsum(torch.randn(B, 8, N, 2, generator=g) * 3.0, 1)).to(DEV)
+        vg = torch.ones(B, 8, N, device=DEV)
+        va = torch.ones(B, 8, N, device=DEV)
+        for mixer in ("torch", "cuda"):
+            m = Pips(S=8, stride=8, loss_path="fused", mixer_path=mixer).to(DEV).train()
+            m.load_state_dict(po.init_state_dict(seed=3, head_scale=0.05))
+
+            def step():
+                m.zero_grad(set_to_none=True)
+                _, _, _, losses = m(xys, rgbs, iters=iters, trajs_g=tg, vis_g=vg, valids=va, is_train=True)
+                sum(losses).backward()
+            try:
+                ms = timed(step, reps, warm=1)
+                gib = peak_of(step)
+                print(f"training step, {label} (B={B}, N={N}, {iters} iterations), mixer {mixer:5s}: {ms:8.1f} ms, "
+                      f"peak {gib:6.2f} GiB")
+            except torch.cuda.OutOfMemoryError:
+                print(f"training step, {label} (B={B}, N={N}, {iters} iterations), mixer {mixer:5s}: does not fit in "
+                      f"{torch.cuda.get_device_properties(0).total_memory / 2**30:.0f} GiB")
+            del m
+            torch.cuda.empty_cache()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--skip-step", action="store_true")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_train.py measures on the GPU; no CUDA device found")
+    print(f"card: {card()}")
+    bench_kernels(args.reps)
+    bench_mixer(args.reps)
+    if not args.skip_step:
+        bench_step(args.reps)
+
+
+if __name__ == "__main__":
+    main()
