@@ -279,6 +279,36 @@ int pips_conv_tc_stats(const void* x_hi, const void* x_lo, int N, int H, int W, 
  * 2*(rgb/255)-1 at x = 2*ox + s - 3, zero outside the image / for k >= 21.  (ABI 3; ABI 2 unfolded the columns only.) */
 int pips_stem_pack(const void* rgb, int dtype, int N, int H, int W, void* out_hi, void* out_lo, void* stream);
 
+/* ---- backward of the feature encoder (csrc/conv_grad.cu, csrc/encoder_grad.cu).  Every sum runs in a fixed order that
+ * depends on the shape only: no atomics, the same bits on any GPU. ----
+ * Weight gradient of a convolution on the tensor cores, bf16x3:
+ *   dw[co, (r*S + s)*Cp + ci] = sum_{n,oy,ox} dy[n,oy,ox,co] * x[n, oy*stride_y + r - pad_y, ox*stride_x + s - pad_x, ci]
+ * x (N, H, W, Cp) bf16 (hi, lo) as pips_conv_tc reads it (zero outside the image); dy bf16 (hi, lo) of channel pitch
+ * ldy >= Cout (multiple of 8): (N, Ho, Wo, ldy) with dy_step 1, or, with dy_step 2 (stride-2 convolutions only),
+ * zero-dilated on the input's (N, H, W, ldy) grid with output pixel (oy, ox) at (2oy, 2ox).  dw (Cout, R*S*Cp) fp32,
+ * dense.  The pixels are split into chunks whose partial sums go to scratch
+ * (pips_conv_wgrad_scratch_floats(N, Ho, Wo, Cout, R*S*Cp) floats; may be NULL when that is 0). */
+size_t pips_conv_wgrad_scratch_floats(int N, int Ho, int Wo, int Cout, int K);
+int pips_conv_wgrad(const void* dy_hi, const void* dy_lo, int ldy, int dy_step, const void* x_hi, const void* x_lo, int N, int H,
+                    int W, int Cp, int Cout, int R, int S, int stride_y, int stride_x, int pad_y, int pad_x, float* scratch,
+                    float* dw, void* stream);
+/* Backward of pips_inorm_apply_pair's main branch (nets/pips.py:154-157 + ReLU): with g = g0 (+ g1) (+ g2) the gradient
+ * of the forward's output (N, H, W, C) fp32, masked by the ReLUs the forward applied (recomputed from y, stats, r,
+ * stats_r, relu_main, relu_out exactly as the forward computed them), and x_hat = (y - mean) * rstd:
+ *   dy = rstd * (g - mean(g) - x_hat * mean(g * x_hat))            (means per image and channel over H*W)
+ * written as a bf16 (hi, lo) pair of row stride pair_ld (channels [C, pair_ld) zero), on the (H, W) grid, or with
+ * dil_h, dil_w != 0 zero-dilated on that (2H or 2H-1, 2W or 2W-1) grid (pixel (y, x) at (2y, 2x), zeros elsewhere).
+ * g_out (optional): g after the output ReLU's mask only -- the gradient of the residual branch.  r requires relu_out.
+ * scratch: pips_inorm_grad_scratch_floats(N, H*W, C) floats, 16-byte aligned. */
+size_t pips_inorm_grad_scratch_floats(int N, int HW, int C);
+int pips_inorm_grad(const float* y, const float* stats, const float* r, const float* stats_r, int relu_main, int relu_out,
+                    const float* g0, const float* g1, const float* g2, int N, int H, int W, int C, float* scratch, void* dy_hi,
+                    void* dy_lo, int pair_ld, int dil_h, int dil_w, float* g_out, void* stream);
+/* Adjoint of pips_resize_pair (bilinear, align_corners=True, (Hs, Ws) -> (Ho, Wo)): out (N, Hs, Ws, C) fp32 from the
+ * channels [c_off, c_off + C) of g (N, Ho, Wo, ldg) fp32.  A gather: every source pixel sums the destination pixels
+ * whose taps touch it, in a fixed order. */
+int pips_resize_grad(const float* g, int ldg, int c_off, int N, int Ho, int Wo, float* out, int Hs, int Ws, int C, void* stream);
+
 /* Whole-iteration operator: everything between `for itr in range(iters)` and the append of
  * coords*stride (nets/pips.py:499-539, minus the dead fcp heat-map :504-511). */
 typedef struct pips_layer_weights {

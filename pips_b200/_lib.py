@@ -115,6 +115,11 @@ _SIGNATURES = {
     "pips_conv_rows_chunks": (_i, [_i, _i]),
     "pips_conv_rows": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p, _p]),
     "pips_inorm_finalize": (_i, [_p, _i, _i, _i, _i, _p, _p]),
+    "pips_conv_wgrad_scratch_floats": (C.c_size_t, [_i] * 5),
+    "pips_conv_wgrad": (_i, [_p, _p, _i, _i, _p, _p] + [_i] * 11 + [_p, _p, _p]),
+    "pips_inorm_grad_scratch_floats": (C.c_size_t, [_i] * 3),
+    "pips_inorm_grad": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _i, _i, _i, _p, _p]),
+    "pips_resize_grad": (_i, [_p, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p]),
     "pips_mixer_forward": (_i, [C.POINTER(Weights), C.POINTER(Workspace), _i, _i, _p]),
     "pips_refine_iter": (_i, [C.POINTER(Problem), C.POINTER(Weights), C.POINTER(Workspace), _p, _p]),
 }

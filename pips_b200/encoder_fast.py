@@ -129,22 +129,27 @@ def _pad64(c: int) -> int:
     return (c + 63) // 64 * 64
 
 
+def pack_conv_weight(w: torch.Tensor):
+    """(Cout, Cin, R, S) -> ((BN, R*S*Cp) bf16 hi, lo) with k = (r*S + s)*Cp + ci, the filter layout of pips_conv_tc."""
+    lib = L.load()
+    cout, cin, R, S = w.shape
+    cp = _pad64(cin)
+    bn = 64 if cout <= 64 else (128 if cout <= 128 else 256)
+    packed = torch.zeros(bn, R, S, cp, dtype=torch.float32, device=w.device)
+    packed[:cout, :, :, :cin] = w.detach().float().permute(0, 2, 3, 1)
+    packed = packed.reshape(bn, R * S * cp).contiguous()
+    hi = torch.empty_like(packed, dtype=torch.bfloat16)
+    lo = torch.empty_like(packed, dtype=torch.bfloat16)
+    L.check(lib.pips_split_bf16(L.ptr(packed), L.ptr(hi), L.ptr(lo), packed.numel(), _st()), "pips_split_bf16")
+    return hi, lo
+
+
 def _packed_weight(conv: torch.nn.Conv2d):
-    """(Cout, Cin, R, S) fp32 -> ((BN, R*S*Cp) bf16 hi, lo) with k = (r*S + s)*Cp + ci; cached per weight version."""
+    """pack_conv_weight of conv.weight, cached per weight version."""
     w = conv.weight
     key = (w.data_ptr(), w._version)
     if getattr(conv, "_wtc_key", None) != key:
-        lib = L.load()
-        cout, cin, R, S = w.shape
-        cp = _pad64(cin)
-        bn = 64 if cout <= 64 else (128 if cout <= 128 else 256)
-        packed = torch.zeros(bn, R, S, cp, dtype=torch.float32, device=w.device)
-        packed[:cout, :, :, :cin] = w.detach().float().permute(0, 2, 3, 1)
-        packed = packed.reshape(bn, R * S * cp).contiguous()
-        hi = torch.empty_like(packed, dtype=torch.bfloat16)
-        lo = torch.empty_like(packed, dtype=torch.bfloat16)
-        L.check(lib.pips_split_bf16(L.ptr(packed), L.ptr(hi), L.ptr(lo), packed.numel(), _st()), "pips_split_bf16")
-        conv._wtc = (hi, lo)
+        conv._wtc = pack_conv_weight(w)
         conv._wtc_key = key
     return conv._wtc
 
@@ -159,16 +164,17 @@ class _Pair:
         self.lo = torch.empty(N, H, W, self.Cp, dtype=torch.bfloat16, device=device)
 
 
-def conv_tc(x: _Pair, conv: torch.nn.Conv2d, bias: bool = False, stats: bool = False):
+def conv_tc(x: _Pair, conv: torch.nn.Conv2d, bias: bool = False, stats: bool = False, w=None):
     """-> output (N,Ho,Wo,Cout) fp32; with ``stats`` also the InstanceNorm statistics (N,2,Cout) of the output, from
-    partial sums the convolution's epilogue accumulates (no separate pass over the output)."""
+    partial sums the convolution's epilogue accumulates (no separate pass over the output).  ``w``: the (hi, lo) filter
+    pack to use instead of the module's cached one."""
     lib = L.load()
     N, H, W = x.shape
     cout, cin, R, S = conv.weight.shape
     assert cin == x.C and conv.stride[0] == conv.stride[1] and conv.padding[0] == conv.padding[1]
     st, pad = conv.stride[0], conv.padding[0]
     Ho, Wo = (H + 2 * pad - R) // st + 1, (W + 2 * pad - S) // st + 1
-    w_hi, w_lo = _packed_weight(conv)
+    w_hi, w_lo = _packed_weight(conv) if w is None else w
     dev = x.hi.device
     out = torch.empty(N, Ho, Wo, cout, dtype=torch.float32, device=dev)
     b = conv.bias.detach().float().contiguous() if bias and conv.bias is not None else None
@@ -197,12 +203,12 @@ def conv_rows_ok(x: _Pair, conv: torch.nn.Conv2d) -> bool:
             and conv.padding == (1, 1) and fill >= 0.75 and os.environ.get("PIPS_B200_CONV_ROWS", "1") != "0")
 
 
-def conv_rows(x: _Pair, conv: torch.nn.Conv2d):
+def conv_rows(x: _Pair, conv: torch.nn.Conv2d, w=None):
     """-> (out (N,H,W,64) fp32, InstanceNorm statistics (N,2,64) of out): the statistics come from partial sums the
     convolution's epilogue accumulates, so no separate pass reads the output."""
     lib = L.load()
     N, H, W = x.shape
-    w_hi, w_lo = _packed_weight(conv)
+    w_hi, w_lo = _packed_weight(conv) if w is None else w
     dev = x.hi.device
     out = torch.empty(N, H, W, 64, dtype=torch.float32, device=dev)
     chunks = lib.pips_conv_rows_chunks(H, W)
@@ -215,14 +221,14 @@ def conv_rows(x: _Pair, conv: torch.nn.Conv2d):
     return out, st
 
 
-def _conv_stats(ops: _Ops, x: _Pair, conv: torch.nn.Conv2d):
+def _conv_stats(ops: _Ops, x: _Pair, conv: torch.nn.Conv2d, w=None):
     """Convolution feeding an InstanceNorm: (output, statistics)."""
     if conv_rows_ok(x, conv):
-        return conv_rows(x, conv)
+        return conv_rows(x, conv, w)
     if os.environ.get("PIPS_B200_CONV_STATS", "1") == "0":      # separate statistics pass (round 1), for A/B
-        y = conv_tc(x, conv)
+        y = conv_tc(x, conv, w=w)
         return y, ops.stats(y)
-    return conv_tc(x, conv, stats=True)
+    return conv_tc(x, conv, stats=True, w=w)
 
 
 def _apply_pair(ops: _Ops, y, stats, r=None, stats_r=None, relu_main=True, relu_out=False, plain=False):
@@ -236,21 +242,26 @@ def _apply_pair(ops: _Ops, y, stats, r=None, stats_r=None, relu_main=True, relu_
     return out_p, pair
 
 
-def _packed_stem_weight(conv: torch.nn.Conv2d):
+def pack_stem_weight(w: torch.Tensor):
     """7x7x3 stem (Cout,3,7,7) -> (64, 4*64) bf16 (hi, lo) for the 4x1 convolution over pips_stem_pack's row-pair pixels:
     tap d (row pair) major, then [filter row 2d: k = s*3 + colour, 21 of 32 | filter row 2d+1: same; row 7 does not exist: 0]."""
+    lib = L.load()
+    cout = w.shape[0]
+    rows = torch.zeros(64, 8, 32, dtype=torch.float32, device=w.device)                    # [co][filter row r][s*3+ci]
+    rows[:cout, :7, :21] = w.detach().float().permute(0, 2, 3, 1).reshape(cout, 7, 21)
+    packed = rows.reshape(64, 4 * 64).contiguous()                                          # (r = 2d, 2d+1) -> 64 channels of tap d
+    hi = torch.empty_like(packed, dtype=torch.bfloat16)
+    lo = torch.empty_like(packed, dtype=torch.bfloat16)
+    L.check(lib.pips_split_bf16(L.ptr(packed), L.ptr(hi), L.ptr(lo), packed.numel(), _st()), "pips_split_bf16")
+    return hi, lo
+
+
+def _packed_stem_weight(conv: torch.nn.Conv2d):
+    """pack_stem_weight of conv.weight, cached per weight version."""
     w = conv.weight
     key = (w.data_ptr(), w._version)
     if getattr(conv, "_wstem_key", None) != key:
-        lib = L.load()
-        cout = w.shape[0]
-        rows = torch.zeros(64, 8, 32, dtype=torch.float32, device=w.device)                    # [co][filter row r][s*3+ci]
-        rows[:cout, :7, :21] = w.detach().float().permute(0, 2, 3, 1).reshape(cout, 7, 21)
-        packed = rows.reshape(64, 4 * 64).contiguous()                                          # (r = 2d, 2d+1) -> 64 channels of tap d
-        hi = torch.empty_like(packed, dtype=torch.bfloat16)
-        lo = torch.empty_like(packed, dtype=torch.bfloat16)
-        L.check(lib.pips_split_bf16(L.ptr(packed), L.ptr(hi), L.ptr(lo), packed.numel(), _st()), "pips_split_bf16")
-        conv._wstem = (hi, lo)
+        conv._wstem = pack_stem_weight(w)
         conv._wstem_key = key
     return conv._wstem
 
@@ -294,20 +305,17 @@ def fnet_tc(enc: Encoder, rgb: torch.Tensor) -> torch.Tensor:
         return _fnet_tc(enc, rgb)
 
 
-def _fnet_tc(enc: Encoder, rgb: torch.Tensor) -> torch.Tensor:
+def stem_tc(rgb: torch.Tensor, w):
+    """The stem's convolution as fnet_tc runs it: rgb (N,3,H,W) contiguous, 0..255, and the pack_stem_weight pack w ->
+    (the pips_stem_pack operand, the (N,Ho,Wo,64) output before its InstanceNorm, that InstanceNorm's statistics).
+    The backward of torch_path.encoder_cuda recomputes the stem through this same function."""
     lib = L.load()
-    LAUNCHES[0] = 0
-    rgb = rgb.contiguous()
-    ops = _Ops(rgb.device)
     N, _, H, W = rgb.shape
-    H8, W8 = H // enc.stride, W // enc.stride
-    x = rgb
-
     Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
     unf = _Pair(N, Ho + 3, Wo, 64, rgb.device)                   # row pairs (2j-3, 2j-2) x 7 column taps x 3 colours
     L.check(lib.pips_stem_pack(L.ptr(rgb), 0 if rgb.dtype == torch.float32 else 1, N, H, W, L.ptr(unf.hi), L.ptr(unf.lo), _st()),
             "pips_stem_pack")
-    w_hi, w_lo = _packed_stem_weight(enc.conv1)
+    w_hi, w_lo = w
     y = torch.empty(N, Ho, Wo, 64, dtype=torch.float32, device=rgb.device)
     chunks = lib.pips_conv_tc_chunks(Ho + 3, Wo, 4, 1, 1, 1, 0, 0)
     partial = torch.empty(N, chunks, 3, 64, dtype=torch.float32, device=rgb.device)
@@ -316,30 +324,50 @@ def _fnet_tc(enc: Encoder, rgb: torch.Tensor) -> torch.Tensor:
                                    None, L.ptr(y), L.ptr(partial), _st()), "pips_conv_tc_stats")
     L.check(lib.pips_inorm_finalize(L.ptr(partial), N, chunks, Ho * Wo, 64, L.ptr(s_stem), _st()), "pips_inorm_finalize")
     LAUNCHES[0] += 3                                   # stem_pack + stem conv + statistics finalize
+    return unf, y, s_stem
+
+
+def _fnet_tc(enc: Encoder, rgb: torch.Tensor, packs=None, keep=None) -> torch.Tensor:
+    """``packs``: {conv module: (hi, lo)} filter packs to use instead of the modules' caches (torch_path.encoder_cuda);
+    ``keep``: a list that receives the block boundaries -- the stem output and every ResBlock output, fp32."""
+    lib = L.load()
+    LAUNCHES[0] = 0
+    rgb = rgb.contiguous()
+    ops = _Ops(rgb.device)
+    N, _, H, W = rgb.shape
+    H8, W8 = H // enc.stride, W // enc.stride
+    x = rgb
+
+    _, y, s_stem = stem_tc(rgb, _packed_stem_weight(enc.conv1) if packs is None else packs[enc.conv1])
     X, XP = _apply_pair(ops, y, s_stem, relu_main=True, plain=True)
+    pk = (lambda conv: None) if packs is None else packs.__getitem__
+    if keep is not None:
+        keep.append(X)
 
     ctot = 64 + 96 + 128 + 128
     cat = _Pair(N, H8, W8, ctot, x.device)
     c_off = 0
     for i in range(1, 5):
         for blk in getattr(enc, f"layer{i}"):
-            y1, s1 = _conv_stats(ops, XP, blk.conv1)
+            y1, s1 = _conv_stats(ops, XP, blk.conv1, pk(blk.conv1))
             _, AP = _apply_pair(ops, y1, s1, relu_main=True)
-            y2, s2 = _conv_stats(ops, AP, blk.conv2)
+            y2, s2 = _conv_stats(ops, AP, blk.conv2, pk(blk.conv2))
             if blk.downsample is not None:
-                d, sd = _conv_stats(ops, XP, blk.downsample[0])
+                d, sd = _conv_stats(ops, XP, blk.downsample[0], pk(blk.downsample[0]))
                 X, XP = _apply_pair(ops, y2, s2, r=d, stats_r=sd, relu_main=True, relu_out=True, plain=True)
             else:
                 X, XP = _apply_pair(ops, y2, s2, r=X, relu_main=True, relu_out=True, plain=True)
+            if keep is not None:
+                keep.append(X)
         Ns, Hs, Ws, Cs = X.shape
         L.check(ops.lib.pips_resize_pair(L.ptr(X), Ns, Hs, Ws, Cs, L.ptr(cat.hi), L.ptr(cat.lo), H8, W8, cat.Cp, c_off, _st()),
                 "pips_resize_pair")
         LAUNCHES[0] += 1
         c_off += Cs
 
-    y, sy = _conv_stats(ops, cat, enc.conv2)
+    y, sy = _conv_stats(ops, cat, enc.conv2, pk(enc.conv2))
     _, AP = _apply_pair(ops, y, sy, relu_main=True)
-    return conv_tc(AP, enc.conv3, bias=True)
+    return conv_tc(AP, enc.conv3, bias=True, w=pk(enc.conv3))
 
 
 # ---- the whole encoder as one CUDA graph per input shape ---------------------------------------------------

@@ -28,7 +28,15 @@ Extra, optional knobs (keyword-only; the reference signature is unchanged):
               and backward run on sm_90a kernels (wgmma GEMMs, recompute per block from the saved block inputs) in
               bf16x3 arithmetic -- always, since PIPS_B200_PRECISION is an inference knob.  CPU tensors keep the module.
               Independent of loss_path; loss_path='fused', mixer_path='cuda' puts both on the CUDA kernels
-Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET, PIPS_B200_LOSSES, PIPS_B200_MIXER.
+  encoder_path 'torch' (default) or 'cuda': where the differentiable path runs the feature encoder.  'torch' is the
+              Encoder module under autograd in strict fp32 (Pips.encode(torch_only=True)), which keeps every convolution
+              output, InstanceNorm input and ReLU output until the backward; 'cuda' is torch_path.encoder_cuda, one
+              autograd node whose forward (the kernels of fnet_tc, same bits) and backward (wgmma weight and input
+              gradients, recompute per ResBlock from the saved block boundaries) run on sm_90a in bf16x3.  CPU tensors and
+              an rgbs that requires grad keep the module; plain inference is unaffected.  Independent of loss_path and
+              mixer_path
+Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET, PIPS_B200_LOSSES, PIPS_B200_MIXER,
+PIPS_B200_ENCODER.
 """
 from __future__ import annotations
 
@@ -105,7 +113,7 @@ def _conv_math(allow_tf32: bool):
 class Pips(nn.Module):
     def __init__(self, S=8, stride=8, *, precision: Optional[str] = None, feat_dtype: Optional[str] = None,
                  fnet_mode: Optional[str] = None, max_seqs: int = 32768, loss_path: Optional[str] = None,
-                 mixer_path: Optional[str] = None):
+                 mixer_path: Optional[str] = None, encoder_path: Optional[str] = None):
         super().__init__()
         self.S = S
         self.stride = stride
@@ -138,6 +146,10 @@ class Pips(nn.Module):
         self.mixer_path = mixer_path or os.environ.get("PIPS_B200_MIXER", "torch")
         if self.mixer_path not in ("torch", "cuda"):
             raise ValueError("mixer_path must be 'torch' (the DeltaBlock module under autograd) or 'cuda' (its forward and "
+                             "backward on the sm_90a kernels, bf16x3)")
+        self.encoder_path = encoder_path or os.environ.get("PIPS_B200_ENCODER", "torch")
+        if self.encoder_path not in ("torch", "cuda"):
+            raise ValueError("encoder_path must be 'torch' (the Encoder module under autograd) or 'cuda' (its forward and "
                              "backward on the sm_90a kernels, bf16x3)")
 
     # ------------------------------------------------------------------ configuration

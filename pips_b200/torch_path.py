@@ -5,7 +5,8 @@ tensors live (it is what ``train.py`` / ``test_on_flt.py`` exercise) and keeps t
 semantics, including the dense score map ``fcps`` that only the score-map loss consumes -- except with
 ``model.loss_path == 'fused'`` on CUDA tensors, where ``fused_score_map_loss`` computes that loss and its gradients
 without ``fcps``, and with ``model.mixer_path == 'cuda'`` on CUDA tensors, where ``delta_block_cuda`` runs the
-DeltaBlock mixer forward and backward on the sm_90a kernels.
+DeltaBlock mixer forward and backward on the sm_90a kernels, and with ``model.encoder_path == 'cuda'`` on CUDA tensors
+that need no gradient, where ``encoder_cuda`` does the same for the feature encoder.
 
 Not used -- and not a fallback -- for plain inference: that path is CUDA-only (pips.py).
 """
@@ -413,6 +414,277 @@ def delta_block_cuda(delta_block, x):
     return _DeltaBlockFn.apply(save, x.contiguous(), *params)
 
 
+# Encoder convolutions in named_parameters order; each contributes (weight, bias) to encoder_cuda's inputs
+ENCODER_CONVS = ("conv1",) + tuple(
+    f"layer{i}.{j}.{c}" for i in range(1, 5) for j in (0, 1)
+    for c in ("conv1", "conv2") + (("downsample.0",) if i > 1 and j == 0 else ())) + ("conv2", "conv3")
+ENCODER_PARAMS = tuple(f"{c}.{p}" for c in ENCODER_CONVS for p in ("weight", "bias"))
+_ENCODER_SHAPES = None
+
+
+def _encoder_params(fnet):
+    """The 44 parameter tensors of the Encoder ``fnet`` in ENCODER_PARAMS order, by attribute lookup (nn.DataParallel
+    replicas list no parameters), and its convolution modules by name."""
+    global _ENCODER_SHAPES
+    if _ENCODER_SHAPES is None:
+        from .encoder import Encoder
+        with torch.device("meta"):
+            _ENCODER_SHAPES = {n: tuple(p.shape) for n, p in Encoder().named_parameters()}
+    params, convs = [], {}
+    for n in ENCODER_PARAMS:
+        mod_name, attr = n.rsplit(".", 1)
+        try:
+            mod = fnet.get_submodule(mod_name)
+            t = getattr(mod, attr)
+        except AttributeError:
+            mod = t = None
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != _ENCODER_SHAPES[n]:
+            raise ValueError(f"encoder_cuda: the module is not a BasicEncoder(output_dim=128) (at {n})")
+        params.append(t)
+        convs[mod_name] = mod
+    return params, convs
+
+
+class _EncRun:
+    """Launch helpers of one encoder_cuda backward: device, stream and the raw entry points."""
+
+    def __init__(self, dev):
+        from . import _lib as L
+        from . import encoder_fast as E
+        self.L, self.E, self.lib, self.dev = L, E, L.load(), dev
+        self.st = torch.cuda.current_stream(dev).cuda_stream
+        self.ops = E._Ops(dev)
+
+    def pair(self, N, H, W, C):
+        return self.E._Pair(N, H, W, C, self.dev)
+
+    def pair_of(self, x):
+        """the (hi, lo) pair of an fp32 activation: the bits pips_inorm_apply_pair wrote for it in the forward"""
+        return self.E._apply_pair(self.ops, x, None, relu_main=False)[1]
+
+    def wgrad(self, dy, step, x, conv_w, R, S, stride, pad):
+        """dL/dW (Cout, Cin, R, S) of a convolution over the pair x, from the pair dy"""
+        L = self.L
+        N, H, W = x.shape
+        cout, cin = conv_w.shape[:2]
+        Ho, Wo = (H + 2 * pad - R) // stride + 1, (W + 2 * pad - S) // stride + 1
+        K = R * S * x.Cp
+        dw = torch.empty(cout, K, device=self.dev)
+        n = self.lib.pips_conv_wgrad_scratch_floats(N, Ho, Wo, cout, K)
+        scratch = torch.empty(n, device=self.dev) if n else None
+        L.check(self.lib.pips_conv_wgrad(L.ptr(dy.hi), L.ptr(dy.lo), dy.Cp, step, L.ptr(x.hi), L.ptr(x.lo), N, H, W, x.Cp, cout, R, S,
+                                         stride, stride, pad, pad, L.ptr(scratch), L.ptr(dw), self.st), "pips_conv_wgrad")
+        return dw.view(cout, R, S, x.Cp)[..., :cin].permute(0, 3, 1, 2)
+
+    def dgrad(self, dy, conv_w, pad, rows=None):
+        """input gradient of a convolution: pips_conv_tc over the pair dy (zero-dilated for stride 2) with the weight
+        flipped in (r, s) and transposed in channels; ``rows`` = (first, end) input channel"""
+        L = self.L
+        wt = conv_w.detach().flip(2, 3).transpose(0, 1)
+        if rows is not None:
+            wt = wt[rows[0]:rows[1]]
+        hi, lo = self.E.pack_conv_weight(wt)
+        N, H, W = dy.shape
+        cout, _, R, S = wt.shape
+        out = torch.empty(N, H, W, cout, device=self.dev)
+        L.check(self.lib.pips_conv_tc(L.ptr(dy.hi), L.ptr(dy.lo), N, H, W, dy.Cp, L.ptr(hi), L.ptr(lo), cout, R, S, 1, pad, None,
+                                      L.ptr(out), self.st), "pips_conv_tc")
+        return out
+
+    def inorm_grad(self, y, stats, addends, r=None, stats_r=None, relu_main=True, relu_out=False, dil=None, skip=False):
+        """-> (dy pair, g after the output ReLU's mask or None); dil = (H, W) of a zero-dilated output grid"""
+        L = self.L
+        N, H, W, C = y.shape
+        dy = self.pair(N, *(dil or (H, W)), C)
+        g_out = torch.empty_like(y) if skip else None
+        scratch = torch.empty(self.lib.pips_inorm_grad_scratch_floats(N, H * W, C), device=self.dev)
+        g = list(addends) + [None] * (3 - len(addends))
+        L.check(self.lib.pips_inorm_grad(L.ptr(y), L.ptr(stats), L.ptr(r), L.ptr(stats_r), int(relu_main), int(relu_out),
+                                         *(L.ptr(t) for t in g), N, H, W, C, L.ptr(scratch), L.ptr(dy.hi), L.ptr(dy.lo), dy.Cp,
+                                         *(dil or (0, 0)), L.ptr(g_out), self.st), "pips_inorm_grad")
+        return dy, g_out
+
+
+class _EncoderFn(torch.autograd.Function):
+    """Encoder.forward on the sm_90a kernels of fnet_tc, bf16x3, with the 44 parameters as explicit inputs.  The forward
+    saves the block boundaries only (the stem output and the output of every ResBlock, fp32) and the image; the backward
+    recomputes each block from its saved input with the forward's kernels -- so the recomputed activations are the
+    forward's bits -- and runs its backward last block first: ReLU masks and InstanceNorm backward (pips_inorm_grad),
+    weight gradients (pips_conv_wgrad), input gradients (pips_conv_tc over flipped weights), the resize adjoint of the
+    head's input (pips_resize_grad).
+
+    The biases of the 21 convolutions that feed an InstanceNorm get an exact zero gradient: InstanceNorm removes a
+    per-channel constant again, so the forward never adds them (conv_tc(..., bias=False)) and the function computed
+    does not depend on them.  conv3's bias gets the column sum of the output gradient."""
+
+    @staticmethod
+    def forward(ctx, save, convs, rgb, *params):
+        from . import encoder_fast as E
+        dev = rgb.device
+        with torch.cuda.device(dev):
+            ws = dict(zip(ENCODER_PARAMS, params))
+            packs = {}
+            for name in ENCODER_CONVS:
+                w = ws[name + ".weight"].detach()
+                packs[convs[name]] = E.pack_stem_weight(w) if name == "conv1" else E.pack_conv_weight(w)
+            keep = [] if save else None
+            out = E._fnet_tc(convs[""], rgb, packs=packs, keep=keep)
+        if save:
+            ctx.save_for_backward(rgb, *keep, *(ws[c + ".weight"] for c in ENCODER_CONVS))
+            ctx.convs, ctx.packs = convs, {n: packs[convs[n]] for n in ENCODER_CONVS}
+            ctx.shapes = [p.shape for p in params]
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        rgb, *rest = ctx.saved_tensors
+        X, wl = rest[:9], dict(zip(ENCODER_CONVS, rest[9:]))
+        convs, packs = ctx.convs, ctx.packs
+        dev = rgb.device
+        g = {}
+        need = dict(zip(ENCODER_PARAMS, ctx.needs_input_grad[3:]))       # weight gradients of frozen convolutions are skipped
+        with torch.cuda.device(dev):
+            run = _EncRun(dev)
+            L, lib, st, ops = run.L, run.lib, run.st, run.ops
+            E = run.E
+            N, H8, W8, _ = gout.shape
+            gout = gout.contiguous()
+            # ---- head: fmaps = conv3(relu(IN(conv2(cat)))) + b3
+            widths = (64, 96, 128, 128)
+            cat = run.pair(N, H8, W8, sum(widths))
+            c_off = 0
+            for l, C in enumerate(widths):
+                Xl = X[2 * l + 2]
+                L.check(lib.pips_resize_pair(L.ptr(Xl), N, Xl.shape[1], Xl.shape[2], C, L.ptr(cat.hi), L.ptr(cat.lo), H8, W8, cat.Cp,
+                                             c_off, st), "pips_resize_pair")
+                c_off += C
+            yh, sh = E._conv_stats(ops, cat, convs["conv2"], packs["conv2"])
+            _, ah = E._apply_pair(ops, yh, sh, relu_main=True)
+            gp = run.pair(N, H8, W8, 128)
+            L.check(lib.pips_split_bf16(L.ptr(gout), L.ptr(gp.hi), L.ptr(gp.lo), gout.numel(), st), "pips_split_bf16")
+            if need["conv3.weight"]:
+                g["conv3.weight"] = run.wgrad(gp, 1, ah, wl["conv3"], 1, 1, 1, 0)
+            if need["conv3.bias"]:
+                M = N * H8 * W8
+                n = lib.pips_colsum_scratch_floats(M, 128)
+                scratch = torch.empty(n, device=dev) if n else None
+                b3 = torch.empty(128, device=dev)
+                L.check(lib.pips_colsum(L.ptr(gout), None, None, 128, M, 128, L.ptr(scratch), L.ptr(b3), st), "pips_colsum")
+                g["conv3.bias"] = b3
+            dah = run.dgrad(gp, wl["conv3"], 0)
+            del gp, ah
+            dyh, _ = run.inorm_grad(yh, sh, [dah])
+            del dah, yh
+            if need["conv2.weight"]:
+                g["conv2.weight"] = run.wgrad(dyh, 1, cat, wl["conv2"], 3, 3, 1, 1)
+            del cat
+            # conv_tc covers 256 output channels: the 416 of the head's input gradient in two launches, split between
+            # layer2 and layer3 so that every layer's slice lies in one of them
+            dcat = (run.dgrad(dyh, wl["conv2"], 1, rows=(0, 160)), run.dgrad(dyh, wl["conv2"], 1, rows=(160, 416)))
+            del dyh
+            gl = []
+            for l, (part, off) in enumerate(((0, 0), (0, 64), (1, 0), (1, 128))):
+                Xl = X[2 * l + 2]
+                d = torch.empty_like(Xl)
+                src = dcat[part]
+                L.check(lib.pips_resize_grad(L.ptr(src), src.shape[-1], off, N, H8, W8, L.ptr(d), Xl.shape[1], Xl.shape[2], Xl.shape[3],
+                                             st), "pips_resize_grad")
+                gl.append(d)
+            del dcat
+            # ---- the 8 ResBlocks, last first; `addends` holds the gradient of the current block's output
+            addends = [gl[3]]
+            for b in reversed(range(8)):
+                i, j = b // 2 + 1, b % 2
+                q = f"layer{i}.{j}."
+                ds = i > 1 and j == 0
+                stride = 2 if ds else 1
+                x_in = X[b]
+                xp = run.pair_of(x_in)
+                y1, s1 = E._conv_stats(ops, xp, convs[q + "conv1"], packs[q + "conv1"])
+                _, a1 = E._apply_pair(ops, y1, s1, relu_main=True)
+                y2, s2 = E._conv_stats(ops, a1, convs[q + "conv2"], packs[q + "conv2"])
+                if ds:
+                    d, sd = E._conv_stats(ops, xp, convs[q + "downsample.0"], packs[q + "downsample.0"])
+                    r, sr = d, sd
+                else:
+                    r, sr = x_in, None
+                dy2, go = run.inorm_grad(y2, s2, addends, r=r, stats_r=sr, relu_out=True, skip=True)
+                del addends, y2
+                if need[q + "conv2.weight"]:
+                    g[q + "conv2.weight"] = run.wgrad(dy2, 1, a1, wl[q + "conv2"], 3, 3, 1, 1)
+                da1 = run.dgrad(dy2, wl[q + "conv2"], 1)
+                del dy2, a1
+                dil = tuple(x_in.shape[1:3]) if ds else None
+                dy1, _ = run.inorm_grad(y1, s1, [da1], dil=dil)
+                del da1, y1
+                if need[q + "conv1.weight"]:
+                    g[q + "conv1.weight"] = run.wgrad(dy1, stride, xp, wl[q + "conv1"], 3, 3, stride, 1)
+                dx1 = run.dgrad(dy1, wl[q + "conv1"], 1)
+                del dy1
+                if ds:
+                    dd, _ = run.inorm_grad(d, sd, [go], relu_main=False, dil=dil)
+                    del d, go
+                    if need[q + "downsample.0.weight"]:
+                        g[q + "downsample.0.weight"] = run.wgrad(dd, 2, xp, wl[q + "downsample.0"], 1, 1, 2, 0)
+                    addends = [dx1, run.dgrad(dd, wl[q + "downsample.0"], 0)]
+                    del dd
+                else:
+                    addends = [go, dx1]
+                if ds:
+                    addends.append(gl[i - 2])                 # the block's input is layer i-1's output
+                del xp
+            # ---- stem: X0 = relu(IN(conv1(image))); no gradient for the image
+            # the stem has no input gradient: with its weight frozen there is nothing left to do
+            if need["conv1.weight"]:
+                Ho, Wo = X[0].shape[1:3]
+                unf, y0, s0 = E.stem_tc(rgb, packs["conv1"])
+                dy0, _ = run.inorm_grad(y0, s0, addends)
+                del addends, y0
+                K = 4 * 64
+                dw = torch.empty(64, K, device=dev)
+                n = lib.pips_conv_wgrad_scratch_floats(N, Ho, Wo, 64, K)
+                scratch = torch.empty(n, device=dev) if n else None
+                L.check(lib.pips_conv_wgrad(L.ptr(dy0.hi), L.ptr(dy0.lo), dy0.Cp, 1, L.ptr(unf.hi), L.ptr(unf.lo), N, Ho + 3, Wo, 64,
+                                            64, 4, 1, 1, 1, 0, 0, L.ptr(scratch), L.ptr(dw), st), "pips_conv_wgrad")
+                # (64, 4*64) over the row pairs -> (64, 3, 7, 7): k = filter row * 32 + s*3 + colour (pack_stem_weight)
+                g["conv1.weight"] = dw.view(64, 8, 32)[:, :7, :21].reshape(64, 7, 7, 3).permute(0, 3, 1, 2)
+        grads = []
+        for n_, sh_ in zip(ENCODER_PARAMS, ctx.shapes):
+            t = g.get(n_)
+            grads.append(None if not need[n_] else torch.zeros(sh_, device=dev) if t is None else t.contiguous())
+        return (None, None, None, *grads)
+
+
+def encoder_cuda(fnet, rgbs):
+    """``Pips.encode`` (nets/pips.py:436-445, the BasicEncoder) on the sm_90a kernels of fnet_tc, differentiable in the
+    encoder's 44 parameters (not in the image): rgbs (B,S,3,H,W) CUDA with values 0..255 -> fmaps (B,S,128,H/stride,
+    W/stride) fp32, a view of the channels-last result like Pips.encode's.  The forward has the bits of fnet_tc; the
+    arithmetic is bf16x3 whatever PIPS_B200_PRECISION or fnet_mode say.  The filters are packed from the parameters on
+    every call, without the modules' caches, and no CUDA graph is used: ``fnet`` may be an nn.DataParallel replica run
+    from a worker thread.  With gradients on, the forward keeps the block boundaries only (about 49 MiB per 384x512
+    frame); under no_grad, nothing but its output."""
+    if not isinstance(rgbs, torch.Tensor) or not rgbs.is_cuda:
+        raise RuntimeError("encoder_cuda runs on the CUDA kernels only; use the Encoder module for CPU tensors")
+    if rgbs.dim() != 5 or rgbs.shape[2] != 3:
+        raise ValueError(f"encoder_cuda: rgbs must be (B, S, 3, H, W); got {tuple(rgbs.shape)}")
+    if rgbs.requires_grad:
+        raise ValueError("encoder_cuda computes no gradient for the image; use the Encoder module when rgbs requires grad")
+    B, S, C, H, W = rgbs.shape
+    params, convs = _encoder_params(fnet)
+    stride = fnet.stride
+    if H // stride == 0 or W // stride == 0:
+        raise ValueError(f"encoder_cuda: a {H}x{W} frame has no feature pixel at stride {stride}")
+    if any(p.device != rgbs.device or p.dtype != torch.float32 for p in params):
+        raise ValueError("encoder_cuda: the parameters must be float32 on rgbs's device")
+    convs[""] = fnet
+    raw = rgbs if rgbs.dtype in (torch.float32, torch.bfloat16) else rgbs.float()
+    raw = raw.reshape(B * S, C, H, W).contiguous()
+    save = torch.is_grad_enabled() and any(p.requires_grad for p in params)
+    f = _EncoderFn.apply(save, convs, raw, *params)
+    H8, W8 = f.shape[1:3]
+    return f.reshape(B, S, H8, W8, f.shape[-1]).permute(0, 1, 4, 2, 3)
+
+
 def sample_clamped(im, x, y):
     """utils/samp.py:5-78: bilinear sample with clamped indices and unclamped weights -> (B,N,C)."""
     B, C, H, W = im.shape
@@ -446,7 +718,10 @@ def forward_torch(model, xys, rgbs, coords_init=None, feat_init=None, iters=3, t
     H8, W8 = H // stride, W // stride
     L, r = model.corr_levels, model.corr_radius
 
-    fmaps = model.encode(rgbs, torch_only=True)          # no CUDA graphs / custom kernels on this path (DataParallel-safe)
+    if getattr(model, "encoder_path", "torch") == "cuda" and rgbs.is_cuda and not rgbs.requires_grad:
+        fmaps = encoder_cuda(model.fnet, rgbs)                # sm_90a forward and backward, no CUDA graphs (DataParallel-safe)
+    else:
+        fmaps = model.encode(rgbs, torch_only=True)      # no CUDA graphs / custom kernels on this path (DataParallel-safe)
     if sw is not None and getattr(sw, "save_this", False) and hasattr(sw, "summ_feats"):
         sw.summ_feats("1_model/0_fmaps", fmaps.unbind(1))                       # nets/pips.py:447-448
 

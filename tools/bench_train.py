@@ -1,8 +1,11 @@
 """Training-path timings on one GPU: the DeltaBlock mixer's forward + backward on the torch module against
 torch_path.delta_block_cuda, each new backward kernel alone, and a whole training step (is_train=True, the backward of the
-three losses) with loss_path='fused' and mixer_path 'torch' against 'cuda'.
+three losses) with loss_path='fused' and mixer_path 'torch' against 'cuda'.  The feature encoder likewise: its forward +
+backward on the torch module (strict fp32, as forward_torch runs it) against torch_path.encoder_cuda at 32 and 128 frames
+of 384 x 512, its backward kernels alone, and training steps with encoder_path 'torch' against 'cuda' (loss_path='fused',
+mixer_path='cuda') at B=4 and at train.py's single-GPU default B=16 (N=768, 4 iterations).
 
-    python tools/bench_train.py [--reps 5] [--skip-step]
+    python tools/bench_train.py [--reps 5] [--skip-step] [--only mixer|encoder]
 
 Shapes: train.py's per-GPU shape (B=4, N=768, 4 iterations, 8 x 384 x 512, stride 8: R = 3072 tracks, M = 24576 mixer
 rows) and BASELINE cfg 2 (N=1024, 6 iterations: M = 32768).  Medians of --reps timed runs after two warm-ups, CUDA
@@ -172,18 +175,142 @@ def bench_step(reps):
             torch.cuda.empty_cache()
 
 
+ENC_LAYERS = [  # (name, Cin, Cout, R, stride, pad, input size at 384 x 512): the convolutions of BasicEncoder
+    ("stem 4x1 over row pairs", 64, 64, 4, 1, 0, (195, 256)),
+    ("layer1 3x3 64->64", 64, 64, 3, 1, 1, (192, 256)),
+    ("layer2.0.conv1 3x3/2 64->96", 64, 96, 3, 2, 1, (192, 256)),
+    ("layer2.0.downsample 1x1/2", 64, 96, 1, 2, 0, (192, 256)),
+    ("layer2 3x3 96->96", 96, 96, 3, 1, 1, (96, 128)),
+    ("layer3.0.conv1 3x3/2 96->128", 96, 128, 3, 2, 1, (96, 128)),
+    ("layer3 3x3 128->128", 128, 128, 3, 1, 1, (48, 64)),
+    ("layer4 3x3 128->128", 128, 128, 3, 1, 1, (24, 32)),
+    ("head conv2 3x3 416->256", 416, 256, 3, 1, 1, (48, 64)),
+    ("head conv3 1x1 256->128", 256, 128, 1, 1, 0, (48, 64)),
+]
+
+
+def bench_encoder_kernels(reps, frames=32):
+    from pips_b200 import encoder_fast as E
+    lib = L.load()
+    st = torch.cuda.current_stream().cuda_stream
+
+    def pair(N, H, W, C):
+        p = E._Pair(N, H, W, C, DEV)
+        v = torch.randn(N, H, W, p.Cp, device=DEV)
+        L.check(lib.pips_split_bf16(L.ptr(v), L.ptr(p.hi), L.ptr(p.lo), v.numel(), st))
+        return p
+
+    N = frames
+    for name, cin, cout, R, stride, pad, (H, W) in ENC_LAYERS:
+        S = 1 if name.startswith("stem") else R
+        Ho, Wo = (H + 2 * pad - R) // stride + 1, (W + 2 * pad - S) // stride + 1
+        x, dy = pair(N, H, W, cin), pair(N, Ho, Wo, cout)
+        K = R * S * x.Cp
+        dw = torch.empty(cout, K, device=DEV)
+        n = lib.pips_conv_wgrad_scratch_floats(N, Ho, Wo, cout, K)
+        sc = torch.empty(max(n, 1), device=DEV)
+        fn = lambda: L.check(lib.pips_conv_wgrad(L.ptr(dy.hi), L.ptr(dy.lo), dy.Cp, 1, L.ptr(x.hi), L.ptr(x.lo), N, H, W, x.Cp, cout,
+                                                 R, S, stride, stride, pad, pad, L.ptr(sc), L.ptr(dw), st))
+        ms = timed(fn, reps, 3)
+        flop = 2.0 * N * Ho * Wo * cout * (7 * 7 * 3 if name.startswith("stem") else R * S * cin)
+        print(f"conv_wgrad {name:30s} {N} frames: {ms * 1e3:8.1f} us, {flop / ms / 1e9:6.1f} TFLOP/s useful")
+        del x, dy, dw, sc
+    for C, (H, W), dil in ((64, (192, 256), None), (96, (96, 128), (192, 256)), (256, (48, 64), None)):
+        y = torch.randn(N, H, W, C, device=DEV)
+        stt = torch.rand(N, 2, C, device=DEV)
+        g0 = torch.randn_like(y)
+        Hd, Wd = dil or (H, W)
+        out = E._Pair(N, Hd, Wd, C, DEV)
+        sc = torch.empty(lib.pips_inorm_grad_scratch_floats(N, H * W, C), device=DEV)
+        fn = lambda: L.check(lib.pips_inorm_grad(L.ptr(y), L.ptr(stt), None, None, 1, 0, L.ptr(g0), None, None, N, H, W, C, L.ptr(sc),
+                                                 L.ptr(out.hi), L.ptr(out.lo), out.Cp, *(dil or (0, 0)), None, st))
+        ms = timed(fn, reps, 3)
+        print(f"inorm_grad {N}x{H}x{W}x{C}{' dilated' if dil else ''}: {ms * 1e3:8.1f} us")
+    g = torch.randn(N, 48, 64, 416, device=DEV)
+    for (Hs, Ws, C, off) in ((192, 256, 64, 0), (96, 128, 96, 64), (48, 64, 128, 160), (24, 32, 128, 288)):
+        out = torch.empty(N, Hs, Ws, C, device=DEV)
+        fn = lambda: L.check(lib.pips_resize_grad(L.ptr(g), 416, off, N, 48, 64, L.ptr(out), Hs, Ws, C, st))
+        print(f"resize_grad {Hs}x{Ws}x{C} <- 48x64: {timed(fn, reps, 3) * 1e3:8.1f} us")
+
+
+def bench_encoder(reps):
+    from pips_b200.encoder import Encoder
+    enc = Encoder(output_dim=128, stride=8).to(DEV)
+    old = strict_fp32()
+    try:
+        for frames in (32, 128):
+            rgbs = po.smooth_video(frames // 8, 8, 384, 512, seed=1).to(DEV).float()
+            dfm = torch.randn(frames // 8, 8, 128, 48, 64, device=DEV)
+            for name in ("torch", "cuda"):
+                def step():
+                    enc.zero_grad(set_to_none=True)
+                    if name == "cuda":
+                        f = torch_path.encoder_cuda(enc, rgbs)
+                    else:
+                        x = 2 * (rgbs / 255.0) - 1.0
+                        f = enc(x.flatten(0, 1)).view(dfm.shape)
+                    f.backward(dfm)
+                try:
+                    ms = timed(step, reps, warm=1)
+                    gib = peak_of(step)
+                    print(f"encoder fwd+bwd {frames} frames 384x512 {name:5s}: {ms:8.1f} ms, peak {gib:6.2f} GiB above inputs")
+                except torch.cuda.OutOfMemoryError:
+                    print(f"encoder fwd+bwd {frames} frames 384x512 {name:5s}: does not fit in "
+                          f"{torch.cuda.get_device_properties(0).total_memory / 2**30:.0f} GiB")
+                torch.cuda.empty_cache()
+            del rgbs, dfm
+    finally:
+        torch.backends.cudnn.enabled, torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
+
+
+def bench_encoder_step(reps):
+    for B in (4, 16):
+        N, iters = 768, 4
+        rgbs = po.smooth_video(B, 8, 384, 512, seed=1).to(DEV)
+        xys = po.random_queries(B, N, 384, 512, seed=2).to(DEV)
+        g = torch.Generator().manual_seed(3)
+        tg = (xys.cpu()[:, None] + torch.cumsum(torch.randn(B, 8, N, 2, generator=g) * 3.0, 1)).to(DEV)
+        vg = torch.ones(B, 8, N, device=DEV)
+        va = torch.ones(B, 8, N, device=DEV)
+        for encoder in ("torch", "cuda"):
+            m = Pips(S=8, stride=8, loss_path="fused", mixer_path="cuda", encoder_path=encoder).to(DEV).train()
+            m.load_state_dict(po.init_state_dict(seed=3, head_scale=0.05))
+
+            def step():
+                m.zero_grad(set_to_none=True)
+                _, _, _, losses = m(xys, rgbs, iters=iters, trajs_g=tg, vis_g=vg, valids=va, is_train=True)
+                sum(losses).backward()
+            label = f"training step B={B}, N={N}, {iters} iterations (mixer cuda, fused loss), encoder {encoder:5s}"
+            try:
+                ms = timed(step, reps, warm=1)
+                gib = peak_of(step)
+                print(f"{label}: {ms:8.1f} ms, peak {gib:6.2f} GiB")
+            except torch.cuda.OutOfMemoryError:
+                print(f"{label}: does not fit in {torch.cuda.get_device_properties(0).total_memory / 2**30:.0f} GiB")
+            del m
+            torch.cuda.empty_cache()
+        del rgbs
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--skip-step", action="store_true")
+    ap.add_argument("--only", choices=("mixer", "encoder"))
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_train.py measures on the GPU; no CUDA device found")
     print(f"card: {card()}")
-    bench_kernels(args.reps)
-    bench_mixer(args.reps)
-    if not args.skip_step:
-        bench_step(args.reps)
+    if args.only != "encoder":
+        bench_kernels(args.reps)
+        bench_mixer(args.reps)
+        if not args.skip_step:
+            bench_step(args.reps)
+    if args.only != "mixer":
+        bench_encoder_kernels(args.reps)
+        bench_encoder(args.reps)
+        if not args.skip_step:
+            bench_encoder_step(args.reps)
 
 
 if __name__ == "__main__":
