@@ -34,6 +34,14 @@ bool encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, uint32_t rank, vo
                   const cuuint64_t* gstride_bytes, const cuuint32_t* box, const cuuint32_t* estride,
                   CUtensorMapSwizzle swizzle);
 
+// the tensor maps of a bf16 (hi, lo) pair of tensors with the same geometry
+inline bool encode_tiled_pair(CUtensorMap* map_hi, CUtensorMap* map_lo, const void* hi, const void* lo, uint32_t rank,
+                              const cuuint64_t* gdim, const cuuint64_t* gstride_bytes, const cuuint32_t* box,
+                              const cuuint32_t* estride, CUtensorMapSwizzle swizzle) {
+    return encode_tiled(map_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(hi), gdim, gstride_bytes, box, estride, swizzle) &&
+           encode_tiled(map_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(lo), gdim, gstride_bytes, box, estride, swizzle);
+}
+
 // ---- programmatic dependent launch (PDL).  Kernels of the per-iteration chain are launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's CTAs may become resident and run their
 // prologue (barrier init, tensor-map prefetch, weight staging into shared memory) while the previous
@@ -46,16 +54,33 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 
 bool pdl_enabled();          // PIPS_B200_PDL != "0" (abi.cu)
 
+// `pdl` = false: a plain launch
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+inline cudaError_t launch_ex(void (*kernel)(KArgs...), bool pdl, dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = pdl && pdl_enabled() ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+    return launch_ex(kernel, true, grid, block, smem, st, static_cast<Args&&>(args)...);
+}
+
+// A kernel with `smem` bytes of dynamic shared memory: sets the opt-in on the current device (once per device and
+// kernel), launches with PDL when `pdl` (see the RULE above) and reports a failure as `name`'s.
+template <auto Kernel, typename... Args>
+inline int launch_kernel(const char* name, bool pdl, dim3 grid, dim3 block, uint32_t smem, cudaStream_t st, Args&&... args) {
+    static bool smem_set[kMaxDevices] = {};
+    cudaError_t e = ensure_dyn_smem(Kernel, smem_set, static_cast<int>(smem));
+    if (e == cudaSuccess) e = launch_ex(Kernel, pdl, grid, block, smem, st, static_cast<Args&&>(args)...);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail_cuda(name, e);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 a, __nv_bfloat16 b) {

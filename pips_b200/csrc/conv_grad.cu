@@ -3,13 +3,17 @@
 //   dW[co, (r*S + s)*Cp + ci] = sum_{n, oy, ox} dY[n, oy, ox, co] * X[n, oy*sy + r - py, ox*sx + s - px, ci]
 //
 // An implicit GEMM with the pixels as the contraction index, on the pipeline of the dense weight-gradient GEMM
-// (gemm_tc.cu, pips_wgrad): a TMA producer warp, a ring of stages, two consumer warpgroups of 64 output channels each,
-// both operands MN-major with 64-byte swizzle.  A ring stage holds one tile of 32 output pixels (TH rows x TW columns
-// of one image): the 128 co of the tile as four {32 co, TW, TH, 1} boxes of dY, and the 128 k of the tile as four
-// {32 ci, TW, TH, 1} boxes of X, each at its filter tap's offset with the element strides set to the conv stride --
+// (gemm_tc.cu, pips_wgrad): a TMA producer warp, the shared ring (gemm_common.cuh), two consumer warpgroups of 64 output
+// channels each, both operands MN-major with 64-byte swizzle.  A ring stage holds one tile of 32 output pixels (TH rows x
+// TW columns of one image): the 128 co of the tile as four {32 co, TW, TH, 1} boxes of dY, and the 128 k of the tile as
+// four {32 ci, TW, TH, 1} boxes of X, each at its filter tap's offset with the element strides set to the conv stride --
 // the same 4-D box conv_tc loads for that tap.  Boxes outside the image are filled with zero by TMA, so padding needs
 // no code and no im2col buffer exists.  With dy_step = 2 the dY boxes read every other pixel of a zero-dilated
 // gradient (the layout the strided convolutions' input gradient needs), so the same buffer serves both.
+//
+// It is a kernel of its own, not a variant of gemm_tc_body's weight-gradient path: there the producer's box coordinates
+// are not kept in uniform registers, so each of a stage's 16 4-D loads goes through an elected-lane loop of register
+// moves, and with 6 MMAs per 32-pixel stage the producer sets the pace (16 % slower on layer1).  Here they are uniform.
 //
 // A work item is (128 co, 128 k, chunk of pixel tiles).  The chunk size depends on the geometry only; every chunk
 // writes its own partial dW, and the chunks are added in order by the column-sum kernel: no atomics, the same bits
@@ -43,24 +47,15 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_co
                   const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
                   const ConvWgradArgs a) {
     pdl_trigger();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + CW_STAGES * CW_STAGE);
-    const uint32_t full0 = smem_u32(bars);
-    const uint32_t empty0 = full0 + 8 * CW_STAGES;
+    uint8_t* smem = aligned_smem();
+    Ring ring(smem, CW_STAGE, CW_STAGES, reinterpret_cast<uint64_t*>(smem + CW_STAGES * CW_STAGE), CW_STAGES);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&map_dy_hi); tma_prefetch_desc(&map_dy_lo);
         tma_prefetch_desc(&map_x_hi); tma_prefetch_desc(&map_x_lo);
     }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < CW_STAGES; ++s) {
-            mbar_init(full0 + 8 * s, 1);
-            mbar_init(empty0 + 8 * s, 2);
-        }
-        fence_barrier_init();
-    }
+    if (warp == 1 && lane == 0) ring.init(2);              // one arrival per consumer warpgroup
     __syncthreads();
     pdl_wait();
 
@@ -78,7 +73,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_co
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (warp == 0 && lane == 0) {
             // ------------------------------------------------------------ TMA producer
-            uint32_t stage = 0, phase = 0;
             for (int t = blockIdx.x; t < a.num_items; t += gridDim.x) {
                 int n0, k0, q0, q1, split;
                 coords(t, n0, k0, q0, q1, split);
@@ -97,18 +91,16 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_co
                     const int img = q / a.tiles_img;
                     const int rem = q - img * a.tiles_img;
                     const int oy0 = (rem / a.tiles_x) * a.TH, ox0 = (rem % a.tiles_x) * a.TW;
-                    mbar_wait(empty0 + 8 * stage, phase ^ 1);
-                    const uint32_t fb = full0 + 8 * stage;
-                    mbar_arrive_expect_tx(fb, CW_STAGE);
-                    const uint32_t base = smem_u32(smem + stage * CW_STAGE);
+                    ring.produce([&](uint32_t base, uint32_t fb) {
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        tma_load_4d(base + i * CW_BOX, &map_dy_hi, fb, n0 + 32 * i, ox0 * a.step, oy0 * a.step, img);
-                        tma_load_4d(base + CW_TILE + i * CW_BOX, &map_x_hi, fb, bc[i], ox0 * a.sx + bx[i], oy0 * a.sy + by[i], img);
-                        tma_load_4d(base + 2 * CW_TILE + i * CW_BOX, &map_dy_lo, fb, n0 + 32 * i, ox0 * a.step, oy0 * a.step, img);
-                        tma_load_4d(base + 3 * CW_TILE + i * CW_BOX, &map_x_lo, fb, bc[i], ox0 * a.sx + bx[i], oy0 * a.sy + by[i], img);
-                    }
-                    if (++stage == CW_STAGES) { stage = 0; phase ^= 1; }
+                        for (int i = 0; i < 4; ++i) {
+                            const int x = ox0 * a.sx + bx[i], y = oy0 * a.sy + by[i];
+                            tma_load_4d(base + i * CW_BOX, &map_dy_hi, fb, n0 + 32 * i, ox0 * a.step, oy0 * a.step, img);
+                            tma_load_4d(base + CW_TILE + i * CW_BOX, &map_x_hi, fb, bc[i], x, y, img);
+                            tma_load_4d(base + 2 * CW_TILE + i * CW_BOX, &map_dy_lo, fb, n0 + 32 * i, ox0 * a.step, oy0 * a.step, img);
+                            tma_load_4d(base + 3 * CW_TILE + i * CW_BOX, &map_x_lo, fb, bc[i], x, y, img);
+                        }
+                    });
                 }
             }
         }
@@ -118,38 +110,32 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dy_hi, const __grid_co
         const int wg = (warp - 4) >> 2;
         const bool releaser = (threadIdx.x & 127) == 0;
         float acc[64];
-        uint32_t stage = 0, phase = 0;
+        auto mma = [&](uint64_t a_desc, uint64_t x_desc, uint32_t accumulate) { wgmma_n128_tt(acc, a_desc, x_desc, accumulate); };
         for (int t = blockIdx.x; t < a.num_items; t += gridDim.x) {
             int n0, k0, q0, q1, split;
             coords(t, n0, k0, q0, q1, split);
             int prev = -1;
             for (int q = q0; q < q1; ++q) {
-                mbar_wait(full0 + 8 * stage, phase);
-                const uint32_t base = smem_u32(smem + stage * CW_STAGE);
+                const uint32_t base = ring.wait();
                 const uint32_t a_hi = base + wg * 2 * CW_BOX, x_hi = base + CW_TILE;
                 const uint32_t a_lo = a_hi + 2 * CW_TILE, x_lo = x_hi + 2 * CW_TILE;
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < CW_PIX / MMA_K; ++k) {
-                    const uint64_t ah = wgmma_desc_sw64_mn(a_hi + k * 1024, CW_BOX);
-                    const uint64_t al = wgmma_desc_sw64_mn(a_lo + k * 1024, CW_BOX);
-                    const uint64_t xh = wgmma_desc_sw64_mn(x_hi + k * 1024, CW_BOX);
-                    const uint64_t xl = wgmma_desc_sw64_mn(x_lo + k * 1024, CW_BOX);
-                    wgmma_n128_tt(acc, ah, xh, (q != q0) | k);
-                    wgmma_n128_tt(acc, al, xh, 1);
-                    wgmma_n128_tt(acc, ah, xl, 1);
+                    mma_bf16x3(mma, wgmma_desc_sw64_mn(a_hi + k * 1024, CW_BOX), wgmma_desc_sw64_mn(a_lo + k * 1024, CW_BOX),
+                               wgmma_desc_sw64_mn(x_hi + k * 1024, CW_BOX), wgmma_desc_sw64_mn(x_lo + k * 1024, CW_BOX), (q != q0) | k);
                 }
                 wgmma_commit();
                 if (prev >= 0) {
                     wgmma_wait<1>();
-                    if (releaser) mbar_arrive(empty0 + 8 * prev);
+                    if (releaser) ring.release(prev);
                 }
-                prev = static_cast<int>(stage);
-                if (++stage == CW_STAGES) { stage = 0; phase ^= 1; }
+                prev = static_cast<int>(ring.stage);
+                ring.advance();
             }
             wgmma_wait<0>();
             wgmma_acc_ready(acc);
-            if (releaser) mbar_arrive(empty0 + 8 * prev);
+            if (releaser) ring.release(prev);
             // the warpgroup's 64 x 128 partial sum straight from registers to its slice of the output
             float* out = a.out + static_cast<size_t>(split) * a.Cout * a.K;
             const int r = (warp & 3) * 16 + (lane >> 2);
@@ -235,8 +221,7 @@ extern "C" int pips_conv_wgrad(const void* dy_hi, const void* dy_lo, int ldy, in
         cuuint64_t gstr[3] = {static_cast<cuuint64_t>(ldy) * 2, static_cast<cuuint64_t>(Wd) * ldy * 2, static_cast<cuuint64_t>(Hd) * Wd * ldy * 2};
         cuuint32_t box[4] = {32, static_cast<cuuint32_t>((a.TW - 1) * dy_step + 1), static_cast<cuuint32_t>((a.TH - 1) * dy_step + 1), 1};
         cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(dy_step), static_cast<cuuint32_t>(dy_step), 1};
-        if (!encode_tiled(&mdy_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(dy_hi), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_64B) ||
-            !encode_tiled(&mdy_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(dy_lo), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_64B))
+        if (!encode_tiled_pair(&mdy_hi, &mdy_lo, dy_hi, dy_lo, 4, gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_64B))
             return fail("pips_conv_wgrad: gradient tensor map failed");
     }
     {
@@ -244,18 +229,14 @@ extern "C" int pips_conv_wgrad(const void* dy_hi, const void* dy_lo, int ldy, in
         cuuint64_t gstr[3] = {static_cast<cuuint64_t>(Cp) * 2, static_cast<cuuint64_t>(W) * Cp * 2, static_cast<cuuint64_t>(H) * W * Cp * 2};
         cuuint32_t box[4] = {32, static_cast<cuuint32_t>((a.TW - 1) * stride_x + 1), static_cast<cuuint32_t>((a.TH - 1) * stride_y + 1), 1};
         cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(stride_x), static_cast<cuuint32_t>(stride_y), 1};
-        if (!encode_tiled(&mx_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x_hi), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_64B) ||
-            !encode_tiled(&mx_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x_lo), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_64B))
+        if (!encode_tiled_pair(&mx_hi, &mx_lo, x_hi, x_lo, 4, gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_64B))
             return fail("pips_conv_wgrad: activation tensor map failed");
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    static bool attr[kMaxDevices] = {};
-    cudaError_t e = ensure_dyn_smem(conv_wgrad_kernel, attr, CW_SMEM);
-    if (e != cudaSuccess) return fail_cuda("pips_conv_wgrad: smem attribute", e);
     const int grid = a.num_items < sm_count() ? a.num_items : sm_count();
-    e = launch_pdl(conv_wgrad_kernel, dim3(grid), dim3(CW_THREADS), CW_SMEM, st, mdy_hi, mdy_lo, mx_hi, mx_lo, a);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda("pips_conv_wgrad: launch", e);
+    if (const int err = launch_kernel<conv_wgrad_kernel>("pips_conv_wgrad", true, grid, CW_THREADS, CW_SMEM, st, mdy_hi, mdy_lo, mx_hi,
+                                                         mx_lo, a))
+        return err;
     if (a.splits == 1) return 0;
     const size_t nk = static_cast<size_t>(Cout) * K;
     return colsum_launch(scratch, nullptr, nullptr, nk, a.splits, static_cast<int>(nk), nullptr, dw, st);

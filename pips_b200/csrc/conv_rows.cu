@@ -269,8 +269,7 @@ extern "C" int pips_conv_rows(const void* x_hi, const void* x_lo, int N, int H, 
         cuuint64_t gstr[3] = {64 * 2, static_cast<cuuint64_t>(W) * 64 * 2, static_cast<cuuint64_t>(H) * W * 64 * 2};
         cuuint32_t box[4] = {64, R_BOX_PX, 1, 1};
         cuuint32_t estr[4] = {1, 1, 1, 1};
-        if (!encode_tiled(&ma_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x_hi), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B) ||
-            !encode_tiled(&ma_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x_lo), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
+        if (!encode_tiled_pair(&ma_hi, &ma_lo, x_hi, x_lo, 4, gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
             return fail("pips_conv_rows: activation tensor map failed");
     }
     {
@@ -278,19 +277,11 @@ extern "C" int pips_conv_rows(const void* x_hi, const void* x_lo, int N, int H, 
         cuuint64_t gstr[1] = {9 * 64 * 2};
         cuuint32_t box[2] = {64, 64};
         cuuint32_t estr[2] = {1, 1};
-        if (!encode_tiled(&mw_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_hi), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B) ||
-            !encode_tiled(&mw_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_lo), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
+        if (!encode_tiled_pair(&mw_hi, &mw_lo, w_hi, w_lo, 2, gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
             return fail("pips_conv_rows: weight tensor map failed");
-    }
-    static bool attr[kMaxDevices] = {};
-    {
-        cudaError_t e = ensure_dyn_smem(conv_rows_kernel, attr, R_SMEM_BYTES);
-        if (e != cudaSuccess) return fail_cuda("pips_conv_rows: smem attribute", e);
     }
     const int work = 2 * N * a.px_blocks * a.row_chunks;
     const int grid = work < sm_count() ? work : sm_count();
-    cudaError_t e = launch_pdl(conv_rows_kernel, dim3(grid), dim3(R_THREADS), R_SMEM_BYTES, static_cast<cudaStream_t>(stream), ma_hi, ma_lo,
-                               mw_hi, mw_lo, a);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail_cuda("pips_conv_rows: launch", e);
+    return launch_kernel<conv_rows_kernel>("pips_conv_rows", true, grid, R_THREADS, R_SMEM_BYTES, static_cast<cudaStream_t>(stream), ma_hi,
+                                           ma_lo, mw_hi, mw_lo, a);
 }

@@ -49,14 +49,10 @@ __global__ void __launch_bounds__(C_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo, const ConvArgs a) {
     pdl_trigger();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+    uint8_t* smem = aligned_smem();
     float* comb = reinterpret_cast<float*>(smem + C_RING_BYTES);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_RING_BYTES + C_COMB_BYTES);
     float* counts = reinterpret_cast<float*>(bars + 2 * C_MAX_STAGES);      // valid pixels per consumer warp and item
-    const uint32_t full0 = smem_u32(bars);
-    const uint32_t empty0 = full0 + 8 * C_MAX_STAGES;
-    const int C_STAGES = a.stages;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int rank = blockIdx.x & 1;
@@ -69,18 +65,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
     constexpr uint32_t W_BYTES = BN * BK * 2;
     constexpr uint32_t C_STAGE_BYTES = 2 * (C_A_BYTES + W_BYTES);             // hi + lo; multiple of 1 KB
     constexpr uint32_t off_w_hi = 2 * C_A_BYTES, off_w_lo = 2 * C_A_BYTES + W_BYTES;
+    Ring ring(smem, C_STAGE_BYTES, a.stages, bars, C_MAX_STAGES);
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&map_a_hi); tma_prefetch_desc(&map_a_lo);
         tma_prefetch_desc(&map_w_hi); tma_prefetch_desc(&map_w_lo);
     }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < C_STAGES; ++s) {
-            mbar_init(full0 + 8 * s, 1);
-            mbar_init(empty0 + 8 * s, 2);
-        }
-        fence_barrier_init();
-    }
+    if (warp == 1 && lane == 0) ring.init(2);
     __syncthreads();
     pdl_wait();                                         // the activation operand comes from the previous kernel
 
@@ -88,7 +79,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (warp == 0 && lane == 0) {
             // ------------------------------------------------------------ TMA producer
-            uint32_t stage = 0, phase = 0;
             for (int item = pair; item < num_items; item += num_pairs) {
                 const int img = item / a.groups_img, p0 = (item - img * a.groups_img) * a.G, p1 = min(a.pt_img, p0 + a.G);
                 for (int ptl = p0; ptl < p1; ++ptl) {
@@ -100,15 +90,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
                         for (int s = 0; s < a.S; ++s) {
                             const int ix = ox0 * a.sx + s - a.px, iy = oy0 * a.sy + r - a.py;
                             for (int c = 0; c < chunks; ++c, ++kb) {
-                                mbar_wait(empty0 + 8 * stage, phase ^ 1);
-                                const uint32_t fb = full0 + 8 * stage;
-                                mbar_arrive_expect_tx(fb, C_STAGE_BYTES);
-                                const uint32_t base = smem_u32(smem + stage * C_STAGE_BYTES);
-                                tma_load_4d(base, &map_a_hi, fb, c * BK, ix, iy, img);
-                                tma_load_4d(base + C_A_BYTES, &map_a_lo, fb, c * BK, ix, iy, img);
-                                tma_load_2d(base + off_w_hi, &map_w_hi, fb, kb * BK, 0);
-                                tma_load_2d(base + off_w_lo, &map_w_lo, fb, kb * BK, 0);
-                                if (++stage == C_STAGES) { stage = 0; phase ^= 1; }
+                                ring.produce([&](uint32_t base, uint32_t fb) {
+                                    tma_load_4d(base, &map_a_hi, fb, c * BK, ix, iy, img);
+                                    tma_load_4d(base + C_A_BYTES, &map_a_lo, fb, c * BK, ix, iy, img);
+                                    tma_load_2d(base + off_w_hi, &map_w_hi, fb, kb * BK, 0);
+                                    tma_load_2d(base + off_w_lo, &map_w_lo, fb, kb * BK, 0);
+                                });
                             }
                         }
                     }
@@ -122,7 +109,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
         const bool releaser = (threadIdx.x & 127) == 0;
         constexpr int NJ = BN / 8;                            // 8-column blocks of the accumulator
         float acc[BN / 2];
-        uint32_t stage = 0, phase = 0;
         for (int item = pair; item < num_items; item += num_pairs) {
             const int img = item / a.groups_img, grp = item - img * a.groups_img;
             const int p0 = grp * a.G, p1 = min(a.pt_img, p0 + a.G);
@@ -136,8 +122,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
             for (int ptl = p0; ptl < p1; ++ptl) {
                 int prev = -1;
                 for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait(full0 + 8 * stage, phase);
-                    const uint32_t base = smem_u32(smem + stage * C_STAGE_BYTES);
+                    const uint32_t base = ring.wait();
                     const uint64_t a_hi = wgmma_desc_sw128(base + wg * (C_A_BYTES / 2));
                     const uint64_t a_lo = wgmma_desc_sw128(base + C_A_BYTES + wg * (C_A_BYTES / 2));
                     const uint64_t w_hi = wgmma_desc_sw128(base + off_w_hi);
@@ -146,21 +131,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
 #pragma unroll
                     for (int k = 0; k < BK / MMA_K; ++k) {
                         const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);
-                        wgmma_tile<BN>(acc, a_hi + adv, w_hi + adv, (kb | k) != 0);
-                        wgmma_tile<BN>(acc, a_lo + adv, w_hi + adv, 1);
-                        wgmma_tile<BN>(acc, a_hi + adv, w_lo + adv, 1);
+                        auto mma = [&](uint64_t a_desc, uint64_t w_desc, uint32_t accumulate) {
+                            wgmma_tile<BN>(acc, a_desc + adv, w_desc + adv, accumulate);
+                        };
+                        mma_bf16x3(mma, a_hi, a_lo, w_hi, w_lo, (kb | k) != 0);
                     }
                     wgmma_commit();
                     if (prev >= 0) {
                         wgmma_wait<1>();
-                        if (releaser) mbar_arrive(empty0 + 8 * prev);
+                        if (releaser) ring.release(prev);
                     }
-                    prev = static_cast<int>(stage);
-                    if (++stage == C_STAGES) { stage = 0; phase ^= 1; }
+                    prev = static_cast<int>(ring.stage);
+                    ring.advance();
                 }
                 wgmma_wait<0>();
                 wgmma_acc_ready(acc);
-                if (releaser) mbar_arrive(empty0 + 8 * prev);
+                if (releaser) ring.release(prev);
 
                 const int rem = 2 * ptl + rank;
                 const int i0 = wg * 64 + w4 * 16 + (lane >> 2);             // pixel index inside the tile (and i0 + 8)
@@ -262,18 +248,11 @@ static void conv_geometry(int Ho, int Wo, int sx, ConvArgs& a) {
 template <int BN>
 static int conv_tc_launch(const CUtensorMap& ma_hi, const CUtensorMap& ma_lo, const CUtensorMap& mw_hi, const CUtensorMap& mw_lo,
                           const ConvArgs& a, void* stream) {
-    static bool attr[kMaxDevices] = {};
-    {
-        cudaError_t e = ensure_dyn_smem(conv_tc_kernel<BN>, attr, C_SMEM_BYTES);
-        if (e != cudaSuccess) return fail_cuda("pips_conv_tc: smem attribute", e);
-    }
     const int items = a.N * a.groups_img;
     const int max_pairs = sm_count() / 2;
     const int pairs = items < max_pairs ? items : max_pairs;
-    cudaError_t e = launch_pdl(conv_tc_kernel<BN>, dim3(2 * pairs), dim3(C_THREADS), C_SMEM_BYTES, static_cast<cudaStream_t>(stream), ma_hi,
-                               ma_lo, mw_hi, mw_lo, a);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail_cuda("pips_conv_tc: launch", e);
+    return launch_kernel<conv_tc_kernel<BN>>("pips_conv_tc", true, 2 * pairs, C_THREADS, C_SMEM_BYTES, static_cast<cudaStream_t>(stream),
+                                             ma_hi, ma_lo, mw_hi, mw_lo, a);
 }
 
 static int conv_tc_impl(const void* x_hi, const void* x_lo, int N, int H, int W, int Cp, const void* w_hi, const void* w_lo,
@@ -304,8 +283,7 @@ static int conv_tc_impl(const void* x_hi, const void* x_lo, int N, int H, int W,
         cuuint32_t box[4] = {static_cast<cuuint32_t>(BK), static_cast<cuuint32_t>((a.TW - 1) * sx + 1),
                              static_cast<cuuint32_t>((a.TH - 1) * sy + 1), 1};
         cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(sx), static_cast<cuuint32_t>(sy), 1};
-        if (!encode_tiled(&ma_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x_hi), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B) ||
-            !encode_tiled(&ma_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x_lo), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
+        if (!encode_tiled_pair(&ma_hi, &ma_lo, x_hi, x_lo, 4, gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
             return fail("pips_conv_tc: activation tensor map failed");
     }
     {
@@ -314,8 +292,7 @@ static int conv_tc_impl(const void* x_hi, const void* x_lo, int N, int H, int W,
         cuuint64_t gstr[1] = {static_cast<cuuint64_t>(K) * 2};
         cuuint32_t box[2] = {static_cast<cuuint32_t>(BK), static_cast<cuuint32_t>(a.BN)};
         cuuint32_t estr[2] = {1, 1};
-        if (!encode_tiled(&mw_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_hi), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B) ||
-            !encode_tiled(&mw_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_lo), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
+        if (!encode_tiled_pair(&mw_hi, &mw_lo, w_hi, w_lo, 2, gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_128B))
             return fail("pips_conv_tc: weight tensor map failed");
     }
     return a.BN == 64 ? conv_tc_launch<64>(ma_hi, ma_lo, mw_hi, mw_lo, a, stream)

@@ -201,13 +201,10 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
     constexpr uint32_t BOX_BYTES = 32 * KB * 2;                    // WGRAD: one {32, 32} box, 2 KB
     static_assert(CLUSTER == 1 || BN == 256, "cluster tiles are 256 columns wide");
     static_assert(!WGRAD || (BN == 128 && CLUSTER == 1 && TERMS == 3), "the weight-gradient variant is bf16x3, 128 x 128");
-    extern __shared__ uint8_t smem_raw[];
     // the 128-byte-swizzled staging buffers need 1024-byte alignment (the 64-byte-swizzled ring needs 512)
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+    uint8_t* smem = aligned_smem();
     uint8_t* staging = smem + kStages * Cfg::kStageBytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(staging + EPI_STAGING_BYTES);
-    const uint32_t full0 = smem_u32(bars);                  // full[kStages], empty[kStages]
-    const uint32_t empty0 = full0 + 8 * kStages;
+    Ring ring(smem, Cfg::kStageBytes, kStages, reinterpret_cast<uint64_t*>(staging + EPI_STAGING_BYTES), kStages);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -250,13 +247,7 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
             tma_prefetch_desc(&maps.out_f32);
         }
     }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < kStages; ++s) {
-            mbar_init(full0 + 8 * s, 1);
-            mbar_init(empty0 + 8 * s, 2 * CLUSTER);         // one arrival per consumer warpgroup that reads the slot's W
-        }
-        fence_barrier_init();
-    }
+    if (warp == 1 && lane == 0) ring.init(2 * CLUSTER);    // one arrival per consumer warpgroup that reads the slot's W
     if (CLUSTER == 2) cluster_sync_all();                   // the peer's barriers exist before anything is sent to them
     else __syncthreads();
     pdl_wait();                                             // operands and the residual stream come from the previous kernel
@@ -266,41 +257,36 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (warp == 0 && lane == 0) {
             // ------------------------------------------------------------ TMA producer
-            uint32_t stage = 0, phase = 0;
             for (int t = worker; t < args.num_tiles; t += num_workers) {
                 int m0, n0, kb0, kb1;
                 tile_coords(t, m0, n0, kb0, kb1);
                 for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(empty0 + 8 * stage, phase ^ 1);
-                    const uint32_t fb = full0 + 8 * stage;
-                    mbar_arrive_expect_tx(fb, Cfg::kStageBytes);
-                    const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
-                    const int k0 = kb * KB;
-                    if constexpr (WGRAD) {                    // m0: first n of the tile, n0: first k, k0: first m
+                    ring.produce([&](uint32_t base, uint32_t fb) {
+                        const int k0 = kb * KB;
+                        if constexpr (WGRAD) {             // m0: first n of the tile, n0: first k, k0: first m
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            tma_load_2d(base + i * BOX_BYTES, &maps.a_hi, fb, m0 + 32 * i, k0);
-                            tma_load_2d(base + A_TILE_BYTES + i * BOX_BYTES, &maps.w_hi, fb, n0 + 32 * i, k0);
-                            tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES + i * BOX_BYTES, &maps.a_lo, fb, m0 + 32 * i, k0);
-                            tma_load_2d(base + 2 * A_TILE_BYTES + W_TILE_BYTES + i * BOX_BYTES, &maps.w_lo, fb, n0 + 32 * i, k0);
+                            for (int i = 0; i < 4; ++i) {
+                                tma_load_2d(base + i * BOX_BYTES, &maps.a_hi, fb, m0 + 32 * i, k0);
+                                tma_load_2d(base + A_TILE_BYTES + i * BOX_BYTES, &maps.w_hi, fb, n0 + 32 * i, k0);
+                                tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES + i * BOX_BYTES, &maps.a_lo, fb, m0 + 32 * i, k0);
+                                tma_load_2d(base + 2 * A_TILE_BYTES + W_TILE_BYTES + i * BOX_BYTES, &maps.w_lo, fb, n0 + 32 * i, k0);
+                            }
+                        } else {
+                            tma_load_2d(base, &maps.a_hi, fb, k0, m0);
+                            if (TERMS == 3) tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES, &maps.a_lo, fb, k0, m0);
+                            if (CLUSTER == 2) {
+                                // this CTA's half of the W tile (box = 128 rows), into both CTAs
+                                const uint32_t half = rank * (W_TILE_BYTES / 2);
+                                tma_load_2d_multicast(base + A_TILE_BYTES + half, &maps.w_hi, fb, k0, n0 + static_cast<int>(rank) * (BN / 2), 3);
+                                if (TERMS == 3)
+                                    tma_load_2d_multicast(base + 2 * A_TILE_BYTES + W_TILE_BYTES + half, &maps.w_lo, fb, k0,
+                                                          n0 + static_cast<int>(rank) * (BN / 2), 3);
+                            } else {
+                                tma_load_2d(base + A_TILE_BYTES, &maps.w_hi, fb, k0, n0);
+                                if (TERMS == 3) tma_load_2d(base + 2 * A_TILE_BYTES + W_TILE_BYTES, &maps.w_lo, fb, k0, n0);
+                            }
                         }
-                        if (++stage == kStages) { stage = 0; phase ^= 1; }
-                        continue;
-                    }
-                    tma_load_2d(base, &maps.a_hi, fb, k0, m0);
-                    if (TERMS == 3) tma_load_2d(base + A_TILE_BYTES + W_TILE_BYTES, &maps.a_lo, fb, k0, m0);
-                    if (CLUSTER == 2) {
-                        // this CTA's half of the W tile (box = 128 rows), into both CTAs
-                        const uint32_t half = rank * (W_TILE_BYTES / 2);
-                        tma_load_2d_multicast(base + A_TILE_BYTES + half, &maps.w_hi, fb, k0, n0 + static_cast<int>(rank) * (BN / 2), 3);
-                        if (TERMS == 3)
-                            tma_load_2d_multicast(base + 2 * A_TILE_BYTES + W_TILE_BYTES + half, &maps.w_lo, fb, k0,
-                                                  n0 + static_cast<int>(rank) * (BN / 2), 3);
-                    } else {
-                        tma_load_2d(base + A_TILE_BYTES, &maps.w_hi, fb, k0, n0);
-                        if (TERMS == 3) tma_load_2d(base + 2 * A_TILE_BYTES + W_TILE_BYTES, &maps.w_lo, fb, k0, n0);
-                    }
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
+                    });
                 }
             }
         }
@@ -312,28 +298,31 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
         const uint32_t my_staging = smem_u32(staging) + wg * 2 * EPI_BUF_BYTES;
         uint32_t chunk = 0;
         float acc[BN / 2];
-        uint32_t stage = 0, phase = 0;
+        auto release = [&](int slot) {
+            if (releaser) {
+                ring.release(slot);
+                if (CLUSTER == 2) mbar_arrive_cluster(ring.empty(slot), rank ^ 1);
+            }
+        };
         for (int t = worker; t < args.num_tiles; t += num_workers) {
             int m0, n0, kb0, kb1;
             tile_coords(t, m0, n0, kb0, kb1);
             int prev = -1;                                   // ring slot whose MMAs are still in flight
             for (int kb = kb0; kb < kb1; ++kb) {
-                mbar_wait(full0 + 8 * stage, phase);
-                const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
+                const uint32_t base = ring.wait();
                 if constexpr (WGRAD) {
                     wgmma_fence();
                     // the warpgroup's 64 n are the boxes 2wg, 2wg + 1; a K=16 step is 16 rows of m = 1 KB into every box
                     const uint32_t a_hi = base + wg * 2 * BOX_BYTES, w_hi = base + A_TILE_BYTES;
                     const uint32_t a_lo = a_hi + A_TILE_BYTES + W_TILE_BYTES, w_lo = w_hi + A_TILE_BYTES + W_TILE_BYTES;
+                    auto mma = [&](uint64_t a, uint64_t w, uint32_t accumulate) {
+                        wgmma_n128_tt(*reinterpret_cast<float(*)[64]>(&acc[0]), a, w, accumulate);
+                    };
 #pragma unroll
                     for (int k = 0; k < KB / MMA_K; ++k) {
-                        const uint64_t ah = wgmma_desc_sw64_mn(a_hi + k * 1024, BOX_BYTES);
-                        const uint64_t al = wgmma_desc_sw64_mn(a_lo + k * 1024, BOX_BYTES);
-                        const uint64_t wh = wgmma_desc_sw64_mn(w_hi + k * 1024, BOX_BYTES);
-                        const uint64_t wl = wgmma_desc_sw64_mn(w_lo + k * 1024, BOX_BYTES);
-                        wgmma_n128_tt(*reinterpret_cast<float(*)[64]>(&acc[0]), ah, wh, (kb != kb0) | k);
-                        wgmma_n128_tt(*reinterpret_cast<float(*)[64]>(&acc[0]), al, wh, 1);
-                        wgmma_n128_tt(*reinterpret_cast<float(*)[64]>(&acc[0]), ah, wl, 1);
+                        mma_bf16x3(mma, wgmma_desc_sw64_mn(a_hi + k * 1024, BOX_BYTES),
+                                   wgmma_desc_sw64_mn(a_lo + k * 1024, BOX_BYTES), wgmma_desc_sw64_mn(w_hi + k * 1024, BOX_BYTES),
+                                   wgmma_desc_sw64_mn(w_lo + k * 1024, BOX_BYTES), (kb != kb0) | k);
                     }
                 } else {
                     const uint64_t a_hi = wgmma_desc_sw64(base + wg * (A_TILE_BYTES / 2));
@@ -344,30 +333,24 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
 #pragma unroll
                     for (int k = 0; k < KB / MMA_K; ++k) {
                         const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);   // 32 B per K=16 step
-                        gemm_mma<BN>(acc, a_hi + adv, w_hi + adv, (kb | k) != 0);
-                        if (TERMS == 3) {
-                            gemm_mma<BN>(acc, a_lo + adv, w_hi + adv, 1);
-                            gemm_mma<BN>(acc, a_hi + adv, w_lo + adv, 1);
-                        }
+                        auto mma = [&](uint64_t a, uint64_t w, uint32_t accumulate) {
+                            gemm_mma<BN>(acc, a + adv, w + adv, accumulate);
+                        };
+                        if (TERMS == 3) mma_bf16x3(mma, a_hi, a_lo, w_hi, w_lo, (kb | k) != 0);
+                        else mma(a_hi, w_hi, (kb | k) != 0);
                     }
                 }
                 wgmma_commit();
                 if (prev >= 0) {
                     wgmma_wait<1>();                         // the previous slot's MMAs have retired: slot reusable
-                    if (releaser) {
-                        mbar_arrive(empty0 + 8 * prev);
-                        if (CLUSTER == 2) mbar_arrive_cluster(empty0 + 8 * prev, rank ^ 1);
-                    }
+                    release(prev);
                 }
-                prev = static_cast<int>(stage);
-                if (++stage == kStages) { stage = 0; phase ^= 1; }
+                prev = static_cast<int>(ring.stage);
+                ring.advance();
             }
             wgmma_wait<0>();
             wgmma_acc_ready(acc);
-            if (releaser) {
-                mbar_arrive(empty0 + 8 * prev);
-                if (CLUSTER == 2) mbar_arrive_cluster(empty0 + 8 * prev, rank ^ 1);
-            }
+            release(prev);
             if constexpr (WGRAD) {
                 const int split = t % splits;
                 float* out = args.out_f32 + static_cast<size_t>(split) * args.N * args.ldo;
@@ -409,14 +392,18 @@ constexpr int WG_SPLIT_ROWS = 2048;
 
 // ---------------------------------------------------------------------------------- host side
 
-static bool make_operand_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld_elems, int box_rows) {
+// the (hi, lo) operand maps; map_lo = nullptr: the hi map only
+static bool make_operand_maps(CUtensorMap* map_hi, CUtensorMap* map_lo, const void* hi, const void* lo, int rows, int K,
+                              int ld_elems, int box_rows) {
     // global tensor (innermost first): {K, rows}, row stride ld_elems*2 bytes; box {32, box_rows}, 64B swizzle
     cuuint64_t gdim[2] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(rows)};
     cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ld_elems) * 2};
     cuuint32_t box[2] = {static_cast<cuuint32_t>(KB), static_cast<cuuint32_t>(box_rows)};
     cuuint32_t estr[2] = {1, 1};
-    return encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_SWIZZLE_64B);
+    if (!map_lo)
+        return encode_tiled(map_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(hi), gdim, gstride, box, estr,
+                            CU_TENSOR_MAP_SWIZZLE_64B);
+    return encode_tiled_pair(map_hi, map_lo, hi, lo, 2, gdim, gstride, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
 // Output tensor {N, M} with row stride `ld` elements; box {EPI_COLS, 64} (one warpgroup's chunk), swizzled like the
@@ -430,17 +417,17 @@ static bool make_output_map(CUtensorMap* map, void* ptr, const GemmArgs& args, i
                         estr, f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
-// every map of the problem; W boxes are `w_box_rows` rows (the tile width, or its half in the pair kernel)
+// every map of the problem (bf16: the lo maps are copies of the hi ones); W boxes are `w_box_rows` rows (the tile width, or
+// its half in the pair kernel)
 static const char* make_maps(GemmMaps* m, bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi,
                              const void* w_lo, int ldw, int w_rows, int w_box_rows, const GemmArgs& args) {
     *m = GemmMaps{};
-    if (!make_operand_map(&m->a_hi, a_hi, a_rows, args.K, lda, BM)) return "tensor map (A hi) failed";
-    if (!make_operand_map(&m->w_hi, w_hi, w_rows, args.K, ldw, w_box_rows)) return "tensor map (W hi) failed";
-    m->a_lo = m->a_hi;
-    m->w_lo = m->w_hi;
-    if (x3) {
-        if (!make_operand_map(&m->a_lo, a_lo, a_rows, args.K, lda, BM)) return "tensor map (A lo) failed";
-        if (!make_operand_map(&m->w_lo, w_lo, w_rows, args.K, ldw, w_box_rows)) return "tensor map (W lo) failed";
+    if (!make_operand_maps(&m->a_hi, x3 ? &m->a_lo : nullptr, a_hi, a_lo, a_rows, args.K, lda, BM)) return "tensor map (A) failed";
+    if (!make_operand_maps(&m->w_hi, x3 ? &m->w_lo : nullptr, w_hi, w_lo, w_rows, args.K, ldw, w_box_rows))
+        return "tensor map (W) failed";
+    if (!x3) {
+        m->a_lo = m->a_hi;
+        m->w_lo = m->w_hi;
     }
     if (bf16_epilogue(args.epilogue)) {
         if (!make_output_map(&m->out_hi, args.out_hi, args, args.ldh, false)) return "tensor map (out hi) failed";
@@ -570,8 +557,8 @@ extern "C" int pips_wgrad(const void* g_hi, const void* g_lo, int ldg, const voi
     if (static_cast<long long>(N) * K > 0x7fffffffLL || splits > 256) return fail("pips_wgrad: problem too large");
     if (splits > 1 && !scratch) return fail("pips_wgrad: scratch of pips_wgrad_scratch_floats(M, N, K) floats is required");
     GemmMaps maps = {};
-    if (!make_operand_map(&maps.a_hi, g_hi, M, N, ldg, 32) || !make_operand_map(&maps.a_lo, g_lo, M, N, ldg, 32)
-        || !make_operand_map(&maps.w_hi, x_hi, M, K, ldx, 32) || !make_operand_map(&maps.w_lo, x_lo, M, K, ldx, 32))
+    if (!make_operand_maps(&maps.a_hi, &maps.a_lo, g_hi, g_lo, M, N, ldg, 32) ||
+        !make_operand_maps(&maps.w_hi, &maps.w_lo, x_hi, x_lo, M, K, ldx, 32))
         return fail("pips_wgrad: tensor map failed");
     GemmArgs a = {};
     a.M = M; a.N = N; a.K = K; a.epilogue = PIPS_EPI_BIAS;
@@ -579,14 +566,9 @@ extern "C" int pips_wgrad(const void* g_hi, const void* g_lo, int ldg, const voi
     a.kb_per_split = WG_SPLIT_ROWS / KB;
     a.num_tiles = ((N + BM - 1) / BM) * ((K + 127) / 128) * splits;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    using Cfg = GemmCfg<3, 128>;
-    static bool attr[kMaxDevices] = {};
-    cudaError_t e = ensure_dyn_smem(wgrad_kernel, attr, Cfg::kSmemBytes);
-    if (e != cudaSuccess) return fail_cuda("pips_wgrad: smem attribute", e);
     const int grid = a.num_tiles < sm_count() ? a.num_tiles : sm_count();
-    e = launch_pdl(wgrad_kernel, dim3(grid), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, maps, a);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e != cudaSuccess) return fail_cuda("pips_wgrad: launch", e);
+    if (const int err = launch_kernel<wgrad_kernel>("pips_wgrad", true, grid, GEMM_THREADS, GemmCfg<3, 128>::kSmemBytes, st, maps, a))
+        return err;
     if (splits == 1) return 0;
     // the splits' partial sums, in split order
     const size_t nk = static_cast<size_t>(N) * K;
@@ -597,35 +579,21 @@ namespace pips {
 
 template <int TERMS, int BN>
 static int launch_variant(const GemmMaps& maps, const GemmArgs& args, cudaStream_t st) {
-    using Cfg = GemmCfg<TERMS, BN>;
-    static bool attr[kMaxDevices] = {};
-    {
-        cudaError_t e = ensure_dyn_smem(gemm_tc_kernel<TERMS, BN>, attr, Cfg::kSmemBytes);
-        if (e != cudaSuccess) return fail_cuda("pips_gemm_tc: smem attribute", e);
-    }
     GemmArgs a = args;
     a.num_tiles = ((args.M + BM - 1) / BM) * ((args.N + BN - 1) / BN);
     const int grid = a.num_tiles < sm_count() ? a.num_tiles : sm_count();
-    cudaError_t e = launch_pdl(gemm_tc_kernel<TERMS, BN>, dim3(grid), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, maps, a);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail_cuda("pips_gemm_tc: launch", e);
+    return launch_kernel<gemm_tc_kernel<TERMS, BN>>("pips_gemm_tc", true, grid, GEMM_THREADS, GemmCfg<TERMS, BN>::kSmemBytes, st,
+                                                    maps, a);
 }
 
 template <int TERMS>
 static int launch_pair_variant(const GemmMaps& maps, const GemmArgs& args, cudaStream_t st) {
-    using Cfg = GemmCfg<TERMS, 256>;
-    static bool attr[kMaxDevices] = {};
-    {
-        cudaError_t e = ensure_dyn_smem(gemm_tc_pair_kernel<TERMS>, attr, Cfg::kSmemBytes);
-        if (e != cudaSuccess) return fail_cuda("pips_gemm_tc (pair): smem attribute", e);
-    }
     GemmArgs a = args;
     a.num_tiles = ((args.M + 255) / 256) * ((args.N + 255) / 256);
     const int max_pairs = sm_count() / 2;
     const int pairs = a.num_tiles < max_pairs ? a.num_tiles : max_pairs;
-    cudaError_t e = launch_pdl(gemm_tc_pair_kernel<TERMS>, dim3(2 * pairs), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, maps, a);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail_cuda("pips_gemm_tc (pair): launch", e);
+    return launch_kernel<gemm_tc_pair_kernel<TERMS>>("pips_gemm_tc (pair)", true, 2 * pairs, GEMM_THREADS,
+                                                     GemmCfg<TERMS, 256>::kSmemBytes, st, maps, a);
 }
 
 int launch_pair(bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo, int ldw,
@@ -644,18 +612,10 @@ int launch_aux(const void* a_hi, const void* a_lo, int lda, int a_rows, const vo
     if (const char* err = make_maps(&maps, true, a_hi, a_lo, lda, a_rows, w_hi, w_lo, ldw, w_rows, 128, args)) {
         return fail((std::string("pips_gemm_tc: ") + err).c_str());
     }
-    using Cfg = GemmCfg<3, 128>;
-    static bool attr[kMaxDevices] = {};
-    {
-        cudaError_t e = ensure_dyn_smem(gemm_tc_aux_kernel, attr, Cfg::kSmemBytes);
-        if (e != cudaSuccess) return fail_cuda("pips_gemm_tc (aux): smem attribute", e);
-    }
     GemmArgs a = args;
     a.num_tiles = ((args.M + BM - 1) / BM) * ((args.N + 127) / 128);
     const int grid = a.num_tiles < sm_count() ? a.num_tiles : sm_count();
-    cudaError_t e = launch_pdl(gemm_tc_aux_kernel, dim3(grid), dim3(GEMM_THREADS), Cfg::kSmemBytes, st, maps, a);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail_cuda("pips_gemm_tc (aux): launch", e);
+    return launch_kernel<gemm_tc_aux_kernel>("pips_gemm_tc (aux)", true, grid, GEMM_THREADS, GemmCfg<3, 128>::kSmemBytes, st, maps, a);
 }
 
 int launch_single(int bn, bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo,

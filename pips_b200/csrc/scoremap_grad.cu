@@ -22,25 +22,13 @@
 //   grad_basis: X = G (128 pixels of one frame),                    Y = F_i (64 particles), O = dG
 // Each CTA owns its 128 output rows and sums over its tiles in a fixed order: no atomics, and the result depends on the
 // shape only.  The two coefficients g/(eps+K), g/(eps+K(P-1)) are read from device memory (no host round trip).
-#include "gemm_common.cuh"
+#include "scoremap_common.cuh"
 
 namespace pips {
 namespace {
+using namespace smap;
 
-constexpr int C = PIPS_C;
 constexpr int L = PIPS_LEVELS;
-constexpr int GR_BM = 128;                             // resident rows per CTA: two consumer warpgroups of 64
-constexpr int GR_BN = 64;                              // streamed rows per ring stage
-constexpr int GR_KB = 32;                              // K-block: 32 bf16 = one 64-byte swizzle row
-constexpr int GR_NKB = C / GR_KB;                      // 4
-constexpr int GR_STAGES = 4;
-constexpr int GR_THREADS = 384;                        // producer warpgroup + 2 consumer warpgroups
-constexpr uint32_t X_KB_BYTES = GR_BM * GR_KB * 2;     // 8 KB
-constexpr uint32_t X_BYTES = 2 * GR_NKB * X_KB_BYTES;  // 64 KB: hi and lo, all of K
-constexpr uint32_t Y_KB_BYTES = GR_BN * GR_KB * 2;     // 4 KB
-constexpr uint32_t Y_STAGE_BYTES = 2 * GR_NKB * Y_KB_BYTES;   // 32 KB
-constexpr uint32_t GR_SMEM_BYTES = 1024 /*align*/ + X_BYTES + GR_STAGES * Y_STAGE_BYTES + 256 /*barriers*/;
-static_assert(GR_SMEM_BYTES <= 227u * 1024u, "resident tile + ring must fit in 227 KB");
 
 struct GradArgs {
     const float* feats;                                // grad_feats: F (iters, frames, N, C) fp32
@@ -52,11 +40,6 @@ struct GradArgs {
     int frames, N, P, iters;
 };
 
-__device__ __forceinline__ uint32_t sw64(int row, int byte) {
-    const uint32_t o = static_cast<uint32_t>(row * 64 + byte);
-    return o ^ (((o >> 7) & 3u) << 4);
-}
-
 // dloss/ds for a kept row: at the target g (sigma(s) - 1)/(eps+K) = -cpos / (1 + e^s) (no cancellation near sigma = 1),
 // elsewhere cneg sigma(s) = cneg / (1 + e^-s)
 __device__ __forceinline__ float score_grad(float s, bool at_target, float cpos, float cneg) {
@@ -66,58 +49,40 @@ __device__ __forceinline__ float score_grad(float s, bool at_target, float cpos,
 // BASIS = false: pips_scoremap_grad_feats, grid (particle tiles, frames, iters).
 // BASIS = true:  pips_scoremap_grad_basis, grid (pixel tiles, frames).
 template <bool BASIS>
-__global__ void __launch_bounds__(GR_THREADS, 1)
+__global__ void __launch_bounds__(THREADS, 1)
 scoremap_grad_kernel(const __grid_constant__ CUtensorMap y_hi, const __grid_constant__ CUtensorMap y_lo, const GradArgs a) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint8_t* ring = smem + X_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(ring + GR_STAGES * Y_STAGE_BYTES);
-    const uint32_t full0 = smem_u32(bars);
-    const uint32_t empty0 = full0 + 8 * GR_STAGES;
+    uint8_t* smem = aligned_smem();
+    Ring ring = y_ring(smem);
 
-    const int x_base = blockIdx.x * GR_BM;             // first resident row: particle (feats) or pixel (basis)
+    const int x_base = blockIdx.x * BM;             // first resident row: particle (feats) or pixel (basis)
     const int frame = blockIdx.y;
     const int it = BASIS ? 0 : blockIdx.z;
     const int x_rows = BASIS ? a.P : a.N;
-    const int y_per_pass = ((BASIS ? a.N : a.P) + GR_BN - 1) / GR_BN;   // streamed tiles per frame (and iteration)
+    const int y_per_pass = ((BASIS ? a.N : a.P) + BN - 1) / BN;   // streamed tiles per frame (and iteration)
     const int tiles = BASIS ? a.iters * y_per_pass : y_per_pass;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&y_hi);
         tma_prefetch_desc(&y_lo);
-        for (int st = 0; st < GR_STAGES; ++st) {
-            mbar_init(full0 + 8 * st, 1);
-            mbar_init(empty0 + 8 * st, 2);             // one arrival per consumer warpgroup
-        }
-        fence_barrier_init();
+        ring.init(2);                                      // one arrival per consumer warpgroup
     }
     __syncthreads();
 
     if (warp < 4) {
         if (warp == 0 && lane == 0) {
             // ------------------------------------------------------------ TMA producer
-            uint32_t stage = 0, phase = 0;
             for (int t = 0; t < tiles; ++t) {
-                mbar_wait(empty0 + 8 * stage, phase ^ 1);
-                const uint32_t fb = full0 + 8 * stage;
-                mbar_arrive_expect_tx(fb, Y_STAGE_BYTES);
-                const uint32_t base = smem_u32(ring + stage * Y_STAGE_BYTES);
                 // rows past this frame's pixels (particles) belong to the next frame (iteration), or are zero-filled
                 // past the tensor: their coefficients are 0
                 int row;
                 if constexpr (BASIS) {
                     const int i = t / y_per_pass;
-                    row = (i * a.frames + frame) * a.N + (t - i * y_per_pass) * GR_BN;
+                    row = (i * a.frames + frame) * a.N + (t - i * y_per_pass) * BN;
                 } else {
-                    row = frame * a.P + t * GR_BN;
+                    row = frame * a.P + t * BN;
                 }
-#pragma unroll
-                for (int kb = 0; kb < GR_NKB; ++kb) {
-                    tma_load_2d(base + kb * Y_KB_BYTES, &y_hi, fb, kb * GR_KB, row);
-                    tma_load_2d(base + (GR_NKB + kb) * Y_KB_BYTES, &y_lo, fb, kb * GR_KB, row);
-                }
-                if (++stage == GR_STAGES) { stage = 0; phase ^= 1; }
+                load_y(ring, &y_hi, &y_lo, row);
             }
         }
         return;
@@ -128,7 +93,7 @@ scoremap_grad_kernel(const __grid_constant__ CUtensorMap y_hi, const __grid_cons
     const int wg = ct >> 7;
     // the resident tile, K-major, 64-byte swizzled; rows past the frame's particles (pixels) are zero
     if constexpr (BASIS) {
-        for (int i = ct; i < GR_BM * (C / 8); i += 256) {  // 16-byte chunks of 8 channels
+        for (int i = ct; i < BM * (C / 8); i += 256) {     // 16-byte chunks of 8 channels
             const int r = i >> 4, c8 = i & 15;
             const int p = x_base + r;
             uint4 h = make_uint4(0, 0, 0, 0), l = h;
@@ -137,26 +102,14 @@ scoremap_grad_kernel(const __grid_constant__ CUtensorMap y_hi, const __grid_cons
                 h = __ldg(reinterpret_cast<const uint4*>(a.g_hi + off) + c8);
                 l = __ldg(reinterpret_cast<const uint4*>(a.g_lo + off) + c8);
             }
-            const int k = 8 * c8, kb = k / GR_KB;
-            const uint32_t o = sw64(r, (k % GR_KB) * 2);
+            const int k = 8 * c8, kb = k / KB;
+            const uint32_t o = sw64(r, (k % KB) * 2);
             *reinterpret_cast<uint4*>(smem + kb * X_KB_BYTES + o) = h;
-            *reinterpret_cast<uint4*>(smem + (GR_NKB + kb) * X_KB_BYTES + o) = l;
+            *reinterpret_cast<uint4*>(smem + (NKB + kb) * X_KB_BYTES + o) = l;
         }
     } else {
         const float* f = a.feats + (static_cast<size_t>(it) * a.frames + frame) * a.N * C;
-        for (int i = ct; i < GR_BM * (C / 4); i += 256) {
-            const int r = i >> 5, c4 = i & 31;
-            const int n = x_base + r;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (n < a.N) v = __ldg(reinterpret_cast<const float4*>(f + static_cast<size_t>(n) * C) + c4);
-            const uint32_t h01 = cvt_bf16x2(v.x, v.y), h23 = cvt_bf16x2(v.z, v.w);
-            const uint32_t l01 = cvt_bf16x2(v.x - __uint_as_float(h01 << 16), v.y - __uint_as_float(h01 & 0xffff0000u));
-            const uint32_t l23 = cvt_bf16x2(v.z - __uint_as_float(h23 << 16), v.w - __uint_as_float(h23 & 0xffff0000u));
-            const int k = 4 * c4, kb = k / GR_KB;
-            const uint32_t o = sw64(r, (k % GR_KB) * 2);
-            *reinterpret_cast<uint2*>(smem + kb * X_KB_BYTES + o) = make_uint2(h01, h23);
-            *reinterpret_cast<uint2*>(smem + (GR_NKB + kb) * X_KB_BYTES + o) = make_uint2(l01, l23);
-        }
+        fill_x_f32(smem, ct, x_base, a.N, [&](int n) { return f + static_cast<size_t>(n) * C; });
     }
     fence_proxy_async_smem();                              // the generic-proxy writes become visible to wgmma
     named_bar_sync(1, 256);
@@ -174,47 +127,31 @@ scoremap_grad_kernel(const __grid_constant__ CUtensorMap y_hi, const __grid_cons
     }
     const bool releaser = (ct & 127) == 0;
     const uint32_t x_hi0 = smem_u32(smem) + wg * (X_KB_BYTES / 2);
-    const uint32_t x_lo0 = smem_u32(smem + GR_NKB * X_KB_BYTES) + wg * (X_KB_BYTES / 2);
-    float sacc[GR_BN / 2];
+    const uint32_t x_lo0 = smem_u32(smem + NKB * X_KB_BYTES) + wg * (X_KB_BYTES / 2);
+    float sacc[BN / 2];
     float oacc[C / 2];
 #pragma unroll
     for (int j = 0; j < C / 2; ++j) oacc[j] = 0.0f;
-    uint32_t stage = 0, phase = 0;
+    auto omma = [&](const uint32_t* c, uint64_t y, uint32_t accumulate) {
+        wgmma_n128_rA_tb(oacc, c[0], c[1], c[2], c[3], y, accumulate);
+    };
     for (int t = 0; t < tiles; ++t) {
-        mbar_wait(full0 + 8 * stage, phase);
-        const uint32_t base = smem_u32(ring + stage * Y_STAGE_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int kb = 0; kb < GR_NKB; ++kb) {
-            const uint64_t xh = wgmma_desc_sw64(x_hi0 + kb * X_KB_BYTES);
-            const uint64_t xl = wgmma_desc_sw64(x_lo0 + kb * X_KB_BYTES);
-            const uint64_t yh = wgmma_desc_sw64(base + kb * Y_KB_BYTES);
-            const uint64_t yl = wgmma_desc_sw64(base + (GR_NKB + kb) * Y_KB_BYTES);
-#pragma unroll
-            for (int k = 0; k < GR_KB / MMA_K; ++k) {
-                const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);   // 32 B per K=16 step
-                wgmma_n64(sacc, xh + adv, yh + adv, (kb | k) != 0);
-                wgmma_n64(sacc, xl + adv, yh + adv, 1);
-                wgmma_n64(sacc, xh + adv, yl + adv, 1);
-            }
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_acc_ready(sacc);
+        const uint32_t base = ring.wait();
+        score_mma(sacc, x_hi0, x_lo0, base);
 
         // c from the fragment: column 8j + cq + e of rows r0 (h = 0) and r0 + 8 (h = 1) is sacc[4j + 2h + e]
         int y0, y_lim;                                     // streamed row of column 0; columns >= y_lim are not ours
         if constexpr (BASIS) {
             const int i = t / y_per_pass;
-            y0 = (t - i * y_per_pass) * GR_BN;
+            y0 = (t - i * y_per_pass) * BN;
             y_lim = a.N - y0;
         } else {
-            y0 = t * GR_BN;
+            y0 = t * BN;
             y_lim = a.P - y0;
         }
-        uint32_t c_hi[GR_BN / 4], c_lo[GR_BN / 4];
+        uint32_t c_hi[BN / 4], c_lo[BN / 4];
 #pragma unroll
-        for (int j = 0; j < GR_BN / 8; ++j) {
+        for (int j = 0; j < BN / 8; ++j) {
             int yt[2];                                     // basis: the column's target pixel
             if constexpr (BASIS) {
 #pragma unroll
@@ -247,18 +184,16 @@ scoremap_grad_kernel(const __grid_constant__ CUtensorMap y_hi, const __grid_cons
         // its A fragment is c[4k .. 4k+3] in the order (r0, lo cols), (r0+8, lo cols), (r0, hi cols), (r0+8, hi cols)
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < GR_BN / MMA_K; ++k) {
+        for (int k = 0; k < BN / MMA_K; ++k) {
             const uint64_t yh = wgmma_desc_sw64_mn(base + k * 1024, Y_KB_BYTES);
-            const uint64_t yl = wgmma_desc_sw64_mn(base + GR_NKB * Y_KB_BYTES + k * 1024, Y_KB_BYTES);
-            wgmma_n128_rA_tb(oacc, c_hi[4 * k], c_hi[4 * k + 1], c_hi[4 * k + 2], c_hi[4 * k + 3], yh, 1);
-            wgmma_n128_rA_tb(oacc, c_lo[4 * k], c_lo[4 * k + 1], c_lo[4 * k + 2], c_lo[4 * k + 3], yh, 1);
-            wgmma_n128_rA_tb(oacc, c_hi[4 * k], c_hi[4 * k + 1], c_hi[4 * k + 2], c_hi[4 * k + 3], yl, 1);
+            const uint64_t yl = wgmma_desc_sw64_mn(base + NKB * Y_KB_BYTES + k * 1024, Y_KB_BYTES);
+            mma_bf16x3(omma, &c_hi[4 * k], &c_lo[4 * k], yh, yl, 1);
         }
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_acc_ready(oacc);
-        if (releaser) mbar_arrive(empty0 + 8 * stage);     // both GEMMs have read the stage
-        if (++stage == GR_STAGES) { stage = 0; phase ^= 1; }
+        if (releaser) ring.release(ring.stage);            // both GEMMs have read the stage
+        ring.advance();
     }
 
     // O rows r0, r0 + 8: channel 8j + cq + e is oacc[4j + 2h + e]
@@ -347,23 +282,15 @@ __global__ void __launch_bounds__(256) scoremap_basis_grad_kernel(const float* _
 template <bool BASIS>
 int launch_grad(const char* name, const void* y_hi, const void* y_lo, long long y_rows, dim3 grid, const GradArgs& a,
                 void* stream) {
-    CUtensorMap maps[2];
-    const void* src[2] = {y_hi, y_lo};
-    for (int i = 0; i < 2; ++i) {
-        cuuint64_t gdim[2] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(y_rows)};
-        cuuint64_t gstride[1] = {static_cast<cuuint64_t>(C) * 2};
-        cuuint32_t box[2] = {static_cast<cuuint32_t>(GR_KB), static_cast<cuuint32_t>(GR_BN)};
-        cuuint32_t estr[2] = {1, 1};
-        if (!encode_tiled(&maps[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(src[i]), gdim, gstride, box, estr,
-                          CU_TENSOR_MAP_SWIZZLE_64B))
-            return fail(BASIS ? "pips_scoremap_grad_basis: tensor map (F) failed" : "pips_scoremap_grad_feats: tensor map (G) failed");
-    }
-    static bool attr[kMaxDevices] = {};
-    cudaError_t e = ensure_dyn_smem(scoremap_grad_kernel<BASIS>, attr, GR_SMEM_BYTES);
-    if (e != cudaSuccess) return fail_cuda(name, e);
-    scoremap_grad_kernel<BASIS><<<grid, GR_THREADS, GR_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(maps[0], maps[1], a);
-    e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail_cuda(name, e);
+    CUtensorMap map_hi, map_lo;
+    cuuint64_t gdim[2] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(y_rows)};
+    cuuint64_t gstride[1] = {static_cast<cuuint64_t>(C) * 2};
+    cuuint32_t box[2] = {static_cast<cuuint32_t>(KB), static_cast<cuuint32_t>(BN)};
+    cuuint32_t estr[2] = {1, 1};
+    if (!encode_tiled_pair(&map_hi, &map_lo, y_hi, y_lo, 2, gdim, gstride, box, estr, CU_TENSOR_MAP_SWIZZLE_64B))
+        return fail(BASIS ? "pips_scoremap_grad_basis: tensor map (F) failed" : "pips_scoremap_grad_feats: tensor map (G) failed");
+    return launch_kernel<scoremap_grad_kernel<BASIS>>(name, false, grid, THREADS, SMEM_BYTES, static_cast<cudaStream_t>(stream),
+                                                      map_hi, map_lo, a);
 }
 
 }  // namespace
@@ -381,12 +308,12 @@ extern "C" int pips_scoremap_grad_feats(const void* G_hi, const void* G_lo, cons
          | reinterpret_cast<uintptr_t>(dffeats)) & 15)
         return fail("pips_scoremap_grad_feats: G_hi, G_lo, ffeats and dffeats must be 16-byte aligned");
     const long long rows = static_cast<long long>(B) * S * H8 * W8;
-    if (rows > 0x7fffffffLL || (N + GR_BM - 1) / GR_BM > 65535 || B * S > 65535 || iters > 65535)
+    if (rows > 0x7fffffffLL || (N + BM - 1) / BM > 65535 || B * S > 65535 || iters > 65535)
         return fail("pips_scoremap_grad_feats: problem too large");
     GradArgs a = {};
     a.feats = ffeats; a.target = target; a.coef = coef; a.out = dffeats;
     a.frames = B * S; a.N = N; a.P = H8 * W8; a.iters = iters;
-    return launch_grad<false>("pips_scoremap_grad_feats", G_hi, G_lo, rows, dim3((N + GR_BM - 1) / GR_BM, B * S, iters), a,
+    return launch_grad<false>("pips_scoremap_grad_feats", G_hi, G_lo, rows, dim3((N + BM - 1) / BM, B * S, iters), a,
                               stream);
 }
 
@@ -407,7 +334,7 @@ extern "C" int pips_scoremap_grad_basis(const void* G_hi, const void* G_lo, cons
     a.g_hi = static_cast<const __nv_bfloat16*>(G_hi); a.g_lo = static_cast<const __nv_bfloat16*>(G_lo);
     a.target = target; a.coef = coef; a.out = dG;
     a.frames = B * S; a.N = N; a.P = P; a.iters = iters;
-    return launch_grad<true>("pips_scoremap_grad_basis", F_hi, F_lo, rows, dim3((P + GR_BM - 1) / GR_BM, B * S), a, stream);
+    return launch_grad<true>("pips_scoremap_grad_basis", F_hi, F_lo, rows, dim3((P + BM - 1) / BM, B * S), a, stream);
 }
 
 extern "C" int pips_scoremap_basis_grad(const float* dG, int frames, int H8, int W8, float* const* dlvl_f32, void* stream) {

@@ -26,27 +26,15 @@
 // Determinism: a row's partial sum depends on its own data, its split and a fixed order (tiles, then fragment columns,
 // then the quad of lanes that share the row); the grid depends on the shape only -- not on particle chunking, on graph
 // or eager launch, or on the SM count.
-#include "gemm_common.cuh"
+#include "scoremap_common.cuh"
 
 namespace pips {
 namespace {
+using namespace smap;                                  // X: the particle tile, Y: pixel tiles of G
 
-constexpr int C = PIPS_C;                              // 128 = K of the score GEMM
 constexpr int L = PIPS_LEVELS;
-constexpr int SL_BM = 128;                             // particles per CTA: two consumer warpgroups of 64
-constexpr int SL_BN = 64;                              // pixels per ring stage
-constexpr int SL_KB = 32;                              // K-block: 32 bf16 = one 64-byte swizzle row
-constexpr int SL_NKB = C / SL_KB;                      // 4
 constexpr int SPLIT_PIX = 512;                         // pixels per split (8 ring stages)
-constexpr int SL_STAGES = 4;
-constexpr int SL_THREADS = 384;                        // producer warpgroup + 2 consumer warpgroups
-constexpr uint32_t A_KB_BYTES = SL_BM * SL_KB * 2;     // 8 KB: one K-block of the particle tile (hi or lo)
-constexpr uint32_t A_BYTES = 2 * SL_NKB * A_KB_BYTES;  // 64 KB: hi and lo, all of K
-constexpr uint32_t G_KB_BYTES = SL_BN * SL_KB * 2;     // 4 KB
-constexpr uint32_t STAGE_BYTES = 2 * SL_NKB * G_KB_BYTES;   // 32 KB
-constexpr uint32_t SL_SMEM_BYTES = 1024 /*align*/ + A_BYTES + SL_STAGES * STAGE_BYTES + 256 /*barriers*/;
-static_assert(SL_SMEM_BYTES <= 227u * 1024u, "particle tile + ring must fit in 227 KB");
-static_assert(SPLIT_PIX % SL_BN == 0, "a split is whole pixel tiles");
+static_assert(SPLIT_PIX % BN == 0, "a split is whole pixel tiles");
 
 struct LossArgs {
     const float* ffeats;                               // ((b*N + n), s, c)
@@ -62,61 +50,33 @@ __device__ __forceinline__ float softplus(float v) {
     return fmaxf(v, 0.0f) + log1pf(__expf(-fabsf(v)));
 }
 
-// byte `byte` of row `row` in a K-block of 64-byte rows, swizzled the way TMA writes CU_TENSOR_MAP_SWIZZLE_64B
-// (the 16-byte unit is XORed with (row / 2) % 4): the layout wgmma_desc_sw64 describes
-__device__ __forceinline__ uint32_t sw64(int row, int byte) {
-    const uint32_t o = static_cast<uint32_t>(row * 64 + byte);
-    return o ^ (((o >> 7) & 3u) << 4);
-}
-
-__global__ void __launch_bounds__(SL_THREADS, 1)
+__global__ void __launch_bounds__(THREADS, 1)
 scoremap_loss_kernel(const __grid_constant__ CUtensorMap g_hi, const __grid_constant__ CUtensorMap g_lo, const LossArgs a) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint8_t* ring = smem + A_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(ring + SL_STAGES * STAGE_BYTES);
-    const uint32_t full0 = smem_u32(bars);                 // full[SL_STAGES], empty[SL_STAGES]
-    const uint32_t empty0 = full0 + 8 * SL_STAGES;
+    uint8_t* smem = aligned_smem();
+    Ring ring = y_ring(smem);
 
     const int split = blockIdx.x;
-    const int n_base = blockIdx.y * SL_BM;
+    const int n_base = blockIdx.y * BM;
     const int frame = blockIdx.z;                          // b * S + s
     const int b = frame / a.S, s = frame - b * a.S;
     const int p_begin = split * SPLIT_PIX;
     const int p_end = min(a.P, p_begin + SPLIT_PIX);
-    const int tiles = (p_end - p_begin + SL_BN - 1) / SL_BN;
+    const int tiles = (p_end - p_begin + BN - 1) / BN;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&g_hi);
         tma_prefetch_desc(&g_lo);
-        for (int st = 0; st < SL_STAGES; ++st) {
-            mbar_init(full0 + 8 * st, 1);
-            mbar_init(empty0 + 8 * st, 2);             // one arrival per consumer warpgroup
-        }
-        fence_barrier_init();
+        ring.init(2);                                      // one arrival per consumer warpgroup
     }
     __syncthreads();
 
     if (warp < 4) {
         if (warp == 0 && lane == 0) {
             // ------------------------------------------------------------ TMA producer (G does not depend on ffeats)
-            uint32_t stage = 0, phase = 0;
-            for (int t = 0; t < tiles; ++t) {
-                mbar_wait(empty0 + 8 * stage, phase ^ 1);
-                const uint32_t fb = full0 + 8 * stage;
-                mbar_arrive_expect_tx(fb, STAGE_BYTES);
-                const uint32_t base = smem_u32(ring + stage * STAGE_BYTES);
-                // rows past this frame's pixels belong to the next frame (or are zero-filled past the tensor): the
-                // epilogue ignores their columns
-                const int row = frame * a.P + p_begin + t * SL_BN;
-#pragma unroll
-                for (int kb = 0; kb < SL_NKB; ++kb) {
-                    tma_load_2d(base + kb * G_KB_BYTES, &g_hi, fb, kb * SL_KB, row);
-                    tma_load_2d(base + (SL_NKB + kb) * G_KB_BYTES, &g_lo, fb, kb * SL_KB, row);
-                }
-                if (++stage == SL_STAGES) { stage = 0; phase ^= 1; }
-            }
+            // rows past this frame's pixels belong to the next frame (or are zero-filled past the tensor): the epilogue
+            // ignores their columns
+            for (int t = 0; t < tiles; ++t) load_y(ring, &g_hi, &g_lo, frame * a.P + p_begin + t * BN);
         }
         return;
     }
@@ -124,23 +84,8 @@ scoremap_loss_kernel(const __grid_constant__ CUtensorMap g_hi, const __grid_cons
     // ---------------------------------------------------------------- consumers
     const int ct = threadIdx.x - 128;                      // 0..255
     const int wg = ct >> 7;
-    // the particle tile: fp32 ffeats rows (frame s of track (b, n)) -> (hi, lo) bf16, K-major, 64-byte swizzled;
-    // rows past N are zero
-    for (int i = ct; i < SL_BM * (C / 4); i += 256) {
-        const int r = i >> 5, c4 = i & 31;
-        const int n = n_base + r;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (n < a.N) v = __ldg(reinterpret_cast<const float4*>(a.ffeats + (static_cast<size_t>(b * a.N + n) * a.S + s) * C) + c4);
-        const uint32_t h01 = cvt_bf16x2(v.x, v.y), h23 = cvt_bf16x2(v.z, v.w);
-        const uint32_t l01 = cvt_bf16x2(v.x - __uint_as_float(h01 << 16), v.y - __uint_as_float(h01 & 0xffff0000u));
-        const uint32_t l23 = cvt_bf16x2(v.z - __uint_as_float(h23 << 16), v.w - __uint_as_float(h23 & 0xffff0000u));
-        const int k = 4 * c4, kb = k / SL_KB;
-        const uint32_t off = sw64(r, (k % SL_KB) * 2);
-        const uint32_t hi = smem_u32(smem + kb * A_KB_BYTES) + off;
-        const uint32_t lo = smem_u32(smem + (SL_NKB + kb) * A_KB_BYTES) + off;
-        asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(hi), "r"(h01), "r"(h23) : "memory");
-        asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(lo), "r"(l01), "r"(l23) : "memory");
-    }
+    // the particle tile: fp32 ffeats rows (frame s of track (b, n)); rows past N are zero
+    fill_x_f32(smem, ct, n_base, a.N, [&](int n) { return a.ffeats + (static_cast<size_t>(b * a.N + n) * a.S + s) * C; });
     fence_proxy_async_smem();                              // the generic-proxy writes become visible to wgmma
     named_bar_sync(1, 256);
 
@@ -157,42 +102,22 @@ scoremap_loss_kernel(const __grid_constant__ CUtensorMap g_hi, const __grid_cons
     }
     float neg[2] = {0.0f, 0.0f};
     const bool releaser = (ct & 127) == 0;
-    const uint32_t a_hi0 = smem_u32(smem) + wg * (A_KB_BYTES / 2);
-    const uint32_t a_lo0 = smem_u32(smem + SL_NKB * A_KB_BYTES) + wg * (A_KB_BYTES / 2);
-    float acc[SL_BN / 2];
-    uint32_t stage = 0, phase = 0;
+    const uint32_t x_hi0 = smem_u32(smem) + wg * (X_KB_BYTES / 2);
+    const uint32_t x_lo0 = smem_u32(smem + NKB * X_KB_BYTES) + wg * (X_KB_BYTES / 2);
+    float acc[BN / 2];
     for (int t = 0; t < tiles; ++t) {
-        mbar_wait(full0 + 8 * stage, phase);
-        const uint32_t base = smem_u32(ring + stage * STAGE_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int kb = 0; kb < SL_NKB; ++kb) {
-            const uint64_t ah = wgmma_desc_sw64(a_hi0 + kb * A_KB_BYTES);
-            const uint64_t al = wgmma_desc_sw64(a_lo0 + kb * A_KB_BYTES);
-            const uint64_t gh = wgmma_desc_sw64(base + kb * G_KB_BYTES);
-            const uint64_t gl = wgmma_desc_sw64(base + (SL_NKB + kb) * G_KB_BYTES);
-#pragma unroll
-            for (int k = 0; k < SL_KB / MMA_K; ++k) {
-                const uint64_t adv = static_cast<uint64_t>((k * MMA_K * 2) >> 4);   // 32 B per K=16 step
-                wgmma_n64(acc, ah + adv, gh + adv, (kb | k) != 0);
-                wgmma_n64(acc, al + adv, gh + adv, 1);
-                wgmma_n64(acc, ah + adv, gl + adv, 1);
-            }
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_acc_ready(acc);
-        if (releaser) mbar_arrive(empty0 + 8 * stage);     // the slot is free while this warpgroup runs its epilogue
-        if (++stage == SL_STAGES) { stage = 0; phase ^= 1; }
+        score_mma(acc, x_hi0, x_lo0, ring.wait());
+        if (releaser) ring.release(ring.stage);            // the slot is free while this warpgroup runs its epilogue
+        ring.advance();
 
-        const int p0 = p_begin + t * SL_BN;
+        const int p0 = p_begin + t * BN;
         const int lim = p_end - p0;                        // columns >= lim are outside this split (or frame)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             if (tgt[h] < 0) continue;
             const int tl = tgt[h] - p0;                    // the target's column in this tile (any value if elsewhere)
 #pragma unroll
-            for (int j = 0; j < SL_BN / 8; ++j) {
+            for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int col = 8 * j + cq + e;
@@ -306,30 +231,21 @@ extern "C" int pips_scoremap_loss(const void* G_hi, const void* G_lo, const floa
     if ((reinterpret_cast<uintptr_t>(G_hi) | reinterpret_cast<uintptr_t>(G_lo) | reinterpret_cast<uintptr_t>(ffeats)) & 15)
         return fail("pips_scoremap_loss: G_hi, G_lo and ffeats must be 16-byte aligned");
     const long long rows = static_cast<long long>(B) * S * H8 * W8;
-    if (rows > 0x7fffffffLL || (N + SL_BM - 1) / SL_BM > 65535 || B * S > 65535)
+    if (rows > 0x7fffffffLL || (N + BM - 1) / BM > 65535 || B * S > 65535)
         return fail("pips_scoremap_loss: problem too large");
-    CUtensorMap maps[2];
-    const void* src[2] = {G_hi, G_lo};
-    for (int i = 0; i < 2; ++i) {
+    CUtensorMap map_hi, map_lo;
+    {
         cuuint64_t gdim[2] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(rows)};
         cuuint64_t gstride[1] = {static_cast<cuuint64_t>(C) * 2};
-        cuuint32_t box[2] = {static_cast<cuuint32_t>(SL_KB), static_cast<cuuint32_t>(SL_BN)};
+        cuuint32_t box[2] = {static_cast<cuuint32_t>(KB), static_cast<cuuint32_t>(BN)};
         cuuint32_t estr[2] = {1, 1};
-        if (!encode_tiled(&maps[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(src[i]), gdim, gstride, box, estr,
-                          CU_TENSOR_MAP_SWIZZLE_64B))
+        if (!encode_tiled_pair(&map_hi, &map_lo, G_hi, G_lo, 2, gdim, gstride, box, estr, CU_TENSOR_MAP_SWIZZLE_64B))
             return fail("pips_scoremap_loss: tensor map (G) failed");
-    }
-    static bool attr[kMaxDevices] = {};
-    {
-        cudaError_t e = ensure_dyn_smem(scoremap_loss_kernel, attr, SL_SMEM_BYTES);
-        if (e != cudaSuccess) return fail_cuda("pips_scoremap_loss: smem attribute", e);
     }
     LossArgs a;
     a.ffeats = ffeats; a.target = target; a.neg_part = neg_part; a.pos_part = pos_part;
     a.S = S; a.N = N; a.P = H8 * W8; a.n_split = pips_scoremap_splits(H8, W8);
     // a plain launch: the next iteration's PDL-launched kernels cannot start before this one has read ffeats
-    dim3 grid(a.n_split, (N + SL_BM - 1) / SL_BM, B * S);
-    scoremap_loss_kernel<<<grid, SL_THREADS, SL_SMEM_BYTES, static_cast<cudaStream_t>(stream)>>>(maps[0], maps[1], a);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail_cuda("pips_scoremap_loss", e);
+    return launch_kernel<scoremap_loss_kernel>("pips_scoremap_loss", false, dim3(a.n_split, (N + BM - 1) / BM, B * S), THREADS,
+                                               SMEM_BYTES, static_cast<cudaStream_t>(stream), map_hi, map_lo, a);
 }
