@@ -74,6 +74,20 @@ int pips_corr_gather(const void* const* lvl, int feat_dtype, int B, int S, int N
                      const int* frame_base /* NULL or [B*N] */, int frames_per_batch,
                      void* x_hi, void* x_lo, float* x_f32, int ldx, void* stream);
 
+/* Backward of pips_corr_gather's correlation columns (x[:, 128:324]) for training (csrc/corr_grad.cu), with respect to
+ * the ffeats and the 4 fp32 levels; the coordinates get no gradient.  S == 8, fp32, no frame_base.  dcorr is the
+ * gradient of those 196 columns, (B*N*S, ld_dcorr) in mixer row order, ld_dcorr >= 196.  Per unit and level the
+ * adjoint of the 49-tap blend is an 8x8 weight matrix A over the unit's footprint (the pixels pips_corr_gather read):
+ *   A[j][i] = (1/sqrt(128)) sum_{dy,dx in {0,1}} w_{dy,dx} dcorr[l*49 + (i-dx)*7 + (j-dy)]   (0 <= i-dx, j-dy < 7)
+ * Every output element is written once, summed in a fixed order (deterministic, no atomics).
+ * pips_corr_grad_feats: dffeat_rows (B*N, S, 128) = sum over levels and footprint pixels of A * level pixel.
+ * pips_corr_grad_levels: dlvl[l] (B*S, H>>l, W>>l, 128) = sum over the frame's units, in ascending n, of A * ffeat
+ *   (ffeat_rows (B*N, S, 128)); pixels no footprint covers are 0. */
+int pips_corr_grad_feats(const float* const* lvl, int B, int S, int N, int H, int W, const float* coords,
+                         const float* dcorr, int ld_dcorr, float* dffeat_rows, void* stream);
+int pips_corr_grad_levels(int B, int S, int N, int H, int W, const float* coords, const float* ffeat_rows,
+                          const float* dcorr, int ld_dcorr, float* const* dlvl, void* stream);
+
 /* nn.Linear on tensor cores: out = epi(A[M,K] . W[N,K]^T + bias).  a_lo/w_lo NULL => plain bf16. */
 int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_rows,
                  const void* w_hi, const void* w_lo, int ldw, int w_rows,

@@ -70,6 +70,8 @@ _SIGNATURES = {
     "pips_pyramid_build_nhwc": (_i, [_p, _i, _i, _i, C.POINTER(_p), C.POINTER(_p), _p]),
     "pips_init_gather": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _p, _p]),
     "pips_corr_gather": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _i, _p, _p, _p, _i, _p]),
+    "pips_corr_grad_feats": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _p, _p, _i, _p, _p]),
+    "pips_corr_grad_levels": (_i, [_i, _i, _i, _i, _i, _p, _p, _p, _i, C.POINTER(_p), _p]),
     "pips_peer_alloc": (_i, [C.c_size_t, C.POINTER(_p), C.c_char_p]),
     "pips_peer_open": (_i, [C.c_char_p, C.POINTER(_p)]),
     "pips_peer_close": (_i, [_p]),

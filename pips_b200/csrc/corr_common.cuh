@@ -1,0 +1,92 @@
+// What the local correlation's forward (corr_gather.cu) and its backward (corr_grad.cu) share: the unit decode, the
+// box origins of a unit's 8x8 footprints and the tensor maps the footprint boxes are read through.  A footprint is the
+// same pixels in both directions only if both use this arithmetic.
+#pragma once
+#include "common.cuh"
+
+namespace pips {
+
+constexpr int CG_ROWS_PER_BOX = 2;     // a footprint is read as 4 boxes {128 ch, 8 px, 2 rows}
+
+struct CgMaps {
+    CUtensorMap m[PIPS_LEVELS];
+};
+
+struct CgArgs {
+    int B, S, N;
+    int H[PIPS_LEVELS], W[PIPS_LEVELS];
+    const float* coords;     // (B,S,N,2)
+    const float* ffeats;     // (B*N,S,128)
+    const float* times;      // [S]
+    const int* frame_base;   // optional [B*N]: window start of each track inside its clip of T frames (chained tracking)
+    int T;                   // frames per batch element in the pyramid (== S when frame_base is null)
+    __nv_bfloat16* x_hi;
+    __nv_bfloat16* x_lo;
+    float* x_f32;
+    int ldx;
+};
+
+struct UnitInfo {
+    float cx, cy;      // coords of (b,s,n), level-0 pixels
+    int frame;         // pyramid frame index
+    int b, n, s;
+    int valid;
+    int ox, oy;        // lane l < 4: TMA box origin (first column, first row) of pyramid level l for this unit
+};
+
+// Unit u = (seq, s) with seq = b*N + n (the mixer's row order); S == 8.  Besides the unit's coordinates every lane
+// computes the box origin of ONE pyramid level (lane & 3), so that issuing a TMA box later costs two shuffles instead
+// of a clamp / floor / convert chain executed by lane 0 alone while 31 lanes wait.  Coordinates are clamped in float
+// so that diverged or non-finite tracks cannot overflow the int conversion (beyond +-8 px of the map all taps are zero).
+__device__ __forceinline__ UnitInfo load_unit(const CgArgs& a, int u, int total) {
+    UnitInfo ui;
+    ui.valid = u < total;
+    ui.cx = 0.f; ui.cy = 0.f; ui.frame = 0; ui.b = 0; ui.n = 0; ui.s = 0; ui.ox = 0; ui.oy = 0;
+    if (ui.valid) {
+        ui.s = u & 7;
+        const int seq = u >> 3;
+        ui.b = seq / a.N; ui.n = seq - ui.b * a.N;
+        const float2 c = *reinterpret_cast<const float2*>(a.coords + ((static_cast<size_t>(ui.b) * 8 + ui.s) * a.N + ui.n) * 2);
+        ui.cx = c.x; ui.cy = c.y;
+        // chained windows replicate the clip's last frame past its end (chain_demo.py:50-52)
+        ui.frame = a.frame_base ? ui.b * a.T + min(a.frame_base[seq] + ui.s, a.T - 1) : ui.b * 8 + ui.s;
+        const int level = threadIdx.x & 3;
+        const float sc = 1.0f / static_cast<float>(1 << level);        // coords / 2**i  (nets/pips.py:373), exact
+        const float cxl = fminf(fmaxf(c.x * sc, -8.0f), static_cast<float>(a.W[level]) + 8.0f);
+        const float cyl = fminf(fmaxf(c.y * sc, -8.0f), static_cast<float>(a.H[level]) + 8.0f);
+        ui.ox = static_cast<int>(floorf(cxl)) - PIPS_RADIUS;
+        ui.oy = static_cast<int>(floorf(cyl)) - PIPS_RADIUS;
+    }
+    return ui;
+}
+
+// The bilinear weights of level `level` for a unit at (cx, cy): the fractional part of the clamped position, as
+// load_unit clamps it.  w00 weighs footprint pixel (j, i) for tap (i, j), w01 (j, i+1), w10 (j+1, i), w11 (j+1, i+1).
+struct TapWeights {
+    float w00, w01, w10, w11;
+};
+
+__device__ __forceinline__ TapWeights tap_weights(float cx, float cy, int level, int W, int H) {
+    const float sc = 1.0f / static_cast<float>(1 << level);
+    const float cxl = fminf(fmaxf(cx * sc, -8.0f), static_cast<float>(W) + 8.0f);
+    const float cyl = fminf(fmaxf(cy * sc, -8.0f), static_cast<float>(H) + 8.0f);
+    const float fx = cxl - floorf(cxl), fy = cyl - floorf(cyl);
+    return {(1.f - fx) * (1.f - fy), fx * (1.f - fy), (1.f - fx) * fy, fx * fy};
+}
+
+// The 4 level maps the footprint boxes {128 ch, 8 px, CG_ROWS_PER_BOX rows} are loaded through: level l is
+// (frames, H[l], W[l], 128) channels-last of `es`-byte elements.  `who` prefixes the error message.
+inline int encode_level_maps(CgMaps& maps, const void* const* lvl, CUtensorMapDataType dt, cuuint64_t es, const int* H,
+                             const int* W, int frames, const char* who) {
+    for (int l = 0; l < PIPS_LEVELS; ++l) {
+        cuuint64_t gdim[4] = {128, static_cast<cuuint64_t>(W[l]), static_cast<cuuint64_t>(H[l]), static_cast<cuuint64_t>(frames)};
+        cuuint64_t gstr[3] = {128 * es, static_cast<cuuint64_t>(W[l]) * 128 * es, static_cast<cuuint64_t>(H[l]) * W[l] * 128 * es};
+        cuuint32_t box[4] = {128, 8, CG_ROWS_PER_BOX, 1};
+        cuuint32_t estr[4] = {1, 1, 1, 1};
+        if (!encode_tiled(&maps.m[l], dt, 4, const_cast<void*>(lvl[l]), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE))
+            return fail(who);
+    }
+    return 0;
+}
+
+}  // namespace pips

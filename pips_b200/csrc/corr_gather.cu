@@ -21,14 +21,13 @@
 //
 // Algorithmic bytes per unit (SURVEY.md 8d): 4 levels x 64 px x 128 ch x e_f  +  128 x 4 (query)
 // +  output row.
-#include "common.cuh"
+#include "corr_common.cuh"
 #include "ptx.cuh"
 
 namespace pips {
 
 constexpr int CG_WARPS = 8;
 constexpr int CG_STAGES = 3;
-constexpr int CG_ROWS_PER_BOX = 2;
 constexpr int CG_ROWBUF = PIPS_KITCHEN_PAD;   // 576 floats
 constexpr uint32_t CG_AUX_BYTES = CG_ROWBUF * 4 + 64 * 4 + 128;    // per warp: row buffer, 64 dot products, 3 mbarriers
 
@@ -41,24 +40,6 @@ struct CgCfg {
     static constexpr uint32_t kSmemBytes = CG_WARPS * CG_STAGES * kBoxBytes + CG_WARPS * CG_AUX_BYTES + kBoxBytes;
 };
 
-struct CgMaps {
-    CUtensorMap m[PIPS_LEVELS];
-};
-
-struct CgArgs {
-    int B, S, N;
-    int H[PIPS_LEVELS], W[PIPS_LEVELS];
-    const float* coords;     // (B,S,N,2)
-    const float* ffeats;     // (B*N,S,128)
-    const float* times;      // [S]
-    const int* frame_base;   // optional [B*N]: window start of each track inside its clip of T frames (chained tracking)
-    int T;                   // frames per batch element in the pyramid (== S when frame_base is null)
-    __nv_bfloat16* x_hi;
-    __nv_bfloat16* x_lo;
-    float* x_f32;
-    int ldx;
-};
-
 __device__ __forceinline__ float4 ld_chan4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ float4 ld_chan4(const __nv_bfloat16* p) {
     const uint2 u = *reinterpret_cast<const uint2*>(p);
@@ -68,40 +49,6 @@ __device__ __forceinline__ float4 ld_chan4(const __nv_bfloat16* p) {
     r.z = __uint_as_float(u.y << 16);
     r.w = __uint_as_float(u.y & 0xffff0000u);
     return r;
-}
-
-struct UnitInfo {
-    float cx, cy;      // coords of (b,s,n), level-0 pixels
-    int frame;         // pyramid frame index
-    int b, n, s;
-    int valid;
-    int ox, oy;        // lane l < 4: TMA box origin (first column, first row) of pyramid level l for this unit
-};
-
-// Unit u = (seq, s) with seq = b*N + n (the mixer's row order); S == 8.  Besides the unit's coordinates every lane
-// computes the box origin of ONE pyramid level (lane & 3), so that issuing a TMA box later costs two shuffles instead
-// of a clamp / floor / convert chain executed by lane 0 alone while 31 lanes wait.  Coordinates are clamped in float
-// so that diverged or non-finite tracks cannot overflow the int conversion (beyond +-8 px of the map all taps are zero).
-__device__ __forceinline__ UnitInfo load_unit(const CgArgs& a, int u, int total) {
-    UnitInfo ui;
-    ui.valid = u < total;
-    ui.cx = 0.f; ui.cy = 0.f; ui.frame = 0; ui.b = 0; ui.n = 0; ui.s = 0; ui.ox = 0; ui.oy = 0;
-    if (ui.valid) {
-        ui.s = u & 7;
-        const int seq = u >> 3;
-        ui.b = seq / a.N; ui.n = seq - ui.b * a.N;
-        const float2 c = *reinterpret_cast<const float2*>(a.coords + ((static_cast<size_t>(ui.b) * 8 + ui.s) * a.N + ui.n) * 2);
-        ui.cx = c.x; ui.cy = c.y;
-        // chained windows replicate the clip's last frame past its end (chain_demo.py:50-52)
-        ui.frame = a.frame_base ? ui.b * a.T + min(a.frame_base[seq] + ui.s, a.T - 1) : ui.b * 8 + ui.s;
-        const int level = threadIdx.x & 3;
-        const float sc = 1.0f / static_cast<float>(1 << level);        // coords / 2**i  (nets/pips.py:373), exact
-        const float cxl = fminf(fmaxf(c.x * sc, -8.0f), static_cast<float>(a.W[level]) + 8.0f);
-        const float cyl = fminf(fmaxf(c.y * sc, -8.0f), static_cast<float>(a.H[level]) + 8.0f);
-        ui.ox = static_cast<int>(floorf(cxl)) - PIPS_RADIUS;
-        ui.oy = static_cast<int>(floorf(cyl)) - PIPS_RADIUS;
-    }
-    return ui;
 }
 
 template <typename T>
@@ -257,16 +204,8 @@ corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
 template <typename T>
 static int launch_corr_gather(const void* const* lvl, CUtensorMapDataType dt, const CgArgs& args, int frames, cudaStream_t st) {
     CgMaps maps;
-    for (int l = 0; l < PIPS_LEVELS; ++l) {
-        const cuuint64_t es = sizeof(T);
-        cuuint64_t gdim[4] = {128, static_cast<cuuint64_t>(args.W[l]), static_cast<cuuint64_t>(args.H[l]), static_cast<cuuint64_t>(frames)};
-        cuuint64_t gstr[3] = {128 * es, static_cast<cuuint64_t>(args.W[l]) * 128 * es,
-                              static_cast<cuuint64_t>(args.H[l]) * args.W[l] * 128 * es};
-        cuuint32_t box[4] = {128, 8, CG_ROWS_PER_BOX, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        if (!encode_tiled(&maps.m[l], dt, 4, const_cast<void*>(lvl[l]), gdim, gstr, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE))
-            return fail("pips_corr_gather: cuTensorMapEncodeTiled failed");
-    }
+    if (encode_level_maps(maps, lvl, dt, sizeof(T), args.H, args.W, frames, "pips_corr_gather: cuTensorMapEncodeTiled failed"))
+        return 1;
     using Cfg = CgCfg<T>;
     static bool attr[kMaxDevices] = {};
     {

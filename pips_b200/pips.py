@@ -35,8 +35,15 @@ Extra, optional knobs (keyword-only; the reference signature is unchanged):
               gradients, recompute per ResBlock from the saved block boundaries) run on sm_90a in bf16x3.  CPU tensors and
               an rgbs that requires grad keep the module; plain inference is unaffected.  Independent of loss_path and
               mixer_path
+  corr_path   'torch' (default) or 'cuda': where the differentiable path computes the local correlation.  'torch' is
+              the reference's formulation under autograd: all-pairs volumes (B,S,N,h,w) of the 4 levels by matmul, 196
+              taps by grid_sample, every volume kept until the backward (whose grid_sample adjoint accumulates with
+              atomics).  'cuda' is torch_path.local_corr_cuda: pips_corr_gather's 8x8 footprints forward and
+              deterministic gather kernels backward, with no volume; volumes are then built only for the dense score
+              maps (loss_path other than 'fused').  CPU tensors, S != 8 and maps under 8x8 keep the torch formulation;
+              plain inference is unaffected.  Independent of the other paths
 Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET, PIPS_B200_LOSSES, PIPS_B200_MIXER,
-PIPS_B200_ENCODER.
+PIPS_B200_ENCODER, PIPS_B200_CORR.
 """
 from __future__ import annotations
 
@@ -113,7 +120,7 @@ def _conv_math(allow_tf32: bool):
 class Pips(nn.Module):
     def __init__(self, S=8, stride=8, *, precision: Optional[str] = None, feat_dtype: Optional[str] = None,
                  fnet_mode: Optional[str] = None, max_seqs: int = 32768, loss_path: Optional[str] = None,
-                 mixer_path: Optional[str] = None, encoder_path: Optional[str] = None):
+                 mixer_path: Optional[str] = None, encoder_path: Optional[str] = None, corr_path: Optional[str] = None):
         super().__init__()
         self.S = S
         self.stride = stride
@@ -151,6 +158,10 @@ class Pips(nn.Module):
         if self.encoder_path not in ("torch", "cuda"):
             raise ValueError("encoder_path must be 'torch' (the Encoder module under autograd) or 'cuda' (its forward and "
                              "backward on the sm_90a kernels, bf16x3)")
+        self.corr_path = corr_path or os.environ.get("PIPS_B200_CORR", "torch")
+        if self.corr_path not in ("torch", "cuda"):
+            raise ValueError("corr_path must be 'torch' (all-pairs volumes and grid_sample under autograd) or 'cuda' (the "
+                             "local correlation and its gradients on the sm_90a kernels, without the volumes)")
 
     # ------------------------------------------------------------------ configuration
     @property

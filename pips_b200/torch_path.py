@@ -5,8 +5,10 @@ tensors live (it is what ``train.py`` / ``test_on_flt.py`` exercise) and keeps t
 semantics, including the dense score map ``fcps`` that only the score-map loss consumes -- except with
 ``model.loss_path == 'fused'`` on CUDA tensors, where ``fused_score_map_loss`` computes that loss and its gradients
 without ``fcps``, and with ``model.mixer_path == 'cuda'`` on CUDA tensors, where ``delta_block_cuda`` runs the
-DeltaBlock mixer forward and backward on the sm_90a kernels, and with ``model.encoder_path == 'cuda'`` on CUDA tensors
-that need no gradient, where ``encoder_cuda`` does the same for the feature encoder.
+DeltaBlock mixer forward and backward on the sm_90a kernels, with ``model.encoder_path == 'cuda'`` on CUDA tensors
+that need no gradient, where ``encoder_cuda`` does the same for the feature encoder, and with ``model.corr_path ==
+'cuda'`` on CUDA tensors (S = 8, feature maps of at least 8x8), where ``local_corr_cuda`` computes the local correlation
+and its gradients without the all-pairs volumes.
 
 Not used -- and not a fallback -- for plain inference: that path is CUDA-only (pips.py).
 """
@@ -685,6 +687,87 @@ def encoder_cuda(fnet, rgbs):
     return f.reshape(B, S, H8, W8, f.shape[-1]).permute(0, 1, 4, 2, 3)
 
 
+class _LocalCorrFn(torch.autograd.Function):
+    """The 196 correlation columns of pips_corr_gather, differentiable in the ffeats and the 4 levels.  The forward is
+    pips_corr_gather into an fp32 row buffer, so it has the bits the inference path feeds its mixer; the backward is
+    pips_corr_grad_feats and pips_corr_grad_levels.  Saves the inputs only: no all-pairs volume exists in either
+    direction."""
+
+    @staticmethod
+    def forward(ctx, coords, ffeat_rows, *levels):
+        from . import _lib as L
+        lib = L.load()
+        B, S, N, _ = coords.shape
+        H, W = levels[0].shape[1:3]
+        dev = coords.device
+        st = torch.cuda.current_stream(dev).cuda_stream
+        x = torch.empty(B * N * S, L.KPAD, device=dev)
+        times = torch.zeros(S, device=dev)                      # the embedding columns are not returned
+        L.check(lib.pips_corr_gather(L.ptr_array(levels), L.FEAT_F32, B, S, N, H, W, L.ptr(coords), L.ptr(ffeat_rows),
+                                     L.ptr(times), None, 0, None, None, L.ptr(x), L.KPAD, st), "pips_corr_gather")
+        ctx.save_for_backward(coords, ffeat_rows, *levels)
+        return x[:, 128:324].reshape(B * N, S, 196).contiguous()      # frees the other 380 columns of the row buffer
+
+    @staticmethod
+    def backward(ctx, grad):
+        from . import _lib as L
+        lib = L.load()
+        coords, ffeat_rows, *levels = ctx.saved_tensors
+        B, S, N, _ = coords.shape
+        H, W = levels[0].shape[1:3]
+        dev = coords.device
+        st = torch.cuda.current_stream(dev).cuda_stream
+        # the gradient of a column slice of the mixer input arrives with the mixer input's row stride
+        if grad.stride(2) != 1 or grad.stride(0) != S * grad.stride(1) or grad.stride(1) < 196:
+            grad = grad.contiguous()
+        ld = grad.stride(1)
+        dff = None
+        if ctx.needs_input_grad[1]:
+            dff = torch.empty(B * N, S, 128, device=dev)
+            L.check(lib.pips_corr_grad_feats(L.ptr_array(levels), B, S, N, H, W, L.ptr(coords), L.ptr(grad), ld, L.ptr(dff),
+                                             st), "pips_corr_grad_feats")
+        dls = [None] * len(levels)
+        if any(ctx.needs_input_grad[2:]):
+            dls = [torch.empty_like(lv) for lv in levels]
+            L.check(lib.pips_corr_grad_levels(B, S, N, H, W, L.ptr(coords), L.ptr(ffeat_rows), L.ptr(grad), ld,
+                                              L.ptr_array(dls), st), "pips_corr_grad_levels")
+        return (None, dff, *dls)
+
+
+def local_corr_cuda(ffeat_rows, levels, coords):
+    """The local correlation of forward_torch (nets/pips.py:355-398: the all-pairs volumes of the 4 levels sampled at
+    the 49 taps around each track) on the sm_90a kernels, differentiable in ``ffeat_rows`` and in each level, never in
+    ``coords`` (detached at the top of every iteration, nets/pips.py:500).  ffeat_rows (B*N, S, 128) fp32; levels the 4
+    channels-last (B*S, H>>l, W>>l, 128) fp32 pyramid levels; coords (B, S, N, 2) fp32 in feature-map pixels.  Returns
+    fcorr (B*N, S, 196): channel l*49 + a*7 + b samples x = cx/2^l + a - 3, y = cy/2^l + b - 3, as forward_torch's.
+    Neither direction builds an all-pairs volume.  S = 8 and a level 0 of at least 8x8 only; allocates through torch's
+    caching allocator on the inputs' device and runs on its current stream, with no CUDA graph and no cache."""
+    levels = list(levels)
+    if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in [ffeat_rows, coords] + levels):
+        raise RuntimeError("local_corr_cuda runs on the CUDA kernels only; use forward_torch's matmul + grid_sample "
+                           "for CPU tensors")
+    if coords.dim() != 4 or coords.shape[1] != 8 or coords.shape[3] != 2:
+        raise ValueError(f"local_corr_cuda: coords must be (B, 8, N, 2) (S = 8 frames); got {tuple(coords.shape)}")
+    B, S, N, _ = coords.shape
+    if B == 0 or N == 0:
+        raise ValueError("local_corr_cuda: no tracks")
+    if tuple(ffeat_rows.shape) != (B * N, S, 128):
+        raise ValueError(f"local_corr_cuda: ffeat_rows must be (B*N, S, 128) = {(B * N, S, 128)}; got {tuple(ffeat_rows.shape)}")
+    if len(levels) != 4 or levels[0].dim() != 4:
+        raise ValueError("local_corr_cuda: levels must be the 4 channels-last pyramid levels (B*S, H>>l, W>>l, 128)")
+    H, W = levels[0].shape[1:3]
+    if H < 8 or W < 8:
+        raise ValueError(f"local_corr_cuda: level 0 must be at least 8x8; got {H}x{W}")
+    for l, lv in enumerate(levels):
+        if tuple(lv.shape) != (B * S, H >> l, W >> l, 128):
+            raise ValueError(f"local_corr_cuda: level {l} must be {(B * S, H >> l, W >> l, 128)}; got {tuple(lv.shape)}")
+    if any(t.dtype != torch.float32 or t.device != coords.device for t in [ffeat_rows] + levels) \
+            or coords.dtype != torch.float32:
+        raise ValueError("local_corr_cuda: every input must be float32 on one device")
+    with torch.cuda.device(coords.device):
+        return _LocalCorrFn.apply(coords.detach().contiguous(), ffeat_rows.contiguous(), *(lv.contiguous() for lv in levels))
+
+
 def sample_clamped(im, x, y):
     """utils/samp.py:5-78: bilinear sample with clamped indices and unclamped weights -> (B,N,C)."""
     B, C, H, W = im.shape
@@ -743,27 +826,38 @@ def forward_torch(model, xys, rgbs, coords_init=None, feat_init=None, iters=3, t
     # dense score maps fcps (B,S,iters,N,H8,W8) are never built
     fused = (trajs_g is not None and getattr(model, "loss_path", "torch") == "fused"
              and all(t.is_cuda for t in (rgbs, trajs_g, vis_g, valids)))
+    # corr_path='cuda': the correlation comes from local_corr_cuda over channels-last levels (built once; a no-op after
+    # encoder_cuda, whose channels-last strides avg_pool2d keeps), so no all-pairs volume is kept for a backward; the
+    # volumes are only built where the dense score maps need them
+    corr_cuda = (getattr(model, "corr_path", "torch") == "cuda" and rgbs.is_cuda and S == 8 and H8 >= 8 and W8 >= 8)
+    if corr_cuda:
+        levels_cl = [lv.permute(0, 1, 3, 4, 2).contiguous().flatten(0, 1) for lv in pyramid]
     preds, anim, fcps, ffeats_per_iter = [], [coords.detach() * stride] * 2, [], []
     for _ in range(iters):
         coords = coords.detach()
-        vols = [torch.matmul(ffeats, f.flatten(3)).reshape(B, S, N, *f.shape[-2:]) / torch.sqrt(torch.tensor(float(f.shape[2])))
-                for f in pyramid]                                               # :384-398
+        feats_ = ffeats.permute(0, 2, 1, 3).reshape(B * N, S, -1)
+        vols = None
+        if not (corr_cuda and fused):
+            vols = [torch.matmul(ffeats, f.flatten(3)).reshape(B, S, N, *f.shape[-2:]) / torch.sqrt(torch.tensor(float(f.shape[2])))
+                    for f in pyramid]                                           # :384-398
         if fused:
             ffeats_per_iter.append(ffeats)
         else:
             fcp = sum(F.interpolate(v.flatten(0, 1), (H8, W8), mode="bilinear", align_corners=True).reshape(B, S, N, H8, W8)
                       for v in vols)                                            # :504-511
             fcps.append(fcp)
-        taps = []
-        for i, v in enumerate(vols):                                            # :355-382
-            h, w = v.shape[-2:]
-            loc = coords.reshape(B * S * N, 1, 1, 2) / 2 ** i + window
-            grid = torch.cat([2 * loc[..., :1] / (w - 1) - 1, 2 * loc[..., 1:] / (h - 1) - 1], dim=-1)
-            taps.append(F.grid_sample(v.reshape(B * S * N, 1, h, w), grid, align_corners=True).view(B, S, N, -1))
-        fcorr = torch.cat(taps, dim=-1).permute(0, 2, 1, 3).reshape(B * N, S, -1)
+        if corr_cuda:
+            fcorr = local_corr_cuda(feats_, levels_cl, coords)                  # :355-382 on sm_90a
+        else:
+            taps = []
+            for i, v in enumerate(vols):                                        # :355-382
+                h, w = v.shape[-2:]
+                loc = coords.reshape(B * S * N, 1, 1, 2) / 2 ** i + window
+                grid = torch.cat([2 * loc[..., :1] / (w - 1) - 1, 2 * loc[..., 1:] / (h - 1) - 1], dim=-1)
+                taps.append(F.grid_sample(v.reshape(B * S * N, 1, h, w), grid, align_corners=True).view(B, S, N, -1))
+            fcorr = torch.cat(taps, dim=-1).permute(0, 2, 1, 3).reshape(B * N, S, -1)
         flow = (coords - coords[:, 0:1]).permute(0, 2, 1, 3).reshape(B * N, S, 2)
         flow = torch.cat([flow, times.expand(B * N, -1, -1)], dim=2)
-        feats_ = ffeats.permute(0, 2, 1, 3).reshape(B * N, S, -1)
         x_mix = torch.cat([feats_, fcorr, motion_embedding(flow)], dim=2)
         if getattr(model, "mixer_path", "torch") == "cuda" and x_mix.is_cuda:
             delta = delta_block_cuda(model.delta_block, x_mix)                                      # :524 on sm_90a

@@ -3,9 +3,12 @@ torch_path.delta_block_cuda, each new backward kernel alone, and a whole trainin
 three losses) with loss_path='fused' and mixer_path 'torch' against 'cuda'.  The feature encoder likewise: its forward +
 backward on the torch module (strict fp32, as forward_torch runs it) against torch_path.encoder_cuda at 32 and 128 frames
 of 384 x 512, its backward kernels alone, and training steps with encoder_path 'torch' against 'cuda' (loss_path='fused',
-mixer_path='cuda') at B=4 and at train.py's single-GPU default B=16 (N=768, 4 iterations).
+mixer_path='cuda') at B=4 and at train.py's single-GPU default B=16 (N=768, 4 iterations).  The local correlation
+likewise: its forward + backward over 4 iterations as forward_torch runs it (matmul volumes and grid_sample) against
+torch_path.local_corr_cuda, its two backward kernels alone, and training steps with corr_path 'torch' against 'cuda'
+(loss_path='fused', mixer and encoder 'cuda'), at B=4 and B=16.
 
-    python tools/bench_train.py [--reps 5] [--skip-step] [--only mixer|encoder]
+    python tools/bench_train.py [--reps 5] [--skip-step] [--only mixer|encoder|corr]
 
 Shapes: train.py's per-GPU shape (B=4, N=768, 4 iterations, 8 x 384 x 512, stride 8: R = 3072 tracks, M = 24576 mixer
 rows) and BASELINE cfg 2 (N=1024, 6 iterations: M = 32768).  Medians of --reps timed runs after two warm-ups, CUDA
@@ -292,25 +295,145 @@ def bench_encoder_step(reps):
         del rgbs
 
 
+def corr_inputs(B, N=768, H8=48, W8=64, seed=5):
+    """4 iterations' ffeat rows (B*N, 8, 128) and coordinates (B, 8, N, 2), channels-last levels of an avg-pooled
+    pyramid, and an upstream gradient per iteration: forward_torch's correlation inputs at 384 x 512, stride 8"""
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    fm = torch.randn(B * 8, H8, W8, 128, device=DEV, generator=g)
+    levels = [fm]
+    for _ in range(3):
+        levels.append(torch.nn.functional.avg_pool2d(levels[-1].permute(0, 3, 1, 2), 2).permute(0, 2, 3, 1).contiguous())
+    ff = [torch.randn(B * N, 8, 128, device=DEV, generator=g) for _ in range(4)]
+    co = [torch.rand(B, 8, N, 2, device=DEV, generator=g) * torch.tensor([W8 - 1.0, H8 - 1.0], device=DEV) for _ in range(4)]
+    dc = [torch.randn(B * N, 8, 196, device=DEV, generator=g) for _ in range(4)]
+    return ff, levels, co, dc
+
+
+def torch_corr(ff_rows, levels, coords):
+    """forward_torch's correlation (nets/pips.py:355-398): matmul all-pairs volumes and grid_sample, (B*N, S, 196)"""
+    B, S, N, _ = coords.shape
+    ffeats = ff_rows.reshape(B, N, S, 128).permute(0, 2, 1, 3)
+    offs = torch.linspace(-3, 3, 7, device=DEV)
+    window = torch.stack(torch.meshgrid(offs, offs, indexing="ij"), dim=-1).view(1, 7, 7, 2)
+    taps = []
+    for i, lv in enumerate(levels):
+        f = lv.reshape(B, S, *lv.shape[1:]).permute(0, 1, 4, 2, 3)          # (B,S,C,h,w), channels-last strides
+        h, w = f.shape[-2:]
+        v = torch.matmul(ffeats, f.flatten(3)).reshape(B, S, N, h, w) / torch.sqrt(torch.tensor(128.0))
+        loc = coords.reshape(B * S * N, 1, 1, 2) / 2 ** i + window
+        grid = torch.cat([2 * loc[..., :1] / (w - 1) - 1, 2 * loc[..., 1:] / (h - 1) - 1], dim=-1)
+        taps.append(torch.nn.functional.grid_sample(v.reshape(B * S * N, 1, h, w), grid, align_corners=True).view(B, S, N, -1))
+    return torch.cat(taps, dim=-1).permute(0, 2, 1, 3).reshape(B * N, S, -1)
+
+
+def bench_corr(reps):
+    """the correlation's forward + backward over 4 iterations, torch against local_corr_cuda, and each backward kernel"""
+    old = strict_fp32()
+    try:
+        for B in (4, 16):
+            ff, levels, co, dc = corr_inputs(B)
+            for name in ("torch", "cuda"):
+                def step():
+                    lv = [l.requires_grad_(True) for l in levels]
+                    fr = [f.requires_grad_(True) for f in ff]
+                    loss = 0
+                    for i in range(4):
+                        out = torch_path.local_corr_cuda(fr[i], lv, co[i]) if name == "cuda" else torch_corr(fr[i], lv, co[i])
+                        loss = loss + (out * dc[i]).sum()
+                    loss.backward()
+                    for t in lv + fr:
+                        t.grad = None
+                try:
+                    ms = timed(step, reps)
+                    gib = peak_of(step)
+                    print(f"correlation fwd+bwd, 4 iterations, B={B}, N=768, 48x64 {name:5s}: {ms:8.2f} ms, peak "
+                          f"{gib * 1024:7.0f} MiB above inputs")
+                except torch.cuda.OutOfMemoryError:
+                    print(f"correlation fwd+bwd, 4 iterations, B={B}, N=768, 48x64 {name:5s}: out of memory")
+                torch.cuda.empty_cache()
+            for t in levels + ff:
+                t.requires_grad_(False)
+            # each backward kernel alone; bytes it must move, from shapes
+            lib = L.load()
+            st = torch.cuda.current_stream().cuda_stream
+            N, M = 768, B * 8 * 768
+            lv_bytes = sum(l.numel() for l in levels) * 4
+            dff = torch.empty(B * N, 8, 128, device=DEV)
+            dls = [torch.empty_like(l) for l in levels]
+            fn = lambda: L.check(lib.pips_corr_grad_feats(L.ptr_array(levels), B, 8, N, 48, 64, L.ptr(co[0]), L.ptr(dc[0]), 196,
+                                                          L.ptr(dff), st))
+            ms = timed(fn, 20, 3)
+            # compulsory traffic: read every level pixel once, each unit's 196 dcorr and coordinates, write its dffeat row;
+            # the footprint boxes move 4 x 64 px x 512 B per unit, mostly from L2 (neighbouring tracks share pixels)
+            byt = lv_bytes + M * (196 * 4 + 8 + 512)
+            print(f"corr_grad_feats B={B} (M={M}): {ms * 1e3:8.1f} us, {byt / 2**20:.0f} MiB compulsory, "
+                  f"{byt / (ms * 1e-3) / 3.35e12:.2f} of 3.35 TB/s; footprint boxes {M * 4 * 64 * 512 / 2**30:.1f} GiB "
+                  f"at {M * 4 * 64 * 512 / (ms * 1e-3) / 1e12:.1f} TB/s")
+            fn = lambda: L.check(lib.pips_corr_grad_levels(B, 8, N, 48, 64, L.ptr(co[0]), L.ptr(ff[0]), L.ptr(dc[0]), 196,
+                                                           L.ptr_array(dls), st))
+            ms = timed(fn, 20, 3)
+            # compulsory traffic: write every level pixel once, read each unit's ffeat row, 196 dcorr and coordinates once
+            byt = lv_bytes + M * (512 + 196 * 4 + 8)
+            print(f"corr_grad_levels B={B} (M={M}): {ms * 1e3:8.1f} us, {byt / 2**20:.0f} MiB compulsory, "
+                  f"{byt / (ms * 1e-3) / 3.35e12:.2f} of 3.35 TB/s")
+            del ff, levels, co, dc, dff, dls
+            torch.cuda.empty_cache()
+    finally:
+        torch.backends.cudnn.enabled, torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
+
+
+def bench_corr_step(reps):
+    for B in (4, 16):
+        N, iters = 768, 4
+        rgbs = po.smooth_video(B, 8, 384, 512, seed=1).to(DEV)
+        xys = po.random_queries(B, N, 384, 512, seed=2).to(DEV)
+        g = torch.Generator().manual_seed(3)
+        tg = (xys.cpu()[:, None] + torch.cumsum(torch.randn(B, 8, N, 2, generator=g) * 3.0, 1)).to(DEV)
+        vg = torch.ones(B, 8, N, device=DEV)
+        va = torch.ones(B, 8, N, device=DEV)
+        for corr in ("torch", "cuda"):
+            m = Pips(S=8, stride=8, loss_path="fused", mixer_path="cuda", encoder_path="cuda", corr_path=corr).to(DEV).train()
+            m.load_state_dict(po.init_state_dict(seed=3, head_scale=0.05))
+
+            def step():
+                m.zero_grad(set_to_none=True)
+                _, _, _, losses = m(xys, rgbs, iters=iters, trajs_g=tg, vis_g=vg, valids=va, is_train=True)
+                sum(losses).backward()
+            label = f"training step B={B}, N={N}, {iters} iterations (mixer, encoder cuda, fused loss), corr {corr:5s}"
+            try:
+                ms = timed(step, reps, warm=1)
+                gib = peak_of(step)
+                print(f"{label}: {ms:8.1f} ms, peak {gib:6.2f} GiB")
+            except torch.cuda.OutOfMemoryError:
+                print(f"{label}: does not fit in {torch.cuda.get_device_properties(0).total_memory / 2**30:.0f} GiB")
+            del m
+            torch.cuda.empty_cache()
+        del rgbs
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--skip-step", action="store_true")
-    ap.add_argument("--only", choices=("mixer", "encoder"))
+    ap.add_argument("--only", choices=("mixer", "encoder", "corr"))
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_train.py measures on the GPU; no CUDA device found")
     print(f"card: {card()}")
-    if args.only != "encoder":
+    if args.only in (None, "mixer"):
         bench_kernels(args.reps)
         bench_mixer(args.reps)
         if not args.skip_step:
             bench_step(args.reps)
-    if args.only != "mixer":
+    if args.only in (None, "encoder"):
         bench_encoder_kernels(args.reps)
         bench_encoder(args.reps)
         if not args.skip_step:
             bench_encoder_step(args.reps)
+    if args.only in (None, "corr"):
+        bench_corr(args.reps)
+        if not args.skip_step:
+            bench_corr_step(args.reps)
 
 
 if __name__ == "__main__":
