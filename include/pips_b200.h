@@ -58,7 +58,9 @@ int pips_pyramid_build_nhwc(const float* fmaps_nhwc, int frames, int H, int W,
                             float* const* lvl_f32, void* const* lvl_bf16, void* stream);
 
 /* utils/samp.py:5-78 via nets/pips.py:463-466: bilinear gather of frame 0 at the query (indices
- * clamped, weights not), broadcast over S.  coords is the full (B,S,N,2) state (frame 0 is read). */
+ * clamped, weights not), broadcast over S.  coords is the full (B,S,N,2) state (frame 0 is read).  With frame_base
+ * (chained tracking) "frame 0" is the first frame of track (b,n)'s window, decoded as in pips_corr_gather: frame
+ * min(base, T-1) of clip b for base >= 0, min(~base, T-1) for a backward window (base < 0). */
 int pips_init_gather(const float* lvl0_f32, int B, int S, int N, int H, int W, const float* coords,
                      const int* frame_base /* NULL or [B*N] */, int frames_per_batch,
                      float* ffeat /* (B*N,128) */, float* ffeats /* (B*N,S,128) */, void* stream);
@@ -68,7 +70,9 @@ int pips_init_gather(const float* lvl0_f32, int B, int S, int N, int H, int W, c
  *   [ ffeat 128 | corr 4x49 | sin/cos(flow_x) 64 | (flow_y) 64 | (t) 64 | flow_x flow_y t | 0-pad to 576 ]
  * for every (b,n,s) without materialising the all-pairs volume.  Any of x_hi/x_lo/x_f32 may be NULL.
  * Chained long-video tracking (chain_demo.py:40-83): when frame_base is non-NULL the pyramid holds
- * frames_per_batch (T) frames per batch element and track (b,n) reads frames min(frame_base[b*N+n] + s, T-1). */
+ * frames_per_batch (T) frames per batch element and track (b,n) with base = frame_base[b*N+n] reads, at step s,
+ * frame min(base + s, T-1) when base >= 0 (a forward window), and frame max(t - s, 0) with t = min(~base, T-1) when
+ * base < 0 (a backward window from frame t: the chain on the time-reversed clip). */
 int pips_corr_gather(const void* const* lvl, int feat_dtype, int B, int S, int N, int H, int W,
                      const float* coords, const float* ffeats, const float* times /* [S] */,
                      const int* frame_base /* NULL or [B*N] */, int frames_per_batch,

@@ -26,6 +26,16 @@ struct CgArgs {
     int ldx;
 };
 
+// Frame index, inside its clip of T frames, of step s of a chained track's window (pips_init_gather reads step 0,
+// pips_corr_gather steps 0..7).  base >= 0: a forward window from frame base, min(base + s, T-1) -- past the clip's
+// end the last frame is replicated (chain_demo.py:50-52).  base < 0: a backward window from frame t = ~base (base =
+// -1-t), max(t - s, 0) -- the same chain run on the time-reversed clip, whose last frame is frame 0 (t is clamped
+// to T-1, as base is on the forward side).  Both kernels decode through this helper so that they agree on which
+// frame a window starts at.
+__device__ __forceinline__ int window_frame(int base, int s, int T) {
+    return base >= 0 ? min(base + s, T - 1) : max(min(~base, T - 1) - s, 0);
+}
+
 struct UnitInfo {
     float cx, cy;      // coords of (b,s,n), level-0 pixels
     int frame;         // pyramid frame index
@@ -48,8 +58,7 @@ __device__ __forceinline__ UnitInfo load_unit(const CgArgs& a, int u, int total)
         ui.b = seq / a.N; ui.n = seq - ui.b * a.N;
         const float2 c = *reinterpret_cast<const float2*>(a.coords + ((static_cast<size_t>(ui.b) * 8 + ui.s) * a.N + ui.n) * 2);
         ui.cx = c.x; ui.cy = c.y;
-        // chained windows replicate the clip's last frame past its end (chain_demo.py:50-52)
-        ui.frame = a.frame_base ? ui.b * a.T + min(a.frame_base[seq] + ui.s, a.T - 1) : ui.b * 8 + ui.s;
+        ui.frame = a.frame_base ? ui.b * a.T + window_frame(a.frame_base[seq], ui.s, a.T) : ui.b * 8 + ui.s;
         const int level = threadIdx.x & 3;
         const float sc = 1.0f / static_cast<float>(1 << level);        // coords / 2**i  (nets/pips.py:373), exact
         const float cxl = fminf(fmaxf(c.x * sc, -8.0f), static_cast<float>(a.W[level]) + 8.0f);

@@ -1,7 +1,7 @@
 // Correlation pyramid and initial feature gather (run once per forward, upstream of the loop).
 //   pips_pyramid_build  nets/pips.py:346-352   NCHW fp32 fmaps -> 4 channels-last levels (fp32, + optional bf16 copy)
 //   pips_init_gather    utils/samp.py:5-78     bilinear sample of frame 0 at the queries, indices clamped
-#include "common.cuh"
+#include "corr_common.cuh"   // window_frame: the chained-window decode pips_corr_gather uses
 
 namespace pips {
 
@@ -80,7 +80,7 @@ __global__ void init_gather_kernel(const float* __restrict__ lvl0, int B, int S,
     const int y1 = static_cast<int>(fminf(fmaxf(y1f, 0.f), static_cast<float>(H - 1)));
     const float w00 = (x1f - x) * (y1f - y), w01 = (x - x0f) * (y1f - y);
     const float w10 = (x1f - x) * (y - y0f), w11 = (x - x0f) * (y - y0f);
-    const int frame = frame_base ? b * T + min(frame_base[warp], T - 1) : b * S;  // first frame of the track's window
+    const int frame = frame_base ? b * T + window_frame(frame_base[warp], 0, T) : b * S;  // first frame of the track's window
     const float* img = lvl0 + static_cast<size_t>(frame) * H * W * 128;
     const float4 a = *reinterpret_cast<const float4*>(img + (static_cast<size_t>(y0) * W + x0) * 128 + lane * 4);
     const float4 bq = *reinterpret_cast<const float4*>(img + (static_cast<size_t>(y0) * W + x1) * 128 + lane * 4);
