@@ -12,15 +12,22 @@
 // Structure (one CTA per SM, persistent over 128 x BN output tiles; BN = 256 for large problems, 128 / 64 when
 // 256-wide tiles would leave most SMs without a tile -- few particles: the demo clip, chained windows):
 //   warp 0       TMA producer  : cp.async.bulk.tensor 64B-swizzled 32-wide K-blocks of A and W -> smem ring
+//   warps 1..3   epilogue warps (BN = 256): bias / GELU + (hi, lo) split / residual of the tiles handed over to them
 //   warps 4..7   consumer warpgroup 0: rows 0..63 of the tile   } wgmma m64nBNk16 straight from the ring, then the
-//   warps 8..11  consumer warpgroup 1: rows 64..127             } epilogue (below)
-// The ring is 4 (x3, BN = 256) to 8 stages deep, so a slot's TMA has several K-blocks of MMAs to land in, and the
-// producer runs ahead into the next tile while the consumers are in their epilogue.
+//   warps 8..11  consumer warpgroup 1: rows 64..127             } epilogue or the handoff (below)
+// The ring is 3 (x3, BN = 256) to 8 stages deep, so a slot's TMA has several K-blocks of MMAs to land in.
 //
-// Epilogue: bias / GELU + (hi, lo) split in registers, then 32-column chunks of the warpgroup's 64 rows go through a
-// double-buffered staging area in shared memory to one TMA store per chunk (a TMA add-reduce for the residual).  No
-// thread waits on global memory; the stores of a tile's last chunks drain while the next tile's MMAs run.  TMA clips
-// the boxes at M and N, which covers partial tiles.
+// Epilogue, BN = 256: a consumer writes its 64 x 256 accumulator into a shared-memory handoff buffer (one warpgroup's
+// half; the two take turns, guarded by mbarriers) as 32-column fp32 chunks in the 128-byte-swizzled layout of the fp32
+// store box, and goes straight on to the next tile's MMAs.  The epilogue warps add the bias chunk by chunk -- in place,
+// then a TMA store (a TMA add-reduce for the residual); or for GELU they write the bf16 hi and lo boxes over the chunk's
+// fp32 values -- so the GELU runs under the next tile's MMAs.  The epilogue warps are the producer warpgroup's idle
+// warps.  A fourth, dedicated warpgroup (512 threads, registers split with setmaxnreg) measured slower: the 128-register
+// launch bound of a 512-thread CTA is below what ptxas needs to compile one m64n256k16 wgmma (C7602, "register target
+// of 154"), so its consumers must issue two m64n128k16 per term and read A twice; FC2 and gemm_in lost 4-9 %.
+// BN = 128 / 64: bias / GELU + (hi, lo) split in the consumers' registers, then 32-column chunks of the warpgroup's 64
+// rows go through a double-buffered staging area in shared memory to one TMA store per chunk.  No thread waits on
+// global memory.  TMA clips the boxes at M and N, which covers partial tiles.
 //
 // CLUSTER = 2 ("pair" tiles, 256 x 256 per cluster): the two CTAs of a cluster take the two 128-row halves of the tile
 // and share its W tile -- each loads one 128-row half of W and TMA-multicasts it into both shared memories, which
@@ -39,18 +46,25 @@ constexpr int GEMM_THREADS = 384;                      // producer warpgroup + 2
 constexpr uint32_t A_TILE_BYTES = BM * KB * 2;         // 8 KB
 constexpr int EPI_COLS = 32;                           // epilogue chunk: 32 columns of a warpgroup's 64 rows
 constexpr uint32_t EPI_BUF_BYTES = 64 * EPI_COLS * 4;  // 8 KB: an fp32 chunk, or a bf16 hi chunk + a bf16 lo chunk
-constexpr uint32_t EPI_STAGING_BYTES = 2 * 2 * EPI_BUF_BYTES;   // two buffers per consumer warpgroup
+constexpr uint32_t EPI_STAGING_BYTES = 2 * 2 * EPI_BUF_BYTES;   // in-consumer epilogue: two buffers per consumer warpgroup
+constexpr int EPI_THREADS = 96;                        // epilogue warps: warps 1..3 of the producer warpgroup
 
-template <int TERMS, int BN>
+// kHandoff: the 256-wide inference tiles, whose consumers hand their accumulators to epilogue warps through a buffer
+// of one 64 x BN fp32 half (a buffer for both halves leaves room for only 2 ring stages, and measured slower).
+// Otherwise (128 / 64-wide tiles, aux, weight gradient): the consumers run the epilogue from registers.
+template <int TERMS, int BN, bool INFERENCE = false>
 struct GemmCfg {
+    static constexpr bool kHandoff = INFERENCE && BN == 256;
     static constexpr uint32_t kWTileBytes = BN * KB * 2;                  // 16 / 8 / 4 KB
     static constexpr int kOperandCopies = TERMS == 3 ? 2 : 1;             // hi (+ lo)
     static constexpr uint32_t kStageBytes = kOperandCopies * (A_TILE_BYTES + kWTileBytes);
-    static constexpr uint32_t kFixedBytes = 1024 /*align*/ + EPI_STAGING_BYTES + 256 /*barriers*/;
+    static constexpr uint32_t kHalfBytes = 64 * BN * 4;                   // one consumer warpgroup's fp32 accumulator
+    static constexpr uint32_t kEpiBytes = kHandoff ? kHalfBytes : EPI_STAGING_BYTES;
+    static constexpr uint32_t kFixedBytes = 1024 /*align*/ + kEpiBytes + 256 /*barriers*/;
     static constexpr int kFit = static_cast<int>((227u * 1024u - kFixedBytes) / kStageBytes);
-    static constexpr int kStages = kFit > 8 ? 8 : kFit;                   // x3: 4 / 6 / 8 for BN = 256 / 128 / 64
+    static constexpr int kStages = kFit > 8 ? 8 : kFit;
     static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kFixedBytes;
-    static_assert(kStages >= 4 && kSmemBytes <= 227u * 1024u, "ring + staging must fit in 227 KB");
+    static_assert(kStages >= 3 && kSmemBytes <= 227u * 1024u, "ring + epilogue buffer must fit in 227 KB");
 };
 
 struct GemmArgs {
@@ -169,6 +183,73 @@ __device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArg
     }
 }
 
+// The epilogue warps' work on one consumer warpgroup's 64 x BN accumulator, handed off at `buf` as BN / 32 chunks
+// of 64 rows x 32 fp32 columns (EPI_BUF_BYTES each, 128-byte swizzle: the layout the fp32 store box reads).  Per chunk:
+// add the bias in place and store / add-reduce the chunk, or for BIAS_GELU write GELU's (hi, lo) split over the chunk's
+// fp32 values as a 64-byte-swizzled bf16 hi box and lo box and store those.  Run by EPI_THREADS threads; thread t takes
+// the 16-byte units t + EPI_THREADS i of a chunk: rows t / 8 + EPI_ROWS i, columns 4 (t % 8) .. + 3, so its four bias
+// values serve every row.  Each value meets the operations of the in-consumer epilogue in the same order: the same bits.
+template <int BN>
+__device__ __forceinline__ void epilogue_handoff(const GemmMaps& maps, const GemmArgs& args, uint32_t buf, int row0, int n0) {
+    constexpr int EPI_ROWS = EPI_THREADS / 8;                             // rows per pass over the threads
+    constexpr int PASSES = (64 + EPI_ROWS - 1) / EPI_ROWS;
+    const int t = threadIdx.x - 32;
+    const int u = t & 7;
+    const bool issuer = t == 0;
+    const bool gelu = args.epilogue == PIPS_EPI_BIAS_GELU;
+#pragma unroll 1
+    for (int c = 0; c < BN / EPI_COLS; ++c) {
+        const int col0 = n0 + c * EPI_COLS;
+        if (col0 >= args.N) break;
+        const uint32_t chunk = buf + c * EPI_BUF_BYTES;
+        const int col = col0 + 4 * u;
+        const float2 b01 = make_float2(col < args.N ? __ldg(args.bias + col) : 0.f, col + 1 < args.N ? __ldg(args.bias + col + 1) : 0.f);
+        const float2 b23 = make_float2(col + 2 < args.N ? __ldg(args.bias + col + 2) : 0.f, col + 3 < args.N ? __ldg(args.bias + col + 3) : 0.f);
+        float4 v[PASSES];
+#pragma unroll
+        for (int i = 0; i < PASSES; ++i)
+            if ((t >> 3) + EPI_ROWS * i < 64) v[i] = ld_shared_f32x4(chunk + staged<EPI_COLS * 4>((t >> 3) + EPI_ROWS * i, 16 * u));
+        if (gelu) {
+            named_bar_sync(1, EPI_THREADS);                              // the chunk is read: its bf16 boxes go over it
+#pragma unroll
+            for (int i = 0; i < PASSES; ++i) {
+                if ((t >> 3) + EPI_ROWS * i >= 64) break;
+                const float2 g01 = gelu_fast2_abs(add2(make_float2(v[i].x, v[i].y), b01));
+                const float2 g23 = gelu_fast2_abs(add2(make_float2(v[i].z, v[i].w), b23));
+                const uint32_t h01 = cvt_bf16x2(g01.x, g01.y), h23 = cvt_bf16x2(g23.x, g23.y);
+                const uint32_t o = staged<EPI_COLS * 2>((t >> 3) + EPI_ROWS * i, 8 * u);
+                st_shared_u32x2(chunk + o, h01, h23);
+                if (args.out_lo) {
+                    // g - hi, one rounding
+                    const float2 l01 = fma2(make_float2(__uint_as_float(h01 << 16), __uint_as_float(h01 & 0xffff0000u)), bcast2(-1.0f), g01);
+                    const float2 l23 = fma2(make_float2(__uint_as_float(h23 << 16), __uint_as_float(h23 & 0xffff0000u)), bcast2(-1.0f), g23);
+                    st_shared_u32x2(chunk + EPI_BUF_BYTES / 2 + o, cvt_bf16x2(l01.x, l01.y), cvt_bf16x2(l23.x, l23.y));
+                }
+            }
+        } else {
+#pragma unroll
+            for (int i = 0; i < PASSES; ++i) {
+                if ((t >> 3) + EPI_ROWS * i >= 64) break;
+                const float2 f01 = add2(make_float2(v[i].x, v[i].y), b01), f23 = add2(make_float2(v[i].z, v[i].w), b23);
+                st_shared_f32x4(chunk + staged<EPI_COLS * 4>((t >> 3) + EPI_ROWS * i, 16 * u), make_float4(f01.x, f01.y, f23.x, f23.y));
+            }
+        }
+        fence_proxy_async_smem();                                         // make the writes visible to the TMA unit
+        named_bar_sync(1, EPI_THREADS);
+        if (issuer) {
+            if (gelu) {
+                tma_store_2d(&maps.out_hi, chunk, col0, row0);
+                if (args.out_lo) tma_store_2d(&maps.out_lo, chunk + EPI_BUF_BYTES / 2, col0, row0);
+            } else if (args.epilogue == PIPS_EPI_BIAS_RESID) {
+                tma_reduce_add_2d(&maps.out_f32, chunk, col0, row0);     // x + (acc + b): the bits of (acc + b) + x
+            } else {
+                tma_store_2d(&maps.out_f32, chunk, col0, row0);
+            }
+            bulk_commit();
+        }
+    }
+}
+
 // Weight-gradient epilogue: the warpgroup's 64 x 128 fp32 partial sum of one split of M goes straight from registers to
 // its slice of the output (rows n, columns k, row stride args.ldo); rows >= N and columns >= K are not stored.
 __device__ __forceinline__ void epilogue_wgrad(const GemmArgs& args, const float (&acc)[64], float* out, int row0, int k0) {
@@ -195,16 +276,22 @@ __device__ __forceinline__ void epilogue_wgrad(const GemmArgs& args, const float
 // each split's partial sum goes to its own slice of args.out_f32 (N*K floats apart) and is summed in a fixed order later.
 template <int TERMS, int BN, int CLUSTER, bool WGRAD = false, bool AUX = false>
 __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArgs& args) {
-    using Cfg = GemmCfg<TERMS, BN>;
+    using Cfg = GemmCfg<TERMS, BN, !WGRAD && !AUX>;
+    constexpr bool HANDOFF = Cfg::kHandoff;
     constexpr int kStages = Cfg::kStages;
     constexpr uint32_t W_TILE_BYTES = Cfg::kWTileBytes;
     constexpr uint32_t BOX_BYTES = 32 * KB * 2;                    // WGRAD: one {32, 32} box, 2 KB
     static_assert(CLUSTER == 1 || BN == 256, "cluster tiles are 256 columns wide");
     static_assert(!WGRAD || (BN == 128 && CLUSTER == 1 && TERMS == 3), "the weight-gradient variant is bf16x3, 128 x 128");
-    // the 128-byte-swizzled staging buffers need 1024-byte alignment (the 64-byte-swizzled ring needs 512)
+    // the 128-byte-swizzled epilogue buffers need 1024-byte alignment (the 64-byte-swizzled ring needs 512)
     uint8_t* smem = aligned_smem();
     uint8_t* staging = smem + kStages * Cfg::kStageBytes;
-    Ring ring(smem, Cfg::kStageBytes, kStages, reinterpret_cast<uint64_t*>(staging + EPI_STAGING_BYTES), kStages);
+    Ring ring(smem, Cfg::kStageBytes, kStages, reinterpret_cast<uint64_t*>(staging + Cfg::kEpiBytes), kStages);
+    // HANDOFF: the consumer warpgroups take turns in the handoff buffer, 0 then 1 on every tile.  ho_full: a consumer has
+    // filled it (128 arrivals).  ho_empty + 8 wg: the epilogue warps' store issuer has drained the other warpgroup's
+    // turn before wg's, and its stores have read the buffer.  A barrier per warpgroup, so that a warpgroup that runs a
+    // whole tile ahead of the epilogue cannot take a phase meant for the other one.
+    const uint32_t ho_full = smem_u32(staging + Cfg::kEpiBytes) + 16 * kStages, ho_empty = ho_full + 8;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -247,14 +334,23 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
             tma_prefetch_desc(&maps.out_f32);
         }
     }
-    if (warp == 1 && lane == 0) ring.init(2 * CLUSTER);    // one arrival per consumer warpgroup that reads the slot's W
+    if (warp == 1 && lane == 0) {
+        if constexpr (HANDOFF) {
+            mbar_init(ho_full, 128);
+            mbar_init(ho_empty, 1);
+            mbar_init(ho_empty + 8, 1);
+        }
+        ring.init(2 * CLUSTER);                             // one arrival per consumer warpgroup that reads the slot's W
+    }
     if (CLUSTER == 2) cluster_sync_all();                   // the peer's barriers exist before anything is sent to them
     else __syncthreads();
     pdl_wait();                                             // operands and the residual stream come from the previous kernel
 
-    // Register budget per warpgroup: the producer warpgroup needs few, the consumers hold the accumulator.
+    // Register budget per warpgroup: the producer warpgroup needs few, the consumers hold the accumulator.  The HANDOFF
+    // kernels keep the launch's 168 per thread everywhere: their producer warpgroup also runs the epilogue warps, and
+    // the consumers' 128-float accumulator with the mainloop's state fits in 168.
     if (warp < 4) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if constexpr (!HANDOFF) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (warp == 0 && lane == 0) {
             // ------------------------------------------------------------ TMA producer
             for (int t = worker; t < args.num_tiles; t += num_workers) {
@@ -289,14 +385,33 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
                     });
                 }
             }
+        } else if (HANDOFF && warp > 0) {
+            // -------------------------------------------------------- epilogue warps: the consumers' halves in turn
+            const bool issuer = threadIdx.x == 32;
+            uint32_t turn = 0;                              // turns taken; turn 2 i + wg: warpgroup wg on tile i
+            for (int t = worker; t < args.num_tiles; t += num_workers) {
+                int m0, n0, kb0, kb1;
+                tile_coords(t, m0, n0, kb0, kb1);
+                for (int wg = 0; wg < 2; ++wg, ++turn) {
+                    mbar_wait(ho_full, turn & 1);
+                    if (m0 + wg * 64 < args.M)              // else the whole half is past M: nothing to store
+                        epilogue_handoff<BN>(maps, args, smem_u32(staging), m0 + wg * 64, n0);
+                    if (issuer) {
+                        bulk_wait_read<0>();                // the stores have read the buffer: the other warpgroup may fill it
+                        mbar_arrive(ho_empty + 8 * (wg ^ 1));
+                    }
+                }
+            }
+            if (issuer) bulk_wait<0>();                     // the last stores have finished writing
         }
     } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-        // ------------------------------------------------------------ consumers: MMA + epilogue, 64 rows each
+        if constexpr (!HANDOFF) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        // ------------------------------------------------------------ consumers: MMA (+ epilogue), 64 rows each
         const int wg = (warp - 4) >> 2;
         const bool releaser = (threadIdx.x & 127) == 0;
-        const uint32_t my_staging = smem_u32(staging) + wg * 2 * EPI_BUF_BYTES;
+        const uint32_t my_staging = smem_u32(staging) + wg * 2 * EPI_BUF_BYTES;   // in-consumer epilogue
         uint32_t chunk = 0;
+        uint32_t turn = wg;                                  // HANDOFF: this warpgroup's next turn in the handoff buffer
         float acc[BN / 2];
         auto release = [&](int slot) {
             if (releaser) {
@@ -355,11 +470,27 @@ __device__ __forceinline__ void gemm_tc_body(const GemmMaps& maps, const GemmArg
                 const int split = t % splits;
                 float* out = args.out_f32 + static_cast<size_t>(split) * args.N * args.ldo;
                 epilogue_wgrad(args, *reinterpret_cast<const float(*)[64]>(&acc[0]), out, m0 + wg * 64, n0);
-            } else {
+            } else if constexpr (!HANDOFF) {
                 epilogue_tma<BN, AUX>(maps, args, acc, m0 + wg * 64, n0, my_staging, chunk, wg);
+            } else {
+                // hand the accumulator to the epilogue warps as BN / 32 fp32 chunks and go on to the next tile
+                // turn 2 i + wg waits for the (i + wg)-th drain on ho_empty + 8 wg (warpgroup 0's first turn: none)
+                mbar_wait(ho_empty + 8 * wg, ((turn >> 1) + wg + 1) & 1);
+                const uint32_t buf = smem_u32(staging);
+                const int r = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // fragment rows r, r + 8 of the 64
+                const int cq = 2 * (lane & 3);                                // fragment columns cq, cq + 1 of each 8
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        st_shared_f32x2(buf + (j / 4) * EPI_BUF_BYTES + staged<EPI_COLS * 4>(r + 8 * h, (8 * (j % 4) + cq) * 4),
+                                        make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
+                }
+                mbar_arrive(ho_full);
+                turn += 2;
             }
         }
-        if (releaser) bulk_wait<0>();                        // the last stores have finished reading shared memory and writing
+        if (!HANDOFF && releaser) bulk_wait<0>();            // the last stores have finished reading shared memory and writing
     }
     if (CLUSTER == 2) cluster_sync_all();                   // nobody leaves while the peer may still signal or write to us
 }
@@ -582,8 +713,8 @@ static int launch_variant(const GemmMaps& maps, const GemmArgs& args, cudaStream
     GemmArgs a = args;
     a.num_tiles = ((args.M + BM - 1) / BM) * ((args.N + BN - 1) / BN);
     const int grid = a.num_tiles < sm_count() ? a.num_tiles : sm_count();
-    return launch_kernel<gemm_tc_kernel<TERMS, BN>>("pips_gemm_tc", true, grid, GEMM_THREADS, GemmCfg<TERMS, BN>::kSmemBytes, st,
-                                                    maps, a);
+    using Cfg = GemmCfg<TERMS, BN, true>;
+    return launch_kernel<gemm_tc_kernel<TERMS, BN>>("pips_gemm_tc", true, grid, GEMM_THREADS, Cfg::kSmemBytes, st, maps, a);
 }
 
 template <int TERMS>
@@ -592,8 +723,9 @@ static int launch_pair_variant(const GemmMaps& maps, const GemmArgs& args, cudaS
     a.num_tiles = ((args.M + 255) / 256) * ((args.N + 255) / 256);
     const int max_pairs = sm_count() / 2;
     const int pairs = a.num_tiles < max_pairs ? a.num_tiles : max_pairs;
-    return launch_kernel<gemm_tc_pair_kernel<TERMS>>("pips_gemm_tc (pair)", true, 2 * pairs, GEMM_THREADS,
-                                                     GemmCfg<TERMS, 256>::kSmemBytes, st, maps, a);
+    using Cfg = GemmCfg<TERMS, 256, true>;
+    return launch_kernel<gemm_tc_pair_kernel<TERMS>>("pips_gemm_tc (pair)", true, 2 * pairs, GEMM_THREADS, Cfg::kSmemBytes, st,
+                                                     maps, a);
 }
 
 int launch_pair(bool x3, const void* a_hi, const void* a_lo, int lda, int a_rows, const void* w_hi, const void* w_lo, int ldw,

@@ -59,6 +59,17 @@ __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
 __device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float2 v) {
     asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
 }
+__device__ __forceinline__ void st_shared_u32x2(uint32_t addr, uint32_t x, uint32_t y) {
+    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(x), "r"(y) : "memory");
+}
+__device__ __forceinline__ void st_shared_f32x4(uint32_t addr, float4 v) {
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+__device__ __forceinline__ float4 ld_shared_f32x4(uint32_t addr) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+    return v;
+}
 
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const void* map) {
