@@ -177,7 +177,7 @@ def _split(t):
     return hi, lo
 
 
-@pytest.mark.parametrize("pair", [False, True, 128, 64])
+@pytest.mark.parametrize("pair", [False, True, 128, 64, "auto"])
 @pytest.mark.parametrize("terms", [3, 1])
 @pytest.mark.parametrize("M,N,K,epi", [
     (128, 256, 64, L.EPI_BIAS),            # one tile, one K block
@@ -185,50 +185,27 @@ def _split(t):
     (96, 512, 576, L.EPI_BIAS),            # partial M tile, 2 N tiles   (first Linear)
     (1000, 2048, 512, L.EPI_BIAS_GELU),    # FC1
     (1000, 512, 2048, L.EPI_BIAS_RESID),   # FC2
-    (300, 1040, 512, L.EPI_BIAS),          # head: partial N tile
+    (300, 1040, 512, L.EPI_BIAS),          # head: partial N tile, 1280 weight rows
     (40000, 512, 512, L.EPI_BIAS_RESID),   # more tiles than SMs: persistent loop
+    (8 * 300, 512, 576, L.EPI_BIAS),       # the first Linear at 300 sequences
+    (8 * 300, 512, 2048, L.EPI_BIAS_RESID),  # FC2 at 300 sequences
 ])
 def test_gemm_tc(terms, M, N, K, epi, pair, monkeypatch):
     """pair=True: the cluster kernel (256x256 per cluster of two CTAs, W multicast); False / 128 / 64: the single-CTA kernel with
-    128 x 256 / 128 / 64 tiles.  The shape is forced -- left alone, pips_gemm_tc picks it from the problem size."""
-    lib = L.load()
-    torch.manual_seed(7)
-    monkeypatch.setenv("PIPS_B200_GEMM_TILE", "pair" if pair is True else str(pair or 256))
-    Ma, Na = (M + 127) // 128 * 128, (N + 255) // 256 * 256
-    if pair is True:
-        Ma = (M + 255) // 256 * 256
-    elif Ma % 256 == 0 and pair is False:
-        Ma += 128
-    a = torch.zeros(Ma, K)
-    a[:M] = torch.randn(M, K)
-    w = torch.zeros(Na, K)
-    w[:N] = torch.randn(N, K) / math.sqrt(K)
-    bias = torch.randn(N)
-    out0 = torch.randn(M, N)
-    a_hi, a_lo = _split(a)
-    w_hi, w_lo = _split(w)
-    if terms == 3:
-        ref = _gemm_ref(a[:M], w[:N], bias, epi, out0)
-        tol = 2e-4
-    else:
-        ref = _gemm_ref(a_hi[:M].float(), w_hi[:N].float(), bias, epi, out0)
-        tol = 2e-4
-    d = lambda t: t.to(DEV).contiguous()
-    a_hi, a_lo, w_hi, w_lo, bd = d(a_hi), d(a_lo), d(w_hi), d(w_lo), d(bias)
-    of = out0.clone().to(DEV)
-    oh = torch.zeros(M, N, dtype=torch.bfloat16, device=DEV)
-    ol = torch.zeros(M, N, dtype=torch.bfloat16, device=DEV)
-    x3 = terms == 3
-    L.check(lib.pips_gemm_tc(L.ptr(a_hi), L.ptr(a_lo) if x3 else 0, K, Ma, L.ptr(w_hi), L.ptr(w_lo) if x3 else 0, K, Na,
-                             M, N, K, L.ptr(bd), epi, L.ptr(of), N, L.ptr(oh), L.ptr(ol) if x3 else 0, N, _st()))
-    _sync_check()
+    128 x 256 / 128 / 64 tiles; "auto": the shape pips_gemm_tc picks from the problem size.  Exact operands
+    (tests/test_tc_exact_gpu.py): the output must equal the fp64 three-term product bit for bit, at lda = ldw = K + 8,
+    ldo = N + 4, ldh = N + 8, with NaN operand rows past M and N, NaN pitch columns and NaN output rows past M that must
+    stay NaN.  BIAS_GELU: bit for bit with pre-activations in GELU's flat tails, then bounded per element against fp64
+    with pre-activations over the centre and both tails."""
+    from tests.test_tc_exact_gpu import check_exact_gemm, check_gelu_bounded
+    tile = "pair" if pair is True else "" if pair == "auto" else str(pair or 256)
+    monkeypatch.setenv("PIPS_B200_GEMM_TILE", tile)
+    g = torch.Generator(device=DEV).manual_seed(M + N + K + terms)
+    n, bad = check_exact_gemm(M, N, K, epi, terms, g, with_lo=terms == 3)
+    print(f"gemm_tc {M}x{N}x{K} epi={epi} terms={terms} tile={tile or 'auto'}: {n} differing elements, poison overwritten: {bad or 'none'}")
+    assert n == 0 and not bad
     if epi == L.EPI_BIAS_GELU:
-        got = oh.float().cpu() + (ol.float().cpu() if x3 else 0)
-        tol = tol + (2 ** -16 if x3 else 2 ** -8) * ref.abs().max().item()
-    else:
-        got = of.cpu()
-    err = (got - ref).abs().max().item()
-    assert err < tol, f"max err {err} (tol {tol})"
+        check_gelu_bounded(M, N, K, terms, terms == 3, f"tile={tile or 'auto'}")
 
 
 @pytest.mark.parametrize("terms", [3, 1])
