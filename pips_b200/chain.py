@@ -47,63 +47,100 @@ def pick_skip(vis: torch.Tensor, thr_table: torch.Tensor) -> torch.Tensor:
     return (sel.long() * idx).max(dim=1).values
 
 
-def _encode_clip(model, rgbs: torch.Tensor) -> torch.Tensor:
-    """The whole clip's feature maps (1, T, 128, H8, W8), encoded once per frame in chunks of 32 frames."""
+def _encode_clip(model, rgbs: torch.Tensor, held: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The clip's feature maps (1, T, 128, H8, W8), encoded once per frame in chunks of 32 frames; after the ``held``
+    feature maps (1, k, 128, H8, W8) of earlier frames when given."""
     T = rgbs.shape[1]
-    fmaps = torch.cat([model.encode(rgbs[:, t0:t0 + 32]) for t0 in range(0, T, 32)], dim=1)   # (1,T,128,H8,W8)
-    if not fmaps.is_contiguous() and not fmaps.reshape(T, *fmaps.shape[2:]).permute(0, 2, 3, 1).is_contiguous():
+    parts = [] if held is None else [held]
+    fmaps = torch.cat(parts + [model.encode(rgbs[:, t0:t0 + 32]) for t0 in range(0, T, 32)], dim=1)
+    if not fmaps.is_contiguous() and not fmaps.reshape(-1, *fmaps.shape[2:]).permute(0, 2, 3, 1).is_contiguous():
         fmaps = fmaps.contiguous()
     return fmaps
 
 
-def _run_rounds(model, fmaps: torch.Tensor, base0: torch.Tensor, length: torch.Tensor, xy: torch.Tensor, iters: int,
-                advance: Optional[int] = None, want_vis: bool = False):
-    """The round loop shared by track_chain and track_queries: track k runs the reference chain from xy[k] (input
-    pixels) over the length[k] frames of its direction, its first window read through frame_base base0[k] (t for a
-    forward track from frame t, ~t for a backward one, see window_frame in csrc/corr_common.cuh).  A window that
-    starts c frames further on is base0[k] + c in both directions (~(t - c) == ~t + c).  Every round is one
-    refinement call over all tracks still inside their clip.  Returns traj (T, n, 2) indexed by frames from the
-    track's start, vis (T, n) likewise -- sigmoid(vis_e) of the window that last wrote the frame; None unless
-    ``want_vis`` -- and the round count."""
-    T = fmaps.shape[1]
-    n = base0.numel()
+class _Tracks:
+    """Per-track state of the round loop.  Track k runs the reference chain from xy[k] (input pixels) over the
+    length[k] frames of its direction.  Its first window is read through frame_base base0[k], counted in frames of the
+    video: t for a forward track from frame t, ~t for a backward one (see window_frame in csrc/corr_common.cuh).  A
+    window that starts c frames further on is base0[k] + c in both directions (~(t - c) == ~t + c).  Step s of the
+    window at cursor c writes row row0[k] + c + s of traj (rows, n, 2) and vis (rows, n); vis holds sigmoid(vis_e) of
+    the window that last wrote the row, and is None unless ``want_vis``."""
+
+    def __init__(self, base0: torch.Tensor, length: torch.Tensor, xy: torch.Tensor, rows: int, want_vis: bool,
+                 fill: float = 0.0):
+        n = base0.numel()
+        dev = base0.device
+        self.base0, self.length = base0, length
+        self.row0 = torch.zeros(n, dtype=torch.long, device=dev)
+        self.pos = xy.float().clone()                                                # start of each track's next window
+        self.cur = torch.zeros(n, dtype=torch.long, device=dev)
+        self.started = torch.zeros(n, dtype=torch.bool, device=dev)
+        self.done = torch.zeros(n, dtype=torch.bool, device=dev)
+        self.feat: Optional[torch.Tensor] = None                                     # (n, 128) first-window features
+        self.traj = torch.full((rows, n, 2), fill, dtype=torch.float32, device=dev)
+        self.vis = torch.full((rows, n), fill, dtype=torch.float32, device=dev) if want_vis else None
+        self.rounds = 0
+
+
+def _run_rounds(model, fmaps: torch.Tensor, tr: _Tracks, iters: int, advance: Optional[int] = None, f0: int = 0,
+                ended: bool = True) -> None:
+    """The round loop shared by track_chain, track_queries and TrackStream.  fmaps (1, F, 128, H8, W8) holds frames
+    f0 .. f0+F-1 of the video.  Every round is one refinement call over all runnable tracks, each reading its window
+    through its frame_base rebased to the held frames; rounds repeat until no track is runnable.  A track is runnable
+    while it is inside its clip and, unless the video has ``ended``, its whole window has arrived.  A window past the
+    last held frame replicates that frame, which is the end-of-clip rule once the video has ended.  A track's first
+    window gathers its own feature; later windows carry it (outs[3], chain_demo.py:57)."""
+    F = fmaps.shape[1]
     dev = fmaps.device
     eng = model.engine
     stride = float(model.stride)
     thr = _threshold_table().to(dev)
-    traj = torch.zeros(T, n, 2, dtype=torch.float32, device=dev)
-    traj[0] = xy.float()
-    vis = torch.zeros(T, n, dtype=torch.float32, device=dev) if want_vis else None
-    cur = torch.zeros(n, dtype=torch.long, device=dev)
-    feat: Optional[torch.Tensor] = None
-    active = torch.arange(n, device=dev)
-    rounds = 0
-    while active.numel() > 0:
-        na = active.numel()
-        c = cur[active]
-        start = traj[c, active]                                                      # (na, 2) current position
-        coords = (start / stride).view(1, 1, na, 2).repeat(1, S_WIN, 1, 1)           # zero-velocity init, :453
-        fi = None if feat is None else feat[:, active]
-        preds, vis_e, ffeat = eng.refine(model, fmaps, coords, fi, iters, stride,
-                                         frame_base=(base0[active] + c).view(1, na).to(torch.int32),
-                                         reuse_pyramid=rounds > 0)                  # same clip every round
-        if feat is None:
-            feat = ffeat                                                             # outs[3], carried (chain_demo.py:57)
+    steps = torch.arange(S_WIN, device=dev).view(S_WIN, 1)
+    built = False                                                                    # the pyramid of fmaps exists
+    while True:
+        live = ~tr.done
+        if not ended:
+            live &= tr.base0 + tr.cur + (S_WIN - 1) <= f0 + F - 1
+        run = live.nonzero().flatten()
+        na = run.numel()
+        if na == 0:
+            return
+        c = tr.cur[run]
+        fb = (tr.base0[run] + c - f0).view(1, na).to(torch.int32)
+        coords = (tr.pos[run] / stride).view(1, 1, na, 2).repeat(1, S_WIN, 1, 1)    # zero-velocity init, :453
+        new = ~tr.started[run]
+        fi = None
+        if not bool(new.all()):
+            if bool(new.any()):
+                # tracks starting beside carried ones: their first-window features alone (initial gather, no iteration)
+                _, _, f_new = eng.refine(model, fmaps, coords[:, :, new], None, 0, stride, frame_base=fb[:, new],
+                                         reuse_pyramid=built)
+                built = True
+                tr.feat[run[new]] = f_new[0]
+                tr.started[run[new]] = True
+            fi = tr.feat[run].unsqueeze(0)
+        preds, vis_e, ffeat = eng.refine(model, fmaps, coords, fi, iters, stride, frame_base=fb, reuse_pyramid=built)
+        built = True
+        if fi is None:
+            if tr.feat is None:
+                tr.feat = torch.empty(tr.base0.numel(), ffeat.shape[-1], dtype=ffeat.dtype, device=dev)
+            tr.feat[run] = ffeat[0]
+            tr.started[run] = True
         xys = preds[-1][0]                                                           # (8, na, 2)
-        lim = length[active]
-        t_idx = c.view(1, na) + torch.arange(S_WIN, device=dev).view(S_WIN, 1)       # (8, na)
+        lim = tr.length[run]
+        t_idx = c.view(1, na) + steps                                                # (8, na)
         ok = t_idx < lim.view(1, na)                                                 # S_local truncation, :61
-        t_ok, cols = t_idx[ok], active.view(1, na).expand(S_WIN, na)[ok]
-        traj[t_ok, cols] = xys[ok]
-        v = torch.sigmoid(vis_e[0]) if want_vis or advance is None else None
-        if want_vis:
-            vis[t_ok, cols] = v[ok]
+        rows, cols = (tr.row0[run].view(1, na) + t_idx)[ok], run.view(1, na).expand(S_WIN, na)[ok]
+        tr.traj[rows, cols] = xys[ok]
+        v = torch.sigmoid(vis_e[0]) if tr.vis is not None or advance is None else None
+        if tr.vis is not None:
+            tr.vis[rows, cols] = v[ok]
         si = pick_skip(v, thr) if advance is None else torch.full_like(c, int(advance))
         nxt = c + si
-        cur[active] = nxt
-        active = active[nxt < lim]
-        rounds += 1
-    return traj, vis, rounds
+        tr.cur[run] = nxt
+        tr.pos[run] = xys[si, torch.arange(na, device=dev)]
+        tr.done[run] = nxt >= lim
+        tr.rounds += 1
 
 
 @torch.no_grad()
@@ -120,10 +157,11 @@ def track_chain(model, rgbs: torch.Tensor, xy0: torch.Tensor, iters: int = 6, re
     N = xy0.shape[1]
     dev = rgbs.device
     fmaps = _encode_clip(model, rgbs)
-    traj, _, rounds = _run_rounds(model, fmaps, torch.zeros(N, dtype=torch.long, device=dev),
-                                  torch.full((N,), T, dtype=torch.long, device=dev), xy0[0], iters, advance)
-    out = traj.unsqueeze(0)
-    return (out, rounds) if return_rounds else out
+    tr = _Tracks(torch.zeros(N, dtype=torch.long, device=dev), torch.full((N,), T, dtype=torch.long, device=dev),
+                 xy0[0], T, want_vis=False)
+    _run_rounds(model, fmaps, tr, iters, advance)
+    out = tr.traj.unsqueeze(0)
+    return (out, tr.rounds) if return_rounds else out
 
 
 def _check_queries(rgbs: torch.Tensor, queries: torch.Tensor) -> torch.Tensor:
@@ -172,8 +210,9 @@ def track_queries(model, rgbs: torch.Tensor, queries: torch.Tensor, iters: int =
     back = (t > 0).nonzero().flatten()                                               # queries with a backward track
     tb = t[back]
     fmaps = _encode_clip(model, rgbs)
-    traj, vis, rounds = _run_rounds(model, fmaps, torch.cat([t, ~tb]), torch.cat([T - t, tb + 1]),
-                                    torch.cat([xy, xy[back]]), iters, want_vis=True)
+    tr = _Tracks(torch.cat([t, ~tb]), torch.cat([T - t, tb + 1]), torch.cat([xy, xy[back]]), T, want_vis=True)
+    _run_rounds(model, fmaps, tr, iters)
+    traj, vis, rounds = tr.traj, tr.vis, tr.rounds
     # frame f of query n: step f - t of its forward track when f >= t, else step t - f of its backward track
     f = torch.arange(T, device=dev).view(T, 1)
     bcol = torch.zeros(N, dtype=torch.long, device=dev)
