@@ -64,6 +64,10 @@ int pips_pyramid_build_nhwc(const float* fmaps_nhwc, int frames, int H, int W,
 int pips_init_gather(const float* lvl0_f32, int B, int S, int N, int H, int W, const float* coords,
                      const int* frame_base /* NULL or [B*N] */, int frames_per_batch,
                      float* ffeat /* (B*N,128) */, float* ffeats /* (B*N,S,128) */, void* stream);
+/* pips_init_gather with a per-track clip table (several videos in one pyramid), decoded as in pips_corr_gather_clips. */
+int pips_init_gather_clips(const float* lvl0_f32, int B, int S, int N, int H, int W, const float* coords,
+                           const int* frame_base /* [B*N] */, int frames_per_batch, const int* clip /* NULL or [B*N][2] */,
+                           float* ffeat /* (B*N,128) */, float* ffeats /* (B*N,S,128) */, void* stream);
 
 /* nets/pips.py:502,:513 (CorrBlock.corr + .sample) fused with the layout glue :517-522 and
  * utils/misc.py:44-69 (get_3d_embedding): writes the 519-wide mixer input row
@@ -77,6 +81,18 @@ int pips_corr_gather(const void* const* lvl, int feat_dtype, int B, int S, int N
                      const float* coords, const float* ffeats, const float* times /* [S] */,
                      const int* frame_base /* NULL or [B*N] */, int frames_per_batch,
                      void* x_hi, void* x_lo, float* x_f32, int ldx, void* stream);
+/* pips_corr_gather with a per-track clip table: several clips of different lengths concatenated in one pyramid of
+ * B * frames_per_batch frames (frames_per_batch still sizes the tensor maps).  clip[b*N+n] = {first, count} (int32
+ * pairs): the first pyramid frame of track (b,n)'s clip and its number of frames, count >= 1 and first + count <=
+ * B * frames_per_batch (not checked: the kernels trust the table).  Step s then reads pyramid frame
+ *   first + min(base + s, count-1)             for base >= 0 (forward: the clip's last frame is replicated)
+ *   first + max(min(~base, count-1) - s, 0)    for base <  0 (backward: clamped at the clip's frame 0)
+ * with base = frame_base[b*N+n] counted inside the clip, so a window never reads another clip's frames.  A clip table
+ * requires frame_base (an error otherwise); clip == NULL is pips_corr_gather. */
+int pips_corr_gather_clips(const void* const* lvl, int feat_dtype, int B, int S, int N, int H, int W,
+                           const float* coords, const float* ffeats, const float* times /* [S] */,
+                           const int* frame_base /* [B*N] */, int frames_per_batch, const int* clip /* NULL or [B*N][2] */,
+                           void* x_hi, void* x_lo, float* x_f32, int ldx, void* stream);
 
 /* Backward of pips_corr_gather's correlation columns (x[:, 128:324]) for training (csrc/corr_grad.cu), with respect to
  * the ffeats and the 4 fp32 levels; the coordinates get no gradient.  S == 8, fp32, no frame_base.  dcorr is the
@@ -379,6 +395,10 @@ int pips_mixer_forward(const pips_weights* w, const pips_workspace* ws, int seqs
 /* one refinement iteration; out_px receives coords*stride (B,S,N,2) */
 int pips_refine_iter(const pips_problem* p, const pips_weights* w, const pips_workspace* ws,
                      float* out_px, void* stream);
+/* pips_refine_iter whose correlation reads each track's window inside its own clip: pips_corr_gather_clips with
+ * p->frame_base (required when clip is non-NULL) and clip [B*N][2]; the mixer and the update are unchanged. */
+int pips_refine_iter_clips(const pips_problem* p, const int* clip /* NULL or [B*N][2] */, const pips_weights* w,
+                           const pips_workspace* ws, float* out_px, void* stream);
 
 #ifdef __cplusplus
 }

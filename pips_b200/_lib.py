@@ -70,6 +70,8 @@ _SIGNATURES = {
     "pips_pyramid_build_nhwc": (_i, [_p, _i, _i, _i, C.POINTER(_p), C.POINTER(_p), _p]),
     "pips_init_gather": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _p, _p]),
     "pips_corr_gather": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _i, _p, _p, _p, _i, _p]),
+    "pips_init_gather_clips": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _p, _p, _p]),
+    "pips_corr_gather_clips": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _i, _p, _p, _p, _p, _i, _p]),
     "pips_corr_grad_feats": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _p, _p, _i, _p, _p]),
     "pips_corr_grad_levels": (_i, [_i, _i, _i, _i, _i, _p, _p, _p, _i, C.POINTER(_p), _p]),
     "pips_peer_alloc": (_i, [C.c_size_t, C.POINTER(_p), C.c_char_p]),
@@ -124,6 +126,7 @@ _SIGNATURES = {
     "pips_resize_grad": (_i, [_p, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p]),
     "pips_mixer_forward": (_i, [C.POINTER(Weights), C.POINTER(Workspace), _i, _i, _p]),
     "pips_refine_iter": (_i, [C.POINTER(Problem), C.POINTER(Weights), C.POINTER(Workspace), _p, _p]),
+    "pips_refine_iter_clips": (_i, [C.POINTER(Problem), _p, C.POINTER(Weights), C.POINTER(Workspace), _p, _p]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

@@ -14,7 +14,8 @@ the per-particle loop up to fp32 noise.
 ``track_chain`` tracks points given at frame 0, forward in time, as the reference does.  ``track_queries`` takes
 (t, x, y) queries at any frame and tracks each both ways: the reference chain on the clip from frame t on, and the
 same chain on the time-reversed clip from frame t back to frame 0.  A backward track reads its windows through a
-negative frame offset (``~t``), so both directions share the pyramid and the rounds.
+negative frame offset (``~t``), so both directions share the pyramid and the rounds.  ``track_queries_batch`` does the
+same for many clips at once: their frames share one pyramid, and every track also carries its clip's place in it.
 """
 from __future__ import annotations
 
@@ -64,13 +65,15 @@ class _Tracks:
     video: t for a forward track from frame t, ~t for a backward one (see window_frame in csrc/corr_common.cuh).  A
     window that starts c frames further on is base0[k] + c in both directions (~(t - c) == ~t + c).  Step s of the
     window at cursor c writes row row0[k] + c + s of traj (rows, n, 2) and vis (rows, n); vis holds sigmoid(vis_e) of
-    the window that last wrote the row, and is None unless ``want_vis``."""
+    the window that last wrote the row, and is None unless ``want_vis``.  ``clip`` (n, 2) int32 (optional): track k's
+    clip {first, count} among the held frames when they hold several videos; base0[k] then counts inside that clip
+    (clip_window_frame in csrc/corr_common.cuh)."""
 
     def __init__(self, base0: torch.Tensor, length: torch.Tensor, xy: torch.Tensor, rows: int, want_vis: bool,
-                 fill: float = 0.0):
+                 fill: float = 0.0, clip: Optional[torch.Tensor] = None):
         n = base0.numel()
         dev = base0.device
-        self.base0, self.length = base0, length
+        self.base0, self.length, self.clip = base0, length, clip
         self.row0 = torch.zeros(n, dtype=torch.long, device=dev)
         self.pos = xy.float().clone()                                                # start of each track's next window
         self.cur = torch.zeros(n, dtype=torch.long, device=dev)
@@ -89,7 +92,8 @@ def _run_rounds(model, fmaps: torch.Tensor, tr: _Tracks, iters: int, advance: Op
     through its frame_base rebased to the held frames; rounds repeat until no track is runnable.  A track is runnable
     while it is inside its clip and, unless the video has ``ended``, its whole window has arrived.  A window past the
     last held frame replicates that frame, which is the end-of-clip rule once the video has ended.  A track's first
-    window gathers its own feature; later windows carry it (outs[3], chain_demo.py:57)."""
+    window gathers its own feature; later windows carry it (outs[3], chain_demo.py:57).  With a per-track clip
+    (tr.clip) the refinement calls pass the runnable tracks' rows of it as ``clip``; without one they pass no clip."""
     F = fmaps.shape[1]
     dev = fmaps.device
     eng = model.engine
@@ -109,17 +113,20 @@ def _run_rounds(model, fmaps: torch.Tensor, tr: _Tracks, iters: int, advance: Op
         fb = (tr.base0[run] + c - f0).view(1, na).to(torch.int32)
         coords = (tr.pos[run] / stride).view(1, 1, na, 2).repeat(1, S_WIN, 1, 1)    # zero-velocity init, :453
         new = ~tr.started[run]
+        cl = None if tr.clip is None else tr.clip[run].view(1, na, 2)
         fi = None
         if not bool(new.all()):
             if bool(new.any()):
                 # tracks starting beside carried ones: their first-window features alone (initial gather, no iteration)
+                kw = {} if cl is None else {"clip": cl[:, new]}
                 _, _, f_new = eng.refine(model, fmaps, coords[:, :, new], None, 0, stride, frame_base=fb[:, new],
-                                         reuse_pyramid=built)
+                                         reuse_pyramid=built, **kw)
                 built = True
                 tr.feat[run[new]] = f_new[0]
                 tr.started[run[new]] = True
             fi = tr.feat[run].unsqueeze(0)
-        preds, vis_e, ffeat = eng.refine(model, fmaps, coords, fi, iters, stride, frame_base=fb, reuse_pyramid=built)
+        kw = {} if cl is None else {"clip": cl}
+        preds, vis_e, ffeat = eng.refine(model, fmaps, coords, fi, iters, stride, frame_base=fb, reuse_pyramid=built, **kw)
         built = True
         if fi is None:
             if tr.feat is None:
@@ -204,7 +211,6 @@ def track_queries(model, rgbs: torch.Tensor, queries: torch.Tensor, iters: int =
     together, one refinement call per round, each reading its own window of the resident pyramid."""
     t = _check_queries(rgbs, queries)
     T = rgbs.shape[1]
-    N = t.numel()
     dev = rgbs.device
     xy = queries[0, :, 1:3].to(device=dev, dtype=torch.float32)
     back = (t > 0).nonzero().flatten()                                               # queries with a backward track
@@ -212,13 +218,113 @@ def track_queries(model, rgbs: torch.Tensor, queries: torch.Tensor, iters: int =
     fmaps = _encode_clip(model, rgbs)
     tr = _Tracks(torch.cat([t, ~tb]), torch.cat([T - t, tb + 1]), torch.cat([xy, xy[back]]), T, want_vis=True)
     _run_rounds(model, fmaps, tr, iters)
-    traj, vis, rounds = tr.traj, tr.vis, tr.rounds
-    # frame f of query n: step f - t of its forward track when f >= t, else step t - f of its backward track
+    out = _merge_directions(tr, t, back, T, 0)
+    return out + (tr.rounds,) if return_rounds else out
+
+
+def _merge_directions(tr: _Tracks, t: torch.Tensor, back: torch.Tensor, T: int, c0: int):
+    """trajs (1, T, N, 2) and vis (1, T, N) of N queries at frames t (N,) whose tracks are the columns c0 .. of tr:
+    the N forward tracks, then the backward tracks of the queries ``back`` (those with t > 0).  Frame f of query n is
+    step f - t of its forward track when f >= t, else step t - f of its backward track."""
+    N = t.numel()
+    dev = tr.traj.device
     f = torch.arange(T, device=dev).view(T, 1)
     bcol = torch.zeros(N, dtype=torch.long, device=dev)
-    bcol[back] = N + torch.arange(back.numel(), device=dev)
+    bcol[back] = c0 + N + torch.arange(back.numel(), device=dev)
     fwd = f >= t.view(1, N)
     step = torch.where(fwd, f - t.view(1, N), t.view(1, N) - f)                     # (T, N)
-    col = torch.where(fwd, torch.arange(N, device=dev).view(1, N), bcol.view(1, N))
-    out = (traj[step, col].unsqueeze(0), vis[step, col].unsqueeze(0))
-    return out + (rounds,) if return_rounds else out
+    col = torch.where(fwd, c0 + torch.arange(N, device=dev).view(1, N), bcol.view(1, N))
+    return tr.traj[step, col].unsqueeze(0), tr.vis[step, col].unsqueeze(0)
+
+
+def _batch_clip(rgbs, i: int) -> torch.Tensor:
+    """Clip i of track_queries_batch, (T, 3, H, W) or (1, T, 3, H, W) -> a (T, 3, H, W) view with T >= 1."""
+    if not isinstance(rgbs, torch.Tensor) or rgbs.dim() not in (4, 5) or rgbs.shape[-3] != 3 \
+            or (rgbs.dim() == 5 and rgbs.shape[0] != 1):
+        raise ValueError(f"clips[{i}] must be (T, 3, H, W) or (1, T, 3, H, W), got {tuple(getattr(rgbs, 'shape', ()))}")
+    v = rgbs if rgbs.dim() == 4 else rgbs[0]
+    if v.shape[0] < 1:
+        raise ValueError(f"clips[{i}] holds no frames")
+    return v
+
+
+def _encode_batch(model, clips, chunk: int = 32) -> torch.Tensor:
+    """The feature maps (1, F, 128, H8, W8) of all frames of ``clips`` ((T_i, 3, H, W) each) back to back, F = sum T_i.
+    Frames are encoded once, ``chunk`` at a time across clip boundaries, so the encoder sees one full-chunk shape and one
+    tail; each chunk goes to the model's device only when it is encoded.  The maps are written into one channels-last
+    buffer as they come, so the batch's maps are never held twice."""
+    dev = next(iter(model.parameters())).device
+    ends = torch.tensor([c.shape[0] for c in clips]).cumsum(0).tolist()
+    F = ends[-1]
+    buf = None
+    for t0 in range(0, F, chunk):
+        t1 = min(F, t0 + chunk)
+        parts = []
+        for c, e in zip(clips, ends):
+            s = e - c.shape[0]                                                   # the clip holds frames s .. e-1
+            if s < t1 and e > t0:
+                parts.append(c[max(t0 - s, 0):min(t1, e) - s].to(dev))
+        f = model.encode(torch.cat(parts).unsqueeze(0))[0]                          # (k, 128, H8, W8)
+        if buf is None:
+            buf = torch.empty(F, f.shape[2], f.shape[3], f.shape[1], dtype=f.dtype, device=dev)
+        buf[t0:t1].copy_(f.permute(0, 2, 3, 1))
+    return buf.permute(0, 3, 1, 2).unsqueeze(0)
+
+
+@torch.no_grad()
+def track_queries_batch(model, clips, queries, iters: int = 6, return_rounds: bool = False):
+    """``track_queries`` over many videos in one pass: every clip's tracks advance in the same rounds.
+
+    ``clips`` is a sequence of videos, each (T_i, 3, H, W) or (1, T_i, 3, H, W), float 0..255 or uint8, on the host or
+    the model's device (converted as ``Pips.encode`` converts them).  All share H x W; T_i may differ, T_i == 1 included.
+    ``queries`` holds one (N_i, 3) or (1, N_i, 3) tensor of (t, x, y) per clip, t integral in 0..T_i-1.  Returns a list
+    with one (trajs (1, T_i, N_i, 2), vis (1, T_i, N_i)) pair per clip -- the same bits as
+    ``track_queries(model, clips[i][None], queries[i][None])`` -- and the number of rounds when ``return_rounds``.
+
+    All frames are encoded once, in 32-frame chunks that run across clip boundaries, into one pyramid.  Every track
+    reads its windows inside its own clip through a per-track clip table (pips_corr_gather_clips), so each round is one
+    refinement call over the tracks of all clips, and the batch takes as many rounds as its longest clip's chain.  The
+    device holds the feature maps and the pyramid of every frame of the batch, about 1.2 MiB per 256x256 frame at
+    stride 8 with fp32 features: the caller bounds the batch."""
+    shard = getattr(model, "_shard", None)
+    if shard is not None and shard[1] > 1:
+        raise RuntimeError("pips_b200.chain: chained tracking does not cover particle-sharded models")
+    if len(clips) != len(queries):
+        raise ValueError(f"{len(clips)} clips but {len(queries)} query sets: one query set per clip")
+    if len(clips) == 0:
+        raise ValueError("empty batch: track_queries_batch needs at least one clip")
+    views = [_batch_clip(c, i) for i, c in enumerate(clips)]
+    hw = tuple(views[0].shape[-2:])
+    for i, v in enumerate(views):
+        if tuple(v.shape[-2:]) != hw:
+            raise ValueError(f"clips[{i}] frames are {tuple(v.shape[-2:])}, clips[0]'s are {hw}: one batch, one size")
+    dev = next(iter(model.parameters())).device
+    ts = []                                                                          # query frames per clip, on dev
+    for i, (v, q) in enumerate(zip(views, queries)):
+        if isinstance(q, torch.Tensor) and q.dim() == 2:
+            q = q.unsqueeze(0)
+        try:
+            ts.append(_check_queries(v.unsqueeze(0), q).to(dev))
+        except ValueError as e:
+            raise ValueError(f"queries[{i}]: {e}") from None
+    fmaps = _encode_batch(model, views)
+    base0, length, xy, clip, cols = [], [], [], [], []
+    first, c0 = 0, 0
+    for v, q, t in zip(views, queries, ts):
+        T, N = v.shape[0], t.numel()
+        qxy = q.reshape(-1, 3)[:, 1:3].to(device=dev, dtype=torch.float32)
+        back = (t > 0).nonzero().flatten()                                           # queries with a backward track
+        tb = t[back]
+        base0 += [t, ~tb]
+        length += [T - t, tb + 1]
+        xy += [qxy, qxy[back]]
+        n = N + back.numel()
+        clip.append(torch.tensor([first, T], dtype=torch.int32, device=dev).expand(n, 2))
+        cols.append((c0, back))
+        first += T
+        c0 += n
+    tr = _Tracks(torch.cat(base0), torch.cat(length), torch.cat(xy), max(v.shape[0] for v in views), want_vis=True,
+                 clip=torch.cat(clip).contiguous())
+    _run_rounds(model, fmaps, tr, iters)
+    outs = [_merge_directions(tr, t, back, v.shape[0], c0) for v, t, (c0, back) in zip(views, ts, cols)]
+    return (outs, tr.rounds) if return_rounds else outs

@@ -148,19 +148,44 @@ extern "C" int pips_mixer_forward(const pips_weights* w, const pips_workspace* w
     return rc;
 }
 
-extern "C" int pips_refine_iter(const pips_problem* p, const pips_weights* w, const pips_workspace* ws,
-                                float* out_px, void* stream) {
-    if (!p || !w || !ws || !out_px) return fail("pips_refine_iter: null argument");
-    if (p->S != PIPS_S) return fail("pips_refine_iter: S must be 8");
+static int refine_iter_entry(const char* who, const pips_problem* p, const int* clip, const pips_weights* w,
+                             const pips_workspace* ws, float* out_px, void* stream) {
+    if (!p || !w || !ws || !out_px) {
+        snprintf(g_err, sizeof(g_err), "%s: null argument", who);
+        return 1;
+    }
+    if (p->S != PIPS_S) {
+        snprintf(g_err, sizeof(g_err), "%s: S must be 8", who);
+        return 1;
+    }
+    if (clip && !p->frame_base) {
+        snprintf(g_err, sizeof(g_err), "%s: a clip table needs frame_base", who);
+        return 1;
+    }
     const int seqs = p->B * p->N;
     const bool f32 = p->precision == PIPS_PREC_F32;
     const bool x3 = p->precision == PIPS_PREC_BF16X3;
-    int rc = pips_corr_gather(p->lvl, p->feat_dtype, p->B, p->S, p->N, p->H, p->W, p->coords, p->ffeats, p->times, p->frame_base, p->frames_per_batch,
-                              f32 ? nullptr : ws->x0_hi, x3 ? ws->x0_lo : nullptr, f32 ? ws->x0_f32 : nullptr,
-                              PIPS_KITCHEN_PAD, stream);
+    int rc = clip ? pips_corr_gather_clips(p->lvl, p->feat_dtype, p->B, p->S, p->N, p->H, p->W, p->coords, p->ffeats, p->times,
+                                           p->frame_base, p->frames_per_batch, clip,
+                                           f32 ? nullptr : ws->x0_hi, x3 ? ws->x0_lo : nullptr, f32 ? ws->x0_f32 : nullptr,
+                                           PIPS_KITCHEN_PAD, stream)
+                  : pips_corr_gather(p->lvl, p->feat_dtype, p->B, p->S, p->N, p->H, p->W, p->coords, p->ffeats, p->times,
+                                     p->frame_base, p->frames_per_batch,
+                                     f32 ? nullptr : ws->x0_hi, x3 ? ws->x0_lo : nullptr, f32 ? ws->x0_f32 : nullptr,
+                                     PIPS_KITCHEN_PAD, stream);
     if (rc) return rc;
     rc = pips_mixer_forward(w, ws, seqs, p->precision, stream);
     if (rc) return rc;
     return pips_update_peer(ws->delta, p->coords, p->coords0, p->ffeats, w->gn_w, w->gn_b, w->upd_w, w->upd_b, out_px,
                             p->stride, p->B, p->S, p->N, &p->peer, stream);
+}
+
+extern "C" int pips_refine_iter(const pips_problem* p, const pips_weights* w, const pips_workspace* ws,
+                                float* out_px, void* stream) {
+    return refine_iter_entry("pips_refine_iter", p, nullptr, w, ws, out_px, stream);
+}
+
+extern "C" int pips_refine_iter_clips(const pips_problem* p, const int* clip, const pips_weights* w,
+                                      const pips_workspace* ws, float* out_px, void* stream) {
+    return refine_iter_entry("pips_refine_iter_clips", p, clip, w, ws, out_px, stream);
 }

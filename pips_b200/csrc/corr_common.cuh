@@ -24,6 +24,7 @@ struct CgArgs {
     __nv_bfloat16* x_lo;
     float* x_f32;
     int ldx;
+    const int* clip;         // optional [B*N][2] {first, count}: each track's clip in the pyramid (clip_window_frame)
 };
 
 // Frame index, inside its clip of T frames, of step s of a chained track's window (pips_init_gather reads step 0,
@@ -34,6 +35,15 @@ struct CgArgs {
 // frame a window starts at.
 __device__ __forceinline__ int window_frame(int base, int s, int T) {
     return base >= 0 ? min(base + s, T - 1) : max(min(~base, T - 1) - s, 0);
+}
+
+// Pyramid frame of step s of track seq when every track carries its own clip (several videos in one pyramid):
+// clip[seq] = {first, count} is the clip's first pyramid frame and its number of frames, and base = frame_base[seq] is
+// decoded inside the clip by window_frame.  A window therefore replicates the clip's last frame going forward and
+// clamps at its frame 0 going backward, and never reads another clip's frames.
+__device__ __forceinline__ int clip_window_frame(const int* clip, int seq, int base, int s) {
+    const int2 c = reinterpret_cast<const int2*>(clip)[seq];
+    return c.x + window_frame(base, s, c.y);
 }
 
 struct UnitInfo {
@@ -48,6 +58,8 @@ struct UnitInfo {
 // computes the box origin of ONE pyramid level (lane & 3), so that issuing a TMA box later costs two shuffles instead
 // of a clamp / floor / convert chain executed by lane 0 alone while 31 lanes wait.  Coordinates are clamped in float
 // so that diverged or non-finite tracks cannot overflow the int conversion (beyond +-8 px of the map all taps are zero).
+// kClips: the frame comes from the per-track clip table (a.clip and a.frame_base both set).
+template <bool kClips = false>
 __device__ __forceinline__ UnitInfo load_unit(const CgArgs& a, int u, int total) {
     UnitInfo ui;
     ui.valid = u < total;
@@ -58,7 +70,8 @@ __device__ __forceinline__ UnitInfo load_unit(const CgArgs& a, int u, int total)
         ui.b = seq / a.N; ui.n = seq - ui.b * a.N;
         const float2 c = *reinterpret_cast<const float2*>(a.coords + ((static_cast<size_t>(ui.b) * 8 + ui.s) * a.N + ui.n) * 2);
         ui.cx = c.x; ui.cy = c.y;
-        ui.frame = a.frame_base ? ui.b * a.T + window_frame(a.frame_base[seq], ui.s, a.T) : ui.b * 8 + ui.s;
+        if (kClips) ui.frame = clip_window_frame(a.clip, seq, a.frame_base[seq], ui.s);
+        else ui.frame = a.frame_base ? ui.b * a.T + window_frame(a.frame_base[seq], ui.s, a.T) : ui.b * 8 + ui.s;
         const int level = threadIdx.x & 3;
         const float sc = 1.0f / static_cast<float>(1 << level);        // coords / 2**i  (nets/pips.py:373), exact
         const float cxl = fminf(fmaxf(c.x * sc, -8.0f), static_cast<float>(a.W[level]) + 8.0f);

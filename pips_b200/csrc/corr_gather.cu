@@ -21,6 +21,8 @@
 //
 // Algorithmic bytes per unit (SURVEY.md 8d): 4 levels x 64 px x 128 ch x e_f  +  128 x 4 (query)
 // +  output row.
+#include <cstdio>
+
 #include "corr_common.cuh"
 #include "ptx.cuh"
 
@@ -51,7 +53,8 @@ __device__ __forceinline__ float4 ld_chan4(const __nv_bfloat16* p) {
     return r;
 }
 
-template <typename T>
+// kClips: each track reads its window inside its own clip of the pyramid (CgArgs::clip, clip_window_frame).
+template <typename T, bool kClips>
 __global__ void __launch_bounds__(CG_WARPS * 32)
 corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
     using Cfg = CgCfg<T>;
@@ -95,8 +98,8 @@ corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
     };
 
     pdl_wait();                                     // coords / ffeats / pyramid come from earlier kernels of the chain
-    UnitInfo cur = load_unit(a, u, total);
-    UnitInfo nxt = load_unit(a, u + nwarps, total);
+    UnitInfo cur = load_unit<kClips>(a, u, total);
+    UnitInfo nxt = load_unit<kClips>(a, u + nwarps, total);
     float4 q = *reinterpret_cast<const float4*>(a.ffeats + static_cast<size_t>(u) * 128 + lane * 4);
     issue(cur, 0, 0, 0);
     issue(cur, 0, 1, 1);
@@ -107,7 +110,7 @@ corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
         // prefetch the next unit's query while this one is processed
         float4 nq = make_float4(0.f, 0.f, 0.f, 0.f);
         if (nxt.valid) nq = *reinterpret_cast<const float4*>(a.ffeats + static_cast<size_t>(u + nwarps) * 128 + lane * 4);
-        const UnitInfo nxt2 = load_unit(a, u + 2 * nwarps, total);
+        const UnitInfo nxt2 = load_unit<kClips>(a, u + 2 * nwarps, total);
 
 #pragma unroll 1
         for (int level = 0; level < PIPS_LEVELS; ++level) {
@@ -201,7 +204,7 @@ corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
     }
 }
 
-template <typename T>
+template <typename T, bool kClips>
 static int launch_corr_gather(const void* const* lvl, CUtensorMapDataType dt, const CgArgs& args, int frames, cudaStream_t st) {
     CgMaps maps;
     if (encode_level_maps(maps, lvl, dt, sizeof(T), args.H, args.W, frames, "pips_corr_gather: cuTensorMapEncodeTiled failed"))
@@ -209,7 +212,7 @@ static int launch_corr_gather(const void* const* lvl, CUtensorMapDataType dt, co
     using Cfg = CgCfg<T>;
     static bool attr[kMaxDevices] = {};
     {
-        cudaError_t e = ensure_dyn_smem(corr_gather_kernel<T>, attr, static_cast<int>(Cfg::kSmemBytes));
+        cudaError_t e = ensure_dyn_smem(corr_gather_kernel<T, kClips>, attr, static_cast<int>(Cfg::kSmemBytes));
         if (e != cudaSuccess) return fail_cuda("pips_corr_gather: smem attribute", e);
     }
     const long long units = static_cast<long long>(args.B) * args.S * args.N;
@@ -218,7 +221,7 @@ static int launch_corr_gather(const void* const* lvl, CUtensorMapDataType dt, co
     long long grid = (units + CG_WARPS - 1) / CG_WARPS;
     const long long cap = static_cast<long long>(sm_count()) * ctas_per_sm;
     if (grid > cap) grid = cap;
-    cudaError_t e = launch_pdl(corr_gather_kernel<T>, dim3(static_cast<unsigned>(grid)), dim3(CG_WARPS * 32), Cfg::kSmemBytes, st, maps, args);
+    cudaError_t e = launch_pdl(corr_gather_kernel<T, kClips>, dim3(static_cast<unsigned>(grid)), dim3(CG_WARPS * 32), Cfg::kSmemBytes, st, maps, args);
     if (e == cudaSuccess) e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail_cuda("pips_corr_gather: launch", e);
 }
@@ -227,29 +230,57 @@ static int launch_corr_gather(const void* const* lvl, CUtensorMapDataType dt, co
 
 using namespace pips;
 
-extern "C" int pips_corr_gather(const void* const* lvl, int feat_dtype, int B, int S, int N, int H, int W, const float* coords,
-                                const float* ffeats, const float* times, const int* frame_base, int frames_per_batch,
-                                void* x_hi, void* x_lo, float* x_f32, int ldx, void* stream) {
-    if (!lvl || !coords || !ffeats || !times) return fail("pips_corr_gather: null pointer");
-    if (S != PIPS_S) return fail("pips_corr_gather: S must be 8");
-    if (B <= 0 || N <= 0) return fail("pips_corr_gather: empty problem");
-    if (H < 8 || W < 8) return fail("pips_corr_gather: level-0 map must be at least 8x8");
-    if (!x_hi && !x_f32) return fail("pips_corr_gather: no output buffer");
-    if (x_lo && !x_hi) return fail("pips_corr_gather: x_lo without x_hi");
-    if (ldx < PIPS_KITCHEN_PAD || (ldx % 8)) return fail("pips_corr_gather: ldx must be >= 576 and a multiple of 8");
+// pips_corr_gather and pips_corr_gather_clips: `who` names the entry point in error messages
+static int corr_gather_entry(const char* who, const void* const* lvl, int feat_dtype, int B, int S, int N, int H, int W,
+                             const float* coords, const float* ffeats, const float* times, const int* frame_base,
+                             int frames_per_batch, const int* clip, void* x_hi, void* x_lo, float* x_f32, int ldx,
+                             void* stream) {
+    char msg[160];
+    auto err = [&](const char* what) {
+        snprintf(msg, sizeof(msg), "%s: %s", who, what);
+        return fail(msg);
+    };
+    if (!lvl || !coords || !ffeats || !times) return err("null pointer");
+    if (S != PIPS_S) return err("S must be 8");
+    if (B <= 0 || N <= 0) return err("empty problem");
+    if (H < 8 || W < 8) return err("level-0 map must be at least 8x8");
+    if (!x_hi && !x_f32) return err("no output buffer");
+    if (x_lo && !x_hi) return err("x_lo without x_hi");
+    if (ldx < PIPS_KITCHEN_PAD || (ldx % 8)) return err("ldx must be >= 576 and a multiple of 8");
     CgArgs a;
     a.B = B; a.S = S; a.N = N;
     int h = H, w = W;
     for (int l = 0; l < PIPS_LEVELS; ++l) {
-        if (!lvl[l]) return fail("pips_corr_gather: null level pointer");
+        if (!lvl[l]) return err("null level pointer");
         a.H[l] = h; a.W[l] = w; h /= 2; w /= 2;
     }
-    if (frame_base && frames_per_batch <= 0) return fail("pips_corr_gather: frame_base needs frames_per_batch > 0");
+    if (frame_base && frames_per_batch <= 0) return err("frame_base needs frames_per_batch > 0");
+    if (clip && !frame_base) return err("a clip table needs frame_base");
     a.coords = coords; a.ffeats = ffeats; a.times = times;
     a.frame_base = frame_base; a.T = frame_base ? frames_per_batch : S;
     a.x_hi = static_cast<__nv_bfloat16*>(x_hi); a.x_lo = static_cast<__nv_bfloat16*>(x_lo); a.x_f32 = x_f32; a.ldx = ldx;
+    a.clip = clip;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (feat_dtype == PIPS_FEAT_F32) return launch_corr_gather<float>(lvl, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a, B * a.T, st);
-    if (feat_dtype == PIPS_FEAT_BF16) return launch_corr_gather<__nv_bfloat16>(lvl, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, a, B * a.T, st);
-    return fail("pips_corr_gather: unknown feat_dtype");
+    if (feat_dtype == PIPS_FEAT_F32)
+        return clip ? launch_corr_gather<float, true>(lvl, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a, B * a.T, st)
+                    : launch_corr_gather<float, false>(lvl, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a, B * a.T, st);
+    if (feat_dtype == PIPS_FEAT_BF16)
+        return clip ? launch_corr_gather<__nv_bfloat16, true>(lvl, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, a, B * a.T, st)
+                    : launch_corr_gather<__nv_bfloat16, false>(lvl, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, a, B * a.T, st);
+    return err("unknown feat_dtype");
+}
+
+extern "C" int pips_corr_gather(const void* const* lvl, int feat_dtype, int B, int S, int N, int H, int W, const float* coords,
+                                const float* ffeats, const float* times, const int* frame_base, int frames_per_batch,
+                                void* x_hi, void* x_lo, float* x_f32, int ldx, void* stream) {
+    return corr_gather_entry("pips_corr_gather", lvl, feat_dtype, B, S, N, H, W, coords, ffeats, times, frame_base,
+                             frames_per_batch, nullptr, x_hi, x_lo, x_f32, ldx, stream);
+}
+
+extern "C" int pips_corr_gather_clips(const void* const* lvl, int feat_dtype, int B, int S, int N, int H, int W,
+                                      const float* coords, const float* ffeats, const float* times, const int* frame_base,
+                                      int frames_per_batch, const int* clip, void* x_hi, void* x_lo, float* x_f32, int ldx,
+                                      void* stream) {
+    return corr_gather_entry("pips_corr_gather_clips", lvl, feat_dtype, B, S, N, H, W, coords, ffeats, times, frame_base,
+                             frames_per_batch, clip, x_hi, x_lo, x_f32, ldx, stream);
 }

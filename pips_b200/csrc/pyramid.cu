@@ -1,7 +1,9 @@
 // Correlation pyramid and initial feature gather (run once per forward, upstream of the loop).
 //   pips_pyramid_build  nets/pips.py:346-352   NCHW fp32 fmaps -> 4 channels-last levels (fp32, + optional bf16 copy)
 //   pips_init_gather    utils/samp.py:5-78     bilinear sample of frame 0 at the queries, indices clamped
-#include "corr_common.cuh"   // window_frame: the chained-window decode pips_corr_gather uses
+#include <cstdio>
+
+#include "corr_common.cuh"   // window_frame / clip_window_frame: the chained-window decode pips_corr_gather uses
 
 namespace pips {
 
@@ -62,10 +64,12 @@ __global__ void f32_to_bf16_kernel(const float* __restrict__ in, __nv_bfloat16* 
     }
 }
 
-// one warp per (b, n): 4 clamped taps x 128 channels, unclamped weights, result broadcast to the S rows
+// one warp per (b, n): 4 clamped taps x 128 channels, unclamped weights, result broadcast to the S rows.
+// kClips: the window starts inside the track's own clip of the pyramid (clip_window_frame).
+template <bool kClips>
 __global__ void init_gather_kernel(const float* __restrict__ lvl0, int B, int S, int N, int H, int W,
                                    const float* __restrict__ coords, const int* __restrict__ frame_base, int T,
-                                   float* __restrict__ ffeat, float* __restrict__ ffeats) {
+                                   float* __restrict__ ffeat, float* __restrict__ ffeats, const int* __restrict__ clip) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= B * N) return;
     const int b = warp / N, n = warp % N;
@@ -80,7 +84,8 @@ __global__ void init_gather_kernel(const float* __restrict__ lvl0, int B, int S,
     const int y1 = static_cast<int>(fminf(fmaxf(y1f, 0.f), static_cast<float>(H - 1)));
     const float w00 = (x1f - x) * (y1f - y), w01 = (x - x0f) * (y1f - y);
     const float w10 = (x1f - x) * (y - y0f), w11 = (x - x0f) * (y - y0f);
-    const int frame = frame_base ? b * T + window_frame(frame_base[warp], 0, T) : b * S;  // first frame of the track's window
+    const int frame = kClips ? clip_window_frame(clip, warp, frame_base[warp], 0)           // first frame of the track's window
+                             : frame_base ? b * T + window_frame(frame_base[warp], 0, T) : b * S;
     const float* img = lvl0 + static_cast<size_t>(frame) * H * W * 128;
     const float4 a = *reinterpret_cast<const float4*>(img + (static_cast<size_t>(y0) * W + x0) * 128 + lane * 4);
     const float4 bq = *reinterpret_cast<const float4*>(img + (static_cast<size_t>(y0) * W + x1) * 128 + lane * 4);
@@ -151,12 +156,42 @@ extern "C" int pips_pyramid_build_nhwc(const float* fmaps_nhwc, int frames, int 
     return pyramid_common(fmaps_nhwc, true, frames, H, W, lvl_f32, lvl_bf16, stream);
 }
 
+static int init_gather_entry(const char* who, const float* lvl0_f32, int B, int S, int N, int H, int W, const float* coords,
+                             const int* frame_base, int frames_per_batch, const int* clip, float* ffeat, float* ffeats,
+                             void* stream) {
+    char msg[160];
+    if (!lvl0_f32 || !coords || !ffeat || !ffeats) {
+        snprintf(msg, sizeof(msg), "%s: null pointer", who);
+        return fail(msg);
+    }
+    if (B <= 0 || N <= 0 || S <= 0) {
+        snprintf(msg, sizeof(msg), "%s: empty problem", who);
+        return fail(msg);
+    }
+    if (clip && !frame_base) {
+        snprintf(msg, sizeof(msg), "%s: a clip table needs frame_base", who);
+        return fail(msg);
+    }
+    const int warps = B * N;
+    const dim3 grid((warps * 32 + 127) / 128), block(128);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (clip)
+        init_gather_kernel<true><<<grid, block, 0, st>>>(lvl0_f32, B, S, N, H, W, coords, frame_base, frames_per_batch, ffeat, ffeats, clip);
+    else
+        init_gather_kernel<false><<<grid, block, 0, st>>>(lvl0_f32, B, S, N, H, W, coords, frame_base, frames_per_batch, ffeat, ffeats, nullptr);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail_cuda(who, e);
+}
+
 extern "C" int pips_init_gather(const float* lvl0_f32, int B, int S, int N, int H, int W, const float* coords,
                                 const int* frame_base, int frames_per_batch, float* ffeat, float* ffeats, void* stream) {
-    if (!lvl0_f32 || !coords || !ffeat || !ffeats) return fail("pips_init_gather: null pointer");
-    if (B <= 0 || N <= 0 || S <= 0) return fail("pips_init_gather: empty problem");
-    const int warps = B * N;
-    init_gather_kernel<<<(warps * 32 + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(lvl0_f32, B, S, N, H, W, coords, frame_base, frames_per_batch, ffeat, ffeats);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail_cuda("pips_init_gather", e);
+    return init_gather_entry("pips_init_gather", lvl0_f32, B, S, N, H, W, coords, frame_base, frames_per_batch, nullptr,
+                             ffeat, ffeats, stream);
+}
+
+extern "C" int pips_init_gather_clips(const float* lvl0_f32, int B, int S, int N, int H, int W, const float* coords,
+                                      const int* frame_base, int frames_per_batch, const int* clip, float* ffeat,
+                                      float* ffeats, void* stream) {
+    return init_gather_entry("pips_init_gather_clips", lvl0_f32, B, S, N, H, W, coords, frame_base, frames_per_batch, clip,
+                             ffeat, ffeats, stream);
 }

@@ -306,11 +306,12 @@ class RefineEngine:
     # ------------------------------------------------------------------ the loop
     def _enqueue(self, lib, wc, pyr: Pyramid, ws: Workspace, fmaps2d, c, c0, ffeat, ffeats, feat_init, out, vis,
                  B, S, nc, H8, W8, iters, stride, on_iter=None, build_pyramid=True, frame_base=None, T=0,
-                 heat=None, peer=None, peer_n0=0, loss=None) -> int:
+                 heat=None, peer=None, peer_n0=0, loss=None, clip=None) -> int:
         """Enqueue every launch of one forward for ``nc`` particles on the current stream: pyramid, initial
         features, ``iters`` refinement iterations, visibility head.  Returns the number of kernels launched.
         ``loss`` (G_hi, G_lo, target (B,S,nc) int32, neg (iters, B*S*nc, n_split), pos (iters, B*S*nc)): also the
-        score-map loss terms of every iteration (pips_scoremap_loss); the basis G is built with the pyramid."""
+        score-map loss terms of every iteration (pips_scoremap_loss); the basis G is built with the pyramid.
+        ``clip`` (B*nc, 2) int32: per-track clip table, read by the ``_clips`` entry points."""
         st = self._stream()
         launches = 0
         if build_pyramid:
@@ -323,8 +324,12 @@ class RefineEngine:
                 launches += 1
         c0.copy_(c)
         if feat_init is None:
-            L.check(lib.pips_init_gather(L.ptr(pyr.f32[0]), B, S, nc, H8, W8, L.ptr(c), L.ptr(frame_base), T, L.ptr(ffeat),
-                                         L.ptr(ffeats), st), "pips_init_gather")
+            if clip is None:
+                L.check(lib.pips_init_gather(L.ptr(pyr.f32[0]), B, S, nc, H8, W8, L.ptr(c), L.ptr(frame_base), T,
+                                             L.ptr(ffeat), L.ptr(ffeats), st), "pips_init_gather")
+            else:
+                L.check(lib.pips_init_gather_clips(L.ptr(pyr.f32[0]), B, S, nc, H8, W8, L.ptr(c), L.ptr(frame_base), T,
+                                                   L.ptr(clip), L.ptr(ffeat), L.ptr(ffeats), st), "pips_init_gather_clips")
             launches += 1
         else:
             ffeat.copy_(feat_init.reshape(B * nc, LATENT))
@@ -361,7 +366,12 @@ class RefineEngine:
                                                L.ptr(neg[it]), L.ptr(pos[it]), st), "pips_scoremap_loss")
                 launches += 1
             with nvtx_range(f"pips/iter{it}"):
-                L.check(lib.pips_refine_iter(C.byref(prob), C.byref(wc), C.byref(ws.c), L.ptr(out[it]), st), "pips_refine_iter")
+                if clip is None:
+                    L.check(lib.pips_refine_iter(C.byref(prob), C.byref(wc), C.byref(ws.c), L.ptr(out[it]), st),
+                            "pips_refine_iter")
+                else:
+                    L.check(lib.pips_refine_iter_clips(C.byref(prob), L.ptr(clip), C.byref(wc), C.byref(ws.c),
+                                                       L.ptr(out[it]), st), "pips_refine_iter_clips")
             launches += 1 + (1 + 3 * L.DEPTH + 2) + 1
             if on_iter is not None:
                 on_iter(it, out[it])
@@ -373,7 +383,8 @@ class RefineEngine:
                iters: int, stride: float, on_iter=None, frame_base: Optional[torch.Tensor] = None,
                reuse_pyramid: bool = False, heat_sel: Optional[torch.Tensor] = None,
                heat_out: Optional[torch.Tensor] = None, peer=None, loss_target: Optional[torch.Tensor] = None,
-               loss_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+               loss_out: Optional[torch.Tensor] = None,
+               clip: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """fmaps (B,S,128,H8,W8) fp32, coords (B,S,N,2) fp32 in feature-map pixels.
         Returns preds (iters,B,S,N,2) in input pixels, vis_e (B,S,N) logits, ffeat (B,N,128).
         ``on_iter(it, coords_px)`` (optional) is called once per iteration when the particles fit one
@@ -387,7 +398,12 @@ class RefineEngine:
         kernel also stores every iteration's prediction into all ranks' slabs (the caller runs the barriers).
         ``loss_target`` (B,S,N) int32 (y*W8 + x of the ground-truth pixel, -1 for a row the loss ignores) + ``loss_out``
         (0-dim fp32): also compute the score-map loss of nets/pips.py:58-90 over all iterations into ``loss_out``,
-        without materialising the score maps (pips_scoremap_loss)."""
+        without materialising the score maps (pips_scoremap_loss).
+        ``clip`` (B,N,2) int32 (optional, with ``frame_base``): several videos in one pyramid.  clip[b,n] = (first, count)
+        is the first frame of track (b,n)'s clip among the B*T frames of fmaps and its number of frames; the track's
+        frame_base then counts inside that clip, and its windows replicate the clip's last frame going forward and clamp
+        at the clip's frame 0 going backward (pips_corr_gather_clips).  The table is checked here, because the kernels
+        trust it."""
         lib = L.load()
         B, T, Cc, H8, W8 = fmaps.shape
         S = coords.shape[1]
@@ -396,6 +412,8 @@ class RefineEngine:
         if frame_base is not None:
             frame_base = frame_base.to(device=fmaps.device, dtype=torch.int32).contiguous()
         N = coords.shape[2]
+        if clip is not None:
+            clip = self._check_clip(clip, frame_base, B, N, B * T, fmaps.device)
         dev = fmaps.device
         w = self.weights(module)
         fmaps2d = fmaps.reshape(B * T, Cc, H8, W8)                  # a view for both NCHW and channels-last inputs
@@ -454,6 +472,7 @@ class RefineEngine:
             out = preds if whole else torch.empty(iters, B, S, nc, 2, dtype=torch.float32, device=dev)
             v = vis if whole else torch.empty(B, S, nc, dtype=torch.float32, device=dev)
             fb = None if frame_base is None else (frame_base if whole else frame_base[:, n0:n1].contiguous())
+            cl = None if clip is None else (clip if whole else clip[:, n0:n1].contiguous())
             heat = None
             if heat_sel is not None:
                 inside = ((heat_sel >= n0) & (heat_sel < n1)).nonzero().flatten()
@@ -468,7 +487,7 @@ class RefineEngine:
             self.launches += self._enqueue(lib, w.c, pyr, ws, fmaps2d, c, c0, ffeat, ffeats, fi, out, v, B, S, nc, H8, W8,
                                            iters, stride, on_iter if whole else None,
                                            build_pyramid=(n0 == 0 and not reuse_pyramid), frame_base=fb, T=T, heat=heat,
-                                           peer=peer, peer_n0=n0, loss=loss)
+                                           peer=peer, peer_n0=n0, loss=loss, clip=cl)
             if not whole:
                 preds[:, :, :, n0:n1] = out
                 vis[:, :, n0:n1] = v
@@ -479,6 +498,24 @@ class RefineEngine:
         if loss_target is not None:
             loss_out.copy_(_score_map_loss(neg, pos, loss_target, iters, H8 * W8))
         return preds, vis, ffeat_out
+
+    @staticmethod
+    def _check_clip(clip: torch.Tensor, frame_base: Optional[torch.Tensor], B: int, N: int, frames: int,
+                    dev) -> torch.Tensor:
+        """The clip table of refine() as (B,N,2) int32 on ``dev``, after checking 1 <= count and 0 <= first,
+        first + count <= frames: the kernels read pyramid frames through it unchecked."""
+        if frame_base is None:
+            raise L.PipsCudaError("pips_b200: a clip table needs frame_base")
+        if not isinstance(clip, torch.Tensor) or tuple(clip.shape) != (B, N, 2) or clip.dtype.is_floating_point \
+                or clip.dtype.is_complex:
+            raise L.PipsCudaError(f"pips_b200: clip must be ({B}, {N}, 2) int32, got "
+                                  f"{tuple(getattr(clip, 'shape', ()))} {getattr(clip, 'dtype', None)}")
+        c = clip.to(device=dev, dtype=torch.long)
+        first, count = c[..., 0], c[..., 1]
+        if bool(((count < 1) | (first < 0) | (first + count > frames)).any()):
+            raise L.PipsCudaError(f"pips_b200: clip table outside the {frames} frames held (need count >= 1, "
+                                  f"first >= 0, first + count <= {frames})")
+        return c.to(torch.int32).contiguous()
 
     def _plan(self, w: PackedWeights, B, S, N, H8, W8, iters, stride, has_feat, dev, nhwc=False, peer=None,
               losses=False) -> "_GraphPlan":
