@@ -94,6 +94,32 @@ int pips_corr_gather_clips(const void* const* lvl, int feat_dtype, int B, int S,
                            const int* frame_base /* [B*N] */, int frames_per_batch, const int* clip /* NULL or [B*N][2] */,
                            void* x_hi, void* x_lo, float* x_f32, int ldx, void* stream);
 
+/* Several pyramids of different map sizes in one call (videos of different frame sizes tracked together): group g
+ * holds frames[g] frames whose level 0 is H[g] x W[g] (at least 8 x 8); lvl[g][l] is its level l, channels-last
+ * (frames[g], H[g] >> l, W[g] >> l, 128), in the storage type the entry point names.  1 <= G <= PIPS_MAX_GROUPS. */
+#define PIPS_MAX_GROUPS 32
+typedef struct pips_groups {
+    int G;
+    const void* lvl[PIPS_MAX_GROUPS][PIPS_LEVELS];
+    int H[PIPS_MAX_GROUPS], W[PIPS_MAX_GROUPS];   /* level 0 */
+    int frames[PIPS_MAX_GROUPS];
+} pips_groups;
+
+/* pips_corr_gather_clips over the pyramids of `groups` (levels in feat_dtype): table[b*N+n] = {first, count, group, 0}
+ * (int32, 16 bytes per track) names the pyramid group of track (b,n) and its clip {first, count} among that group's
+ * frames, decoded as in pips_corr_gather_clips; the window's boxes, clamps and taps use the group's map sizes.
+ * 0 <= group < G, count >= 1, first + count <= frames[group] (not checked: the kernels trust the table).  frame_base
+ * and the table are required. */
+int pips_corr_gather_groups(const pips_groups* groups, int feat_dtype, int B, int S, int N,
+                            const float* coords, const float* ffeats, const float* times /* [S] */,
+                            const int* frame_base /* [B*N] */, const int* table /* [B*N][4] */,
+                            void* x_hi, void* x_lo, float* x_f32, int ldx, void* stream);
+/* pips_init_gather_clips over the pyramids of `groups`, decoded as in pips_corr_gather_groups: lvl[g][0] is read as
+ * group g's fp32 level 0 (the other levels are not read and may be NULL). */
+int pips_init_gather_groups(const pips_groups* groups, int B, int S, int N, const float* coords,
+                            const int* frame_base /* [B*N] */, const int* table /* [B*N][4] */,
+                            float* ffeat /* (B*N,128) */, float* ffeats /* (B*N,S,128) */, void* stream);
+
 /* Backward of pips_corr_gather's correlation columns (x[:, 128:324]) for training (csrc/corr_grad.cu), with respect to
  * the ffeats and the 4 fp32 levels; the coordinates get no gradient.  S == 8, fp32, no frame_base.  dcorr is the
  * gradient of those 196 columns, (B*N*S, ld_dcorr) in mixer row order, ld_dcorr >= 196.  Per unit and level the
@@ -399,6 +425,11 @@ int pips_refine_iter(const pips_problem* p, const pips_weights* w, const pips_wo
  * p->frame_base (required when clip is non-NULL) and clip [B*N][2]; the mixer and the update are unchanged. */
 int pips_refine_iter_clips(const pips_problem* p, const int* clip /* NULL or [B*N][2] */, const pips_weights* w,
                            const pips_workspace* ws, float* out_px, void* stream);
+/* pips_refine_iter whose correlation reads each track's window in its own pyramid group: pips_corr_gather_groups
+ * over `groups` (levels in p->feat_dtype) with p->frame_base (required) and table [B*N][4] (required).  p->lvl, p->H,
+ * p->W and p->frames_per_batch are ignored; the mixer and the update are unchanged. */
+int pips_refine_iter_groups(const pips_problem* p, const pips_groups* groups, const int* table /* [B*N][4] */,
+                            const pips_weights* w, const pips_workspace* ws, float* out_px, void* stream);
 
 #ifdef __cplusplus
 }

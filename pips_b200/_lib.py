@@ -57,6 +57,15 @@ class PeerOut(C.Structure):
     _fields_ = [("out", _p * MAX_PEERS), ("n_peers", _i), ("n_offset", _i), ("n_total", _i)]
 
 
+MAX_GROUPS = 32                                  # PIPS_MAX_GROUPS
+
+
+class Groups(C.Structure):
+    """pips_groups: several pyramids of different map sizes (the _groups entry points)."""
+    _fields_ = [("G", _i), ("lvl", (_p * LEVELS) * MAX_GROUPS), ("H", _i * MAX_GROUPS), ("W", _i * MAX_GROUPS),
+                ("frames", _i * MAX_GROUPS)]
+
+
 class Problem(C.Structure):
     _fields_ = [("B", _i), ("S", _i), ("N", _i), ("H", _i), ("W", _i), ("feat_dtype", _i), ("precision", _i),
                 ("lvl", _p * LEVELS), ("times", _p), ("coords", _p), ("coords0", _p), ("ffeats", _p), ("stride", _f),
@@ -72,6 +81,8 @@ _SIGNATURES = {
     "pips_corr_gather": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _i, _p, _p, _p, _i, _p]),
     "pips_init_gather_clips": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _p, _p, _p]),
     "pips_corr_gather_clips": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _i, _p, _p, _p, _p, _i, _p]),
+    "pips_init_gather_groups": (_i, [C.POINTER(Groups), _i, _i, _i, _p, _p, _p, _p, _p, _p]),
+    "pips_corr_gather_groups": (_i, [C.POINTER(Groups), _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p]),
     "pips_corr_grad_feats": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _p, _p, _i, _p, _p]),
     "pips_corr_grad_levels": (_i, [_i, _i, _i, _i, _i, _p, _p, _p, _i, C.POINTER(_p), _p]),
     "pips_peer_alloc": (_i, [C.c_size_t, C.POINTER(_p), C.c_char_p]),
@@ -127,6 +138,8 @@ _SIGNATURES = {
     "pips_mixer_forward": (_i, [C.POINTER(Weights), C.POINTER(Workspace), _i, _i, _p]),
     "pips_refine_iter": (_i, [C.POINTER(Problem), C.POINTER(Weights), C.POINTER(Workspace), _p, _p]),
     "pips_refine_iter_clips": (_i, [C.POINTER(Problem), _p, C.POINTER(Weights), C.POINTER(Workspace), _p, _p]),
+    "pips_refine_iter_groups": (_i, [C.POINTER(Problem), C.POINTER(Groups), _p, C.POINTER(Weights),
+                                     C.POINTER(Workspace), _p, _p]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

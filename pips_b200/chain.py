@@ -16,6 +16,7 @@ the per-particle loop up to fp32 noise.
 same chain on the time-reversed clip from frame t back to frame 0.  A backward track reads its windows through a
 negative frame offset (``~t``), so both directions share the pyramid and the rounds.  ``track_queries_batch`` does the
 same for many clips at once: their frames share one pyramid, and every track also carries its clip's place in it.
+``track_queries_mixed`` takes clips of any frame sizes: one pyramid per size, and every track also names its pyramid.
 """
 from __future__ import annotations
 
@@ -24,6 +25,9 @@ from typing import Optional
 import torch
 
 S_WIN = 8
+# Distinct frame sizes one refinement call of track_queries_mixed reads (PIPS_MAX_GROUPS of the C library): a batch
+# with more sizes runs as successive sub-batches of at most this many.
+MAX_GROUPS = 32
 
 
 def _threshold_table(n: int = 64) -> torch.Tensor:
@@ -67,7 +71,8 @@ class _Tracks:
     window at cursor c writes row row0[k] + c + s of traj (rows, n, 2) and vis (rows, n); vis holds sigmoid(vis_e) of
     the window that last wrote the row, and is None unless ``want_vis``.  ``clip`` (n, 2) int32 (optional): track k's
     clip {first, count} among the held frames when they hold several videos; base0[k] then counts inside that clip
-    (clip_window_frame in csrc/corr_common.cuh)."""
+    (clip_window_frame in csrc/corr_common.cuh).  With feature maps in groups (track_queries_mixed) ``clip`` is (n, 3)
+    {first, count, group}: the clip among the frames of pyramid group ``group``."""
 
     def __init__(self, base0: torch.Tensor, length: torch.Tensor, xy: torch.Tensor, rows: int, want_vis: bool,
                  fill: float = 0.0, clip: Optional[torch.Tensor] = None):
@@ -93,9 +98,12 @@ def _run_rounds(model, fmaps: torch.Tensor, tr: _Tracks, iters: int, advance: Op
     while it is inside its clip and, unless the video has ``ended``, its whole window has arrived.  A window past the
     last held frame replicates that frame, which is the end-of-clip rule once the video has ended.  A track's first
     window gathers its own feature; later windows carry it (outs[3], chain_demo.py:57).  With a per-track clip
-    (tr.clip) the refinement calls pass the runnable tracks' rows of it as ``clip``; without one they pass no clip."""
-    F = fmaps.shape[1]
-    dev = fmaps.device
+    (tr.clip) the refinement calls pass the runnable tracks' rows of it as ``clip``; without one they pass no clip.
+    ``fmaps`` may also be a list of such tensors of different map sizes, one per pyramid group, with a 3-column
+    tr.clip and ``ended``."""
+    grouped = isinstance(fmaps, (list, tuple))
+    F = None if grouped else fmaps.shape[1]
+    dev = (fmaps[0] if grouped else fmaps).device
     eng = model.engine
     stride = float(model.stride)
     thr = _threshold_table().to(dev)
@@ -113,7 +121,7 @@ def _run_rounds(model, fmaps: torch.Tensor, tr: _Tracks, iters: int, advance: Op
         fb = (tr.base0[run] + c - f0).view(1, na).to(torch.int32)
         coords = (tr.pos[run] / stride).view(1, 1, na, 2).repeat(1, S_WIN, 1, 1)    # zero-velocity init, :453
         new = ~tr.started[run]
-        cl = None if tr.clip is None else tr.clip[run].view(1, na, 2)
+        cl = None if tr.clip is None else tr.clip[run].view(1, na, tr.clip.shape[1])
         fi = None
         if not bool(new.all()):
             if bool(new.any()):
@@ -286,20 +294,38 @@ def track_queries_batch(model, clips, queries, iters: int = 6, return_rounds: bo
     refinement call over the tracks of all clips, and the batch takes as many rounds as its longest clip's chain.  The
     device holds the feature maps and the pyramid of every frame of the batch, about 1.2 MiB per 256x256 frame at
     stride 8 with fp32 features: the caller bounds the batch."""
+    views = _batch_views(model, clips, queries, "track_queries_batch")
+    hw = tuple(views[0].shape[-2:])
+    for i, v in enumerate(views):
+        if tuple(v.shape[-2:]) != hw:
+            raise ValueError(f"clips[{i}] frames are {tuple(v.shape[-2:])}, clips[0]'s are {hw}: one batch, one size")
+    ts = _batch_query_frames(model, views, queries)
+    fmaps = _encode_batch(model, views)
+    first = torch.tensor([0] + [v.shape[0] for v in views]).cumsum(0).tolist()
+    tr, cols = _batch_tracks(views, queries, ts, [[first[i], v.shape[0]] for i, v in enumerate(views)])
+    _run_rounds(model, fmaps, tr, iters)
+    outs = [_merge_directions(tr, t, back, v.shape[0], c0) for v, t, (c0, back) in zip(views, ts, cols)]
+    return (outs, tr.rounds) if return_rounds else outs
+
+
+def _batch_views(model, clips, queries, who: str):
+    """The checks track_queries_batch and track_queries_mixed make before any work; returns the clips as
+    (T_i, 3, H_i, W_i) views."""
     shard = getattr(model, "_shard", None)
     if shard is not None and shard[1] > 1:
         raise RuntimeError("pips_b200.chain: chained tracking does not cover particle-sharded models")
     if len(clips) != len(queries):
         raise ValueError(f"{len(clips)} clips but {len(queries)} query sets: one query set per clip")
     if len(clips) == 0:
-        raise ValueError("empty batch: track_queries_batch needs at least one clip")
-    views = [_batch_clip(c, i) for i, c in enumerate(clips)]
-    hw = tuple(views[0].shape[-2:])
-    for i, v in enumerate(views):
-        if tuple(v.shape[-2:]) != hw:
-            raise ValueError(f"clips[{i}] frames are {tuple(v.shape[-2:])}, clips[0]'s are {hw}: one batch, one size")
+        raise ValueError(f"empty batch: {who} needs at least one clip")
+    return [_batch_clip(c, i) for i, c in enumerate(clips)]
+
+
+def _batch_query_frames(model, views, queries):
+    """Checks every clip's queries as track_queries does; returns each clip's query frames (N_i,) on the model's
+    device."""
     dev = next(iter(model.parameters())).device
-    ts = []                                                                          # query frames per clip, on dev
+    ts = []
     for i, (v, q) in enumerate(zip(views, queries)):
         if isinstance(q, torch.Tensor) and q.dim() == 2:
             q = q.unsqueeze(0)
@@ -307,10 +333,17 @@ def track_queries_batch(model, clips, queries, iters: int = 6, return_rounds: bo
             ts.append(_check_queries(v.unsqueeze(0), q).to(dev))
         except ValueError as e:
             raise ValueError(f"queries[{i}]: {e}") from None
-    fmaps = _encode_batch(model, views)
+    return ts
+
+
+def _batch_tracks(views, queries, ts, rows):
+    """The _Tracks of a batch: each clip's forward tracks, then its backward tracks (queries with t > 0), clip after
+    clip, every track of clip i carrying the clip table row rows[i].  Returns the tracks and, per clip, (its first
+    column, its queries with a backward track) for _merge_directions."""
+    dev = ts[0].device
     base0, length, xy, clip, cols = [], [], [], [], []
-    first, c0 = 0, 0
-    for v, q, t in zip(views, queries, ts):
+    c0 = 0
+    for v, q, t, row in zip(views, queries, ts, rows):
         T, N = v.shape[0], t.numel()
         qxy = q.reshape(-1, 3)[:, 1:3].to(device=dev, dtype=torch.float32)
         back = (t > 0).nonzero().flatten()                                           # queries with a backward track
@@ -319,12 +352,54 @@ def track_queries_batch(model, clips, queries, iters: int = 6, return_rounds: bo
         length += [T - t, tb + 1]
         xy += [qxy, qxy[back]]
         n = N + back.numel()
-        clip.append(torch.tensor([first, T], dtype=torch.int32, device=dev).expand(n, 2))
+        clip.append(torch.tensor(row, dtype=torch.int32, device=dev).expand(n, len(row)))
         cols.append((c0, back))
-        first += T
         c0 += n
     tr = _Tracks(torch.cat(base0), torch.cat(length), torch.cat(xy), max(v.shape[0] for v in views), want_vis=True,
                  clip=torch.cat(clip).contiguous())
-    _run_rounds(model, fmaps, tr, iters)
-    outs = [_merge_directions(tr, t, back, v.shape[0], c0) for v, t, (c0, back) in zip(views, ts, cols)]
-    return (outs, tr.rounds) if return_rounds else outs
+    return tr, cols
+
+
+@torch.no_grad()
+def track_queries_mixed(model, clips, queries, iters: int = 6, return_rounds: bool = False):
+    """``track_queries_batch`` for clips of any frame sizes: every clip's tracks advance in the same rounds.
+
+    ``clips`` and ``queries`` are as in track_queries_batch, except that each clip may have its own H x W; its feature
+    map, (H // stride) x (W // stride), must be at least 8 x 8.  Returns a list with one (trajs (1, T_i, N_i, 2),
+    vis (1, T_i, N_i)) pair per clip -- the same bits as ``track_queries(model, clips[i][None], queries[i][None])`` --
+    and the number of rounds when ``return_rounds``.
+
+    The clips are grouped by frame size.  Each group's frames are encoded once, in 32-frame chunks that run across its
+    clips' boundaries, into that group's own pyramid.  Every track reads its windows inside its own clip of its own
+    group's pyramid through a per-track table {first, count, group} (pips_corr_gather_groups), so each round is one
+    refinement call over the tracks of all clips of all sizes, and the batch takes as many rounds as its longest clip's
+    chain.  A batch with more than MAX_GROUPS sizes runs as successive sub-batches of at most MAX_GROUPS sizes, each
+    with its own rounds.  The device holds the feature maps and the pyramids of every frame of a sub-batch: the caller
+    bounds the batch."""
+    views = _batch_views(model, clips, queries, "track_queries_mixed")
+    stride = int(model.stride)
+    for i, v in enumerate(views):
+        h, w = v.shape[-2:]
+        if h // stride < 8 or w // stride < 8:
+            raise ValueError(f"clips[{i}] frames are {h}x{w}: the feature map at stride {stride} is "
+                             f"{h // stride}x{w // stride}, under the 8x8 the 4-level pyramid needs")
+    ts = _batch_query_frames(model, views, queries)
+    sizes = list(dict.fromkeys(tuple(v.shape[-2:]) for v in views))                # in order of first appearance
+    outs, rounds = [None] * len(views), 0
+    for s0 in range(0, len(sizes), MAX_GROUPS):
+        fmaps, order, rows = [], [], []
+        for g, hw in enumerate(sizes[s0:s0 + MAX_GROUPS]):
+            idx = [i for i, v in enumerate(views) if tuple(v.shape[-2:]) == hw]
+            fmaps.append(_encode_batch(model, [views[i] for i in idx]))
+            first = 0
+            for i in idx:
+                order.append(i)
+                rows.append([first, views[i].shape[0], g])
+                first += views[i].shape[0]
+        tr, cols = _batch_tracks([views[i] for i in order], [queries[i] for i in order], [ts[i] for i in order], rows)
+        _run_rounds(model, fmaps, tr, iters)
+        for i, (c0, back) in zip(order, cols):
+            outs[i] = _merge_directions(tr, ts[i], back, views[i].shape[0], c0)
+        rounds += tr.rounds
+        del fmaps, tr                                   # a sub-batch's maps go before the next one's are encoded
+    return (outs, rounds) if return_rounds else outs

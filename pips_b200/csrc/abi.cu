@@ -148,8 +148,9 @@ extern "C" int pips_mixer_forward(const pips_weights* w, const pips_workspace* w
     return rc;
 }
 
+// pips_refine_iter, _clips and _groups: `groups` (with clip as its [B*N][4] table) selects pips_corr_gather_groups
 static int refine_iter_entry(const char* who, const pips_problem* p, const int* clip, const pips_weights* w,
-                             const pips_workspace* ws, float* out_px, void* stream) {
+                             const pips_workspace* ws, float* out_px, void* stream, const pips_groups* groups = nullptr) {
     if (!p || !w || !ws || !out_px) {
         snprintf(g_err, sizeof(g_err), "%s: null argument", who);
         return 1;
@@ -165,7 +166,11 @@ static int refine_iter_entry(const char* who, const pips_problem* p, const int* 
     const int seqs = p->B * p->N;
     const bool f32 = p->precision == PIPS_PREC_F32;
     const bool x3 = p->precision == PIPS_PREC_BF16X3;
-    int rc = clip ? pips_corr_gather_clips(p->lvl, p->feat_dtype, p->B, p->S, p->N, p->H, p->W, p->coords, p->ffeats, p->times,
+    int rc = groups ? pips_corr_gather_groups(groups, p->feat_dtype, p->B, p->S, p->N, p->coords, p->ffeats, p->times,
+                                              p->frame_base, clip,
+                                              f32 ? nullptr : ws->x0_hi, x3 ? ws->x0_lo : nullptr, f32 ? ws->x0_f32 : nullptr,
+                                              PIPS_KITCHEN_PAD, stream)
+           : clip ? pips_corr_gather_clips(p->lvl, p->feat_dtype, p->B, p->S, p->N, p->H, p->W, p->coords, p->ffeats, p->times,
                                            p->frame_base, p->frames_per_batch, clip,
                                            f32 ? nullptr : ws->x0_hi, x3 ? ws->x0_lo : nullptr, f32 ? ws->x0_f32 : nullptr,
                                            PIPS_KITCHEN_PAD, stream)
@@ -188,4 +193,13 @@ extern "C" int pips_refine_iter(const pips_problem* p, const pips_weights* w, co
 extern "C" int pips_refine_iter_clips(const pips_problem* p, const int* clip, const pips_weights* w,
                                       const pips_workspace* ws, float* out_px, void* stream) {
     return refine_iter_entry("pips_refine_iter_clips", p, clip, w, ws, out_px, stream);
+}
+
+extern "C" int pips_refine_iter_groups(const pips_problem* p, const pips_groups* groups, const int* table,
+                                       const pips_weights* w, const pips_workspace* ws, float* out_px, void* stream) {
+    if (!groups || !table) {
+        snprintf(g_err, sizeof(g_err), "pips_refine_iter_groups: the grouped mode needs groups and a table");
+        return 1;
+    }
+    return refine_iter_entry("pips_refine_iter_groups", p, table, w, ws, out_px, stream, groups);
 }

@@ -9,7 +9,17 @@ namespace pips {
 constexpr int CG_ROWS_PER_BOX = 2;     // a footprint is read as 4 boxes {128 ch, 8 px, 2 rows}
 
 struct CgMaps {
+    static constexpr bool kGroups = false;
     CUtensorMap m[PIPS_LEVELS];
+};
+
+// The grouped mode of pips_corr_gather (several pyramids of different map sizes in one call): each track's clip table
+// entry names its group, and group g's levels are read through m[g][l] with the dims H[g][l], W[g][l].  A
+// __grid_constant__ kernel parameter, so that the per-track indexing by group reads the parameter bank directly.
+struct CgGroupMaps {
+    static constexpr bool kGroups = true;
+    CUtensorMap m[PIPS_MAX_GROUPS][PIPS_LEVELS];
+    int H[PIPS_MAX_GROUPS][PIPS_LEVELS], W[PIPS_MAX_GROUPS][PIPS_LEVELS];
 };
 
 struct CgArgs {
@@ -24,8 +34,12 @@ struct CgArgs {
     __nv_bfloat16* x_lo;
     float* x_f32;
     int ldx;
-    const int* clip;         // optional [B*N][2] {first, count}: each track's clip in the pyramid (clip_window_frame)
+    const int* clip;         // optional [B*N][2] {first, count}: each track's clip in the pyramid (clip_window_frame);
+                             // [B*N][4] {first, count, group, 0} in the grouped mode (CgGroupMaps)
 };
+
+// Kernel parameters are limited to 32 764 bytes (CUDA >= 12.1 on sm_70+); the grouped mode passes all its maps there.
+static_assert(sizeof(CgGroupMaps) + sizeof(CgArgs) <= 32764, "grouped corr_gather parameters exceed the 32 764-byte limit");
 
 // Frame index, inside its clip of T frames, of step s of a chained track's window (pips_init_gather reads step 0,
 // pips_corr_gather steps 0..7).  base >= 0: a forward window from frame base, min(base + s, T-1) -- past the clip's
@@ -46,9 +60,19 @@ __device__ __forceinline__ int clip_window_frame(const int* clip, int seq, int b
     return c.x + window_frame(base, s, c.y);
 }
 
+// Level dims and tensor map of level l for a unit of pyramid group g: the call's own (CgArgs / CgMaps, g ignored) or
+// group g's (CgGroupMaps).
+__device__ __forceinline__ int level_w(const CgArgs& a, const CgMaps*, int, int l) { return a.W[l]; }
+__device__ __forceinline__ int level_h(const CgArgs& a, const CgMaps*, int, int l) { return a.H[l]; }
+__device__ __forceinline__ int level_w(const CgArgs&, const CgGroupMaps* m, int g, int l) { return m->W[g][l]; }
+__device__ __forceinline__ int level_h(const CgArgs&, const CgGroupMaps* m, int g, int l) { return m->H[g][l]; }
+__device__ __forceinline__ const CUtensorMap* level_map(const CgMaps& m, int, int l) { return &m.m[l]; }
+__device__ __forceinline__ const CUtensorMap* level_map(const CgGroupMaps& m, int g, int l) { return &m.m[g][l]; }
+
 struct UnitInfo {
     float cx, cy;      // coords of (b,s,n), level-0 pixels
-    int frame;         // pyramid frame index
+    int frame;         // pyramid frame index (inside the track's group in the grouped mode)
+    int group;         // pyramid group (grouped mode; 0 otherwise)
     int b, n, s;
     int valid;
     int ox, oy;        // lane l < 4: TMA box origin (first column, first row) of pyramid level l for this unit
@@ -58,24 +82,32 @@ struct UnitInfo {
 // computes the box origin of ONE pyramid level (lane & 3), so that issuing a TMA box later costs two shuffles instead
 // of a clamp / floor / convert chain executed by lane 0 alone while 31 lanes wait.  Coordinates are clamped in float
 // so that diverged or non-finite tracks cannot overflow the int conversion (beyond +-8 px of the map all taps are zero).
-// kClips: the frame comes from the per-track clip table (a.clip and a.frame_base both set).
-template <bool kClips = false>
-__device__ __forceinline__ UnitInfo load_unit(const CgArgs& a, int u, int total) {
+// kClips: the frame comes from the per-track clip table (a.clip and a.frame_base both set).  With CgGroupMaps the table
+// entry is one int4 {first, count, group, 0}, and the level dims are the group's.
+template <bool kClips = false, typename Maps = CgMaps>
+__device__ __forceinline__ UnitInfo load_unit(const CgArgs& a, int u, int total, const Maps* maps = nullptr) {
     UnitInfo ui;
     ui.valid = u < total;
-    ui.cx = 0.f; ui.cy = 0.f; ui.frame = 0; ui.b = 0; ui.n = 0; ui.s = 0; ui.ox = 0; ui.oy = 0;
+    ui.cx = 0.f; ui.cy = 0.f; ui.frame = 0; ui.group = 0; ui.b = 0; ui.n = 0; ui.s = 0; ui.ox = 0; ui.oy = 0;
     if (ui.valid) {
         ui.s = u & 7;
         const int seq = u >> 3;
         ui.b = seq / a.N; ui.n = seq - ui.b * a.N;
         const float2 c = *reinterpret_cast<const float2*>(a.coords + ((static_cast<size_t>(ui.b) * 8 + ui.s) * a.N + ui.n) * 2);
         ui.cx = c.x; ui.cy = c.y;
-        if (kClips) ui.frame = clip_window_frame(a.clip, seq, a.frame_base[seq], ui.s);
-        else ui.frame = a.frame_base ? ui.b * a.T + window_frame(a.frame_base[seq], ui.s, a.T) : ui.b * 8 + ui.s;
+        if constexpr (Maps::kGroups) {
+            const int4 e = reinterpret_cast<const int4*>(a.clip)[seq];
+            ui.frame = e.x + window_frame(a.frame_base[seq], ui.s, e.y);
+            ui.group = e.z;
+        } else if (kClips) {
+            ui.frame = clip_window_frame(a.clip, seq, a.frame_base[seq], ui.s);
+        } else {
+            ui.frame = a.frame_base ? ui.b * a.T + window_frame(a.frame_base[seq], ui.s, a.T) : ui.b * 8 + ui.s;
+        }
         const int level = threadIdx.x & 3;
         const float sc = 1.0f / static_cast<float>(1 << level);        // coords / 2**i  (nets/pips.py:373), exact
-        const float cxl = fminf(fmaxf(c.x * sc, -8.0f), static_cast<float>(a.W[level]) + 8.0f);
-        const float cyl = fminf(fmaxf(c.y * sc, -8.0f), static_cast<float>(a.H[level]) + 8.0f);
+        const float cxl = fminf(fmaxf(c.x * sc, -8.0f), static_cast<float>(level_w(a, maps, ui.group, level)) + 8.0f);
+        const float cyl = fminf(fmaxf(c.y * sc, -8.0f), static_cast<float>(level_h(a, maps, ui.group, level)) + 8.0f);
         ui.ox = static_cast<int>(floorf(cxl)) - PIPS_RADIUS;
         ui.oy = static_cast<int>(floorf(cyl)) - PIPS_RADIUS;
     }

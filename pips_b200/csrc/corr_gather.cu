@@ -54,9 +54,11 @@ __device__ __forceinline__ float4 ld_chan4(const __nv_bfloat16* p) {
 }
 
 // kClips: each track reads its window inside its own clip of the pyramid (CgArgs::clip, clip_window_frame).
-template <typename T, bool kClips>
+// Maps = CgGroupMaps (with kClips): the grouped mode -- the clip table also names each track's pyramid group, whose
+// tensor maps and level dims its boxes, clamps and taps use.
+template <typename T, bool kClips, typename Maps = CgMaps>
 __global__ void __launch_bounds__(CG_WARPS * 32)
-corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
+corr_gather_kernel(const __grid_constant__ Maps maps, const CgArgs a) {
     using Cfg = CgCfg<T>;
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
@@ -93,13 +95,13 @@ corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
         if (lane == 0) {
             const uint32_t bar = bar0 + 8 * slot;
             mbar_arrive_expect_tx(bar, Cfg::kBoxBytes);
-            tma_load_4d(stage0 + slot * Cfg::kBoxBytes, &maps.m[level], bar, 0, x0, y0, ui.frame);
+            tma_load_4d(stage0 + slot * Cfg::kBoxBytes, level_map(maps, ui.group, level), bar, 0, x0, y0, ui.frame);
         }
     };
 
     pdl_wait();                                     // coords / ffeats / pyramid come from earlier kernels of the chain
-    UnitInfo cur = load_unit<kClips>(a, u, total);
-    UnitInfo nxt = load_unit<kClips>(a, u + nwarps, total);
+    UnitInfo cur = load_unit<kClips>(a, u, total, &maps);
+    UnitInfo nxt = load_unit<kClips>(a, u + nwarps, total, &maps);
     float4 q = *reinterpret_cast<const float4*>(a.ffeats + static_cast<size_t>(u) * 128 + lane * 4);
     issue(cur, 0, 0, 0);
     issue(cur, 0, 1, 1);
@@ -110,7 +112,7 @@ corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
         // prefetch the next unit's query while this one is processed
         float4 nq = make_float4(0.f, 0.f, 0.f, 0.f);
         if (nxt.valid) nq = *reinterpret_cast<const float4*>(a.ffeats + static_cast<size_t>(u + nwarps) * 128 + lane * 4);
-        const UnitInfo nxt2 = load_unit<kClips>(a, u + 2 * nwarps, total);
+        const UnitInfo nxt2 = load_unit<kClips>(a, u + 2 * nwarps, total, &maps);
 
 #pragma unroll 1
         for (int level = 0; level < PIPS_LEVELS; ++level) {
@@ -148,8 +150,8 @@ corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
             }
             {
                 const float sc = 1.0f / static_cast<float>(1 << level);
-                const float cxl = fminf(fmaxf(cur.cx * sc, -8.0f), static_cast<float>(a.W[level]) + 8.0f);
-                const float cyl = fminf(fmaxf(cur.cy * sc, -8.0f), static_cast<float>(a.H[level]) + 8.0f);
+                const float cxl = fminf(fmaxf(cur.cx * sc, -8.0f), static_cast<float>(level_w(a, &maps, cur.group, level)) + 8.0f);
+                const float cyl = fminf(fmaxf(cur.cy * sc, -8.0f), static_cast<float>(level_h(a, &maps, cur.group, level)) + 8.0f);
                 const float fx = cxl - floorf(cxl), fy = cyl - floorf(cyl);
                 const float w00 = (1.f - fx) * (1.f - fy), w01 = fx * (1.f - fy), w10 = (1.f - fx) * fy, w11 = fx * fy;
 #pragma unroll
@@ -204,15 +206,12 @@ corr_gather_kernel(const __grid_constant__ CgMaps maps, const CgArgs a) {
     }
 }
 
-template <typename T, bool kClips>
-static int launch_corr_gather(const void* const* lvl, CUtensorMapDataType dt, const CgArgs& args, int frames, cudaStream_t st) {
-    CgMaps maps;
-    if (encode_level_maps(maps, lvl, dt, sizeof(T), args.H, args.W, frames, "pips_corr_gather: cuTensorMapEncodeTiled failed"))
-        return 1;
+template <typename T, bool kClips, typename Maps>
+static int launch_corr_gather(const Maps& maps, const CgArgs& args, cudaStream_t st) {
     using Cfg = CgCfg<T>;
     static bool attr[kMaxDevices] = {};
     {
-        cudaError_t e = ensure_dyn_smem(corr_gather_kernel<T, kClips>, attr, static_cast<int>(Cfg::kSmemBytes));
+        cudaError_t e = ensure_dyn_smem(corr_gather_kernel<T, kClips, Maps>, attr, static_cast<int>(Cfg::kSmemBytes));
         if (e != cudaSuccess) return fail_cuda("pips_corr_gather: smem attribute", e);
     }
     const long long units = static_cast<long long>(args.B) * args.S * args.N;
@@ -221,9 +220,35 @@ static int launch_corr_gather(const void* const* lvl, CUtensorMapDataType dt, co
     long long grid = (units + CG_WARPS - 1) / CG_WARPS;
     const long long cap = static_cast<long long>(sm_count()) * ctas_per_sm;
     if (grid > cap) grid = cap;
-    cudaError_t e = launch_pdl(corr_gather_kernel<T, kClips>, dim3(static_cast<unsigned>(grid)), dim3(CG_WARPS * 32), Cfg::kSmemBytes, st, maps, args);
+    cudaError_t e = launch_pdl(corr_gather_kernel<T, kClips, Maps>, dim3(static_cast<unsigned>(grid)), dim3(CG_WARPS * 32), Cfg::kSmemBytes, st, maps, args);
     if (e == cudaSuccess) e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail_cuda("pips_corr_gather: launch", e);
+}
+
+template <typename T, bool kClips>
+static int launch_corr_gather(const void* const* lvl, CUtensorMapDataType dt, const CgArgs& args, int frames, cudaStream_t st) {
+    CgMaps maps;
+    if (encode_level_maps(maps, lvl, dt, sizeof(T), args.H, args.W, frames, "pips_corr_gather: cuTensorMapEncodeTiled failed"))
+        return 1;
+    return launch_corr_gather<T, kClips, CgMaps>(maps, args, st);
+}
+
+// The grouped mode: group g's 4 level maps and dims; its levels are (frames[g], H[g] >> l, W[g] >> l, 128).
+template <typename T>
+static int launch_corr_gather_groups(const pips_groups& g, CUtensorMapDataType dt, const CgArgs& args, cudaStream_t st) {
+    CgGroupMaps maps;
+    for (int k = 0; k < g.G; ++k) {
+        int h = g.H[k], w = g.W[k];
+        for (int l = 0; l < PIPS_LEVELS; ++l) {
+            maps.H[k][l] = h; maps.W[k][l] = w; h /= 2; w /= 2;
+        }
+        CgMaps one;
+        if (encode_level_maps(one, g.lvl[k], dt, sizeof(T), maps.H[k], maps.W[k], g.frames[k],
+                              "pips_corr_gather_groups: cuTensorMapEncodeTiled failed"))
+            return 1;
+        for (int l = 0; l < PIPS_LEVELS; ++l) maps.m[k][l] = one.m[l];
+    }
+    return launch_corr_gather<T, true, CgGroupMaps>(maps, args, st);
 }
 
 }  // namespace pips
@@ -283,4 +308,40 @@ extern "C" int pips_corr_gather_clips(const void* const* lvl, int feat_dtype, in
                                       void* stream) {
     return corr_gather_entry("pips_corr_gather_clips", lvl, feat_dtype, B, S, N, H, W, coords, ffeats, times, frame_base,
                              frames_per_batch, clip, x_hi, x_lo, x_f32, ldx, stream);
+}
+
+extern "C" int pips_corr_gather_groups(const pips_groups* groups, int feat_dtype, int B, int S, int N, const float* coords,
+                                       const float* ffeats, const float* times, const int* frame_base, const int* table,
+                                       void* x_hi, void* x_lo, float* x_f32, int ldx, void* stream) {
+    const char* who = "pips_corr_gather_groups";
+    char msg[160];
+    auto err = [&](const char* what) {
+        snprintf(msg, sizeof(msg), "%s: %s", who, what);
+        return fail(msg);
+    };
+    if (!groups || !coords || !ffeats || !times) return err("null pointer");
+    if (!frame_base || !table) return err("the grouped mode needs frame_base and a table");
+    if (S != PIPS_S) return err("S must be 8");
+    if (B <= 0 || N <= 0) return err("empty problem");
+    if (groups->G < 1 || groups->G > PIPS_MAX_GROUPS) return err("need 1 <= G <= PIPS_MAX_GROUPS");
+    for (int k = 0; k < groups->G; ++k) {
+        if (groups->H[k] < 8 || groups->W[k] < 8) return err("every group's level-0 map must be at least 8x8");
+        if (groups->frames[k] < 1) return err("every group needs frames >= 1");
+        for (int l = 0; l < PIPS_LEVELS; ++l)
+            if (!groups->lvl[k][l]) return err("null level pointer");
+    }
+    if (!x_hi && !x_f32) return err("no output buffer");
+    if (x_lo && !x_hi) return err("x_lo without x_hi");
+    if (ldx < PIPS_KITCHEN_PAD || (ldx % 8)) return err("ldx must be >= 576 and a multiple of 8");
+    CgArgs a = {};
+    a.B = B; a.S = S; a.N = N;
+    a.coords = coords; a.ffeats = ffeats; a.times = times;
+    a.frame_base = frame_base; a.T = 0;                        // frames and dims come from each track's group
+    a.x_hi = static_cast<__nv_bfloat16*>(x_hi); a.x_lo = static_cast<__nv_bfloat16*>(x_lo); a.x_f32 = x_f32; a.ldx = ldx;
+    a.clip = table;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (feat_dtype == PIPS_FEAT_F32) return launch_corr_gather_groups<float>(*groups, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a, st);
+    if (feat_dtype == PIPS_FEAT_BF16)
+        return launch_corr_gather_groups<__nv_bfloat16>(*groups, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, a, st);
+    return err("unknown feat_dtype");
 }

@@ -64,17 +64,11 @@ __global__ void f32_to_bf16_kernel(const float* __restrict__ in, __nv_bfloat16* 
     }
 }
 
-// one warp per (b, n): 4 clamped taps x 128 channels, unclamped weights, result broadcast to the S rows.
-// kClips: the window starts inside the track's own clip of the pyramid (clip_window_frame).
-template <bool kClips>
-__global__ void init_gather_kernel(const float* __restrict__ lvl0, int B, int S, int N, int H, int W,
-                                   const float* __restrict__ coords, const int* __restrict__ frame_base, int T,
-                                   float* __restrict__ ffeat, float* __restrict__ ffeats, const int* __restrict__ clip) {
-    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (warp >= B * N) return;
-    const int b = warp / N, n = warp % N;
-    const size_t ci = ((static_cast<size_t>(b) * S + 0) * N + n) * 2;
-    const float x = coords[ci], y = coords[ci + 1];
+// Track `warp` = (b, n) of one init_gather warp: 4 clamped taps x 128 channels of frame `frame` of the H x W level 0,
+// unclamped weights, result broadcast to the S rows.
+__device__ __forceinline__ void init_gather_track(const float* __restrict__ lvl0, int S, int H, int W, int frame, float x,
+                                                  float y, int warp, int lane, float* __restrict__ ffeat,
+                                                  float* __restrict__ ffeats) {
     const float x0f = floorf(x), y0f = floorf(y);
     const float x1f = x0f + 1.0f, y1f = y0f + 1.0f;
     // clamp in float first so that huge / non-finite coordinates cannot overflow the int conversion
@@ -84,8 +78,6 @@ __global__ void init_gather_kernel(const float* __restrict__ lvl0, int B, int S,
     const int y1 = static_cast<int>(fminf(fmaxf(y1f, 0.f), static_cast<float>(H - 1)));
     const float w00 = (x1f - x) * (y1f - y), w01 = (x - x0f) * (y1f - y);
     const float w10 = (x1f - x) * (y - y0f), w11 = (x - x0f) * (y - y0f);
-    const int frame = kClips ? clip_window_frame(clip, warp, frame_base[warp], 0)           // first frame of the track's window
-                             : frame_base ? b * T + window_frame(frame_base[warp], 0, T) : b * S;
     const float* img = lvl0 + static_cast<size_t>(frame) * H * W * 128;
     const float4 a = *reinterpret_cast<const float4*>(img + (static_cast<size_t>(y0) * W + x0) * 128 + lane * 4);
     const float4 bq = *reinterpret_cast<const float4*>(img + (static_cast<size_t>(y0) * W + x1) * 128 + lane * 4);
@@ -99,6 +91,41 @@ __global__ void init_gather_kernel(const float* __restrict__ lvl0, int B, int S,
     *reinterpret_cast<float4*>(ffeat + static_cast<size_t>(warp) * 128 + lane * 4) = o;
     for (int s = 0; s < S; ++s)
         *reinterpret_cast<float4*>(ffeats + (static_cast<size_t>(warp) * S + s) * 128 + lane * 4) = o;
+}
+
+// one warp per (b, n).  kClips: the window starts inside the track's own clip of the pyramid (clip_window_frame).
+template <bool kClips>
+__global__ void init_gather_kernel(const float* __restrict__ lvl0, int B, int S, int N, int H, int W,
+                                   const float* __restrict__ coords, const int* __restrict__ frame_base, int T,
+                                   float* __restrict__ ffeat, float* __restrict__ ffeats, const int* __restrict__ clip) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= B * N) return;
+    const int b = warp / N, n = warp % N;
+    const size_t ci = ((static_cast<size_t>(b) * S + 0) * N + n) * 2;
+    const float x = coords[ci], y = coords[ci + 1];
+    const int frame = kClips ? clip_window_frame(clip, warp, frame_base[warp], 0)           // first frame of the track's window
+                             : frame_base ? b * T + window_frame(frame_base[warp], 0, T) : b * S;
+    init_gather_track(lvl0, S, H, W, frame, x, y, warp, lane, ffeat, ffeats);
+}
+
+// Level 0 of each pyramid group of pips_init_gather_groups.
+struct IgGroups {
+    const float* lvl0[PIPS_MAX_GROUPS];
+    int H[PIPS_MAX_GROUPS], W[PIPS_MAX_GROUPS];
+};
+
+// init_gather_kernel<true> over several pyramids: table[warp] = {first, count, group, 0} (pips_corr_gather_groups).
+__global__ void init_gather_groups_kernel(const __grid_constant__ IgGroups g, int B, int S, int N,
+                                          const float* __restrict__ coords, const int* __restrict__ frame_base,
+                                          const int4* __restrict__ table, float* __restrict__ ffeat,
+                                          float* __restrict__ ffeats) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= B * N) return;
+    const int b = warp / N, n = warp % N;
+    const size_t ci = ((static_cast<size_t>(b) * S + 0) * N + n) * 2;
+    const int4 e = table[warp];
+    const int frame = e.x + window_frame(frame_base[warp], 0, e.y);
+    init_gather_track(g.lvl0[e.z], S, g.H[e.z], g.W[e.z], frame, coords[ci], coords[ci + 1], warp, lane, ffeat, ffeats);
 }
 
 }  // namespace pips
@@ -194,4 +221,27 @@ extern "C" int pips_init_gather_clips(const float* lvl0_f32, int B, int S, int N
                                       float* ffeats, void* stream) {
     return init_gather_entry("pips_init_gather_clips", lvl0_f32, B, S, N, H, W, coords, frame_base, frames_per_batch, clip,
                              ffeat, ffeats, stream);
+}
+
+extern "C" int pips_init_gather_groups(const pips_groups* groups, int B, int S, int N, const float* coords,
+                                       const int* frame_base, const int* table, float* ffeat, float* ffeats,
+                                       void* stream) {
+    if (!groups || !coords || !ffeat || !ffeats) return fail("pips_init_gather_groups: null pointer");
+    if (!frame_base || !table) return fail("pips_init_gather_groups: the grouped mode needs frame_base and a table");
+    if (B <= 0 || N <= 0 || S <= 0) return fail("pips_init_gather_groups: empty problem");
+    if (groups->G < 1 || groups->G > PIPS_MAX_GROUPS) return fail("pips_init_gather_groups: need 1 <= G <= PIPS_MAX_GROUPS");
+    IgGroups g = {};
+    for (int k = 0; k < groups->G; ++k) {
+        if (groups->H[k] < 8 || groups->W[k] < 8)
+            return fail("pips_init_gather_groups: every group's level-0 map must be at least 8x8");
+        if (groups->frames[k] < 1) return fail("pips_init_gather_groups: every group needs frames >= 1");
+        if (!groups->lvl[k][0]) return fail("pips_init_gather_groups: null level pointer");
+        g.lvl0[k] = static_cast<const float*>(groups->lvl[k][0]);
+        g.H[k] = groups->H[k]; g.W[k] = groups->W[k];
+    }
+    const int warps = B * N;
+    init_gather_groups_kernel<<<(warps * 32 + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
+        g, B, S, N, coords, frame_base, reinterpret_cast<const int4*>(table), ffeat, ffeats);
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail_cuda("pips_init_gather_groups", e);
 }

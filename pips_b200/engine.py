@@ -235,6 +235,30 @@ class Pyramid:
                                                 self.bf16_ptrs, stream), "pips_pyramid_build_nhwc")
 
 
+class GroupPyramids:
+    """One Pyramid per group of feature maps of different sizes (the grouped mode of refine()), and the two
+    pips_groups views of them: fp32 level 0 for pips_init_gather_groups, the levels in ``feat_dtype`` for
+    pips_refine_iter_groups."""
+
+    def __init__(self, shapes, feat_dtype: int, device):
+        if not 1 <= len(shapes) <= L.MAX_GROUPS:
+            raise L.PipsCudaError(f"pips_b200: need 1 to {L.MAX_GROUPS} pyramid groups, got {len(shapes)}")
+        self.shapes = tuple(shapes)
+        self.pyrs = [Pyramid(f, h, w, feat_dtype, device) for f, h, w in shapes]
+        self.c_f32, self.c_lvl = L.Groups(), L.Groups()
+        for c, f32 in ((self.c_f32, True), (self.c_lvl, False)):
+            c.G = len(self.pyrs)
+            for g, p in enumerate(self.pyrs):
+                lv = p.f32 if f32 else p.levels()
+                for l in range(L.LEVELS):
+                    c.lvl[g][l] = L.ptr(lv[l])
+                c.H[g], c.W[g], c.frames[g] = p.H, p.W, p.frames
+
+    def build(self, fmaps2d, stream) -> None:
+        for p, f in zip(self.pyrs, fmaps2d):
+            p.build(f, stream)
+
+
 class RefineEngine:
     """Runs the refinement loop for one model on one device."""
 
@@ -250,6 +274,7 @@ class RefineEngine:
         self._weights_key = None
         self._ws: Optional[Workspace] = None
         self._pyr: Optional[Pyramid] = None
+        self._gpyr: Optional[GroupPyramids] = None
         self._times = None
         self._plans: Dict[tuple, "_GraphPlan"] = {}
         self.use_graph = os.environ.get("PIPS_B200_GRAPH", "1") != "0"
@@ -296,6 +321,14 @@ class RefineEngine:
             self._pyr = Pyramid(frames, H, W, self.feat_dtype, device)
         return self._pyr
 
+    def group_pyramids(self, shapes, device) -> GroupPyramids:
+        """The pyramids of the grouped mode, one per (frames, H, W) of ``shapes``; kept for the next call."""
+        p = self._gpyr
+        if p is None or p.shapes != tuple(shapes) or p.pyrs[0].f32[0].device != device:
+            self._gpyr = None
+            self._gpyr = GroupPyramids(shapes, self.feat_dtype, device)
+        return self._gpyr
+
     def times(self, device) -> torch.Tensor:
         if self._times is None or self._times.device != device:
             # computed on the host exactly as the reference does (nets/pips.py:519); the sin/cos
@@ -311,20 +344,25 @@ class RefineEngine:
         features, ``iters`` refinement iterations, visibility head.  Returns the number of kernels launched.
         ``loss`` (G_hi, G_lo, target (B,S,nc) int32, neg (iters, B*S*nc, n_split), pos (iters, B*S*nc)): also the
         score-map loss terms of every iteration (pips_scoremap_loss); the basis G is built with the pyramid.
-        ``clip`` (B*nc, 2) int32: per-track clip table, read by the ``_clips`` entry points."""
+        ``clip`` (B*nc, 2) int32: per-track clip table, read by the ``_clips`` entry points.  With a GroupPyramids
+        ``pyr`` (and ``fmaps2d`` one tensor per group), ``clip`` is the (B*nc, 4) table of the ``_groups`` entry points."""
         st = self._stream()
         launches = 0
+        grouped = isinstance(pyr, GroupPyramids)
         if build_pyramid:
             with nvtx_range("pips/pyramid"):
                 pyr.build(fmaps2d, st)
-            launches += 4
+            launches += 4 * len(pyr.pyrs) if grouped else 4
             if loss is not None:
                 L.check(lib.pips_scoremap_basis(pyr.f32_ptrs, pyr.frames, H8, W8, L.ptr(loss[0]), L.ptr(loss[1]), st),
                         "pips_scoremap_basis")
                 launches += 1
         c0.copy_(c)
         if feat_init is None:
-            if clip is None:
+            if grouped:
+                L.check(lib.pips_init_gather_groups(C.byref(pyr.c_f32), B, S, nc, L.ptr(c), L.ptr(frame_base), L.ptr(clip),
+                                                    L.ptr(ffeat), L.ptr(ffeats), st), "pips_init_gather_groups")
+            elif clip is None:
                 L.check(lib.pips_init_gather(L.ptr(pyr.f32[0]), B, S, nc, H8, W8, L.ptr(c), L.ptr(frame_base), T,
                                              L.ptr(ffeat), L.ptr(ffeats), st), "pips_init_gather")
             else:
@@ -334,12 +372,13 @@ class RefineEngine:
         else:
             ffeat.copy_(feat_init.reshape(B * nc, LATENT))
             ffeats.copy_(ffeat.unsqueeze(1).expand(-1, S, -1))
-        lvl = pyr.levels()
         prob = L.Problem()
         prob.B, prob.S, prob.N, prob.H, prob.W = B, S, nc, H8, W8
         prob.feat_dtype, prob.precision = self.feat_dtype, self.precision
-        for i in range(L.LEVELS):
-            prob.lvl[i] = L.ptr(lvl[i])
+        if not grouped:                             # the grouped entry points read the levels from pyr.c_lvl
+            lvl = pyr.levels()
+            for i in range(L.LEVELS):
+                prob.lvl[i] = L.ptr(lvl[i])
         prob.times, prob.coords, prob.coords0, prob.ffeats = L.ptr(self.times(c.device)), L.ptr(c), L.ptr(c0), L.ptr(ffeats)
         prob.stride = float(stride)
         prob.frame_base, prob.frames_per_batch = L.ptr(frame_base), T
@@ -366,7 +405,10 @@ class RefineEngine:
                                                L.ptr(neg[it]), L.ptr(pos[it]), st), "pips_scoremap_loss")
                 launches += 1
             with nvtx_range(f"pips/iter{it}"):
-                if clip is None:
+                if grouped:
+                    L.check(lib.pips_refine_iter_groups(C.byref(prob), C.byref(pyr.c_lvl), L.ptr(clip), C.byref(wc),
+                                                        C.byref(ws.c), L.ptr(out[it]), st), "pips_refine_iter_groups")
+                elif clip is None:
                     L.check(lib.pips_refine_iter(C.byref(prob), C.byref(wc), C.byref(ws.c), L.ptr(out[it]), st),
                             "pips_refine_iter")
                 else:
@@ -403,22 +445,45 @@ class RefineEngine:
         is the first frame of track (b,n)'s clip among the B*T frames of fmaps and its number of frames; the track's
         frame_base then counts inside that clip, and its windows replicate the clip's last frame going forward and clamp
         at the clip's frame 0 going backward (pips_corr_gather_clips).  The table is checked here, because the kernels
-        trust it."""
+        trust it.
+        Grouped mode (videos of different frame sizes in one call): ``fmaps`` is a list of G <= 32 tensors
+        (B_g, T_g, 128, H8_g, W8_g), one per group, and ``clip`` (B,N,3) int32 holds (first, count, group): track (b,n)
+        reads its windows in the clip (first, count) among group ``group``'s B_g*T_g frames, as above, with that group's
+        map size (pips_refine_iter_groups).  ``frame_base`` is required; ``reuse_pyramid`` reuses all groups'
+        pyramids."""
         lib = L.load()
-        B, T, Cc, H8, W8 = fmaps.shape
+        grouped = isinstance(fmaps, (list, tuple))
+        if grouped:
+            if frame_base is None or clip is None:
+                raise L.PipsCudaError("pips_b200: feature maps in groups need frame_base and a (B, N, 3) clip table")
+            if heat_sel is not None or peer is not None or loss_target is not None:
+                raise L.PipsCudaError("pips_b200: score maps, losses and sharding do not cover feature maps in groups")
+            shapes = []
+            for g, f in enumerate(fmaps):
+                if not isinstance(f, torch.Tensor) or f.dim() != 5 or f.shape[2] != LATENT or f.dtype != torch.float32:
+                    raise L.PipsCudaError(f"pips_b200: fmaps[{g}] must be (B_g, T_g, 128, H8, W8) fp32, got "
+                                          f"{tuple(getattr(f, 'shape', ()))}")
+                shapes.append((f.shape[0] * f.shape[1], f.shape[3], f.shape[4]))
+            B, T, Cc, H8, W8 = coords.shape[0], 0, LATENT, 0, 0
+            dev = fmaps[0].device
+        else:
+            B, T, Cc, H8, W8 = fmaps.shape
+            dev = fmaps.device
         S = coords.shape[1]
         if S != S_FRAMES or Cc != LATENT or (frame_base is None and T != S):
             raise L.PipsCudaError(f"pips_b200 CUDA path supports S=8, C=128 (got S={S}, T={T}, C={Cc})")
         if frame_base is not None:
-            frame_base = frame_base.to(device=fmaps.device, dtype=torch.int32).contiguous()
+            frame_base = frame_base.to(device=dev, dtype=torch.int32).contiguous()
         N = coords.shape[2]
-        if clip is not None:
-            clip = self._check_clip(clip, frame_base, B, N, B * T, fmaps.device)
-        dev = fmaps.device
+        if grouped:
+            clip = self._check_groups(clip, frame_base, B, N, [f for f, _, _ in shapes], dev)
+        elif clip is not None:
+            clip = self._check_clip(clip, frame_base, B, N, B * T, dev)
         w = self.weights(module)
-        fmaps2d = fmaps.reshape(B * T, Cc, H8, W8)                  # a view for both NCHW and channels-last inputs
-        if not fmaps2d.is_contiguous() and not fmaps2d.permute(0, 2, 3, 1).is_contiguous():
-            fmaps2d = fmaps2d.contiguous()
+        if grouped:
+            fmaps2d = [self._frames2d(f) for f in fmaps]
+        else:
+            fmaps2d = self._frames2d(fmaps)
         chunk = max(1, self.max_seqs // B)
 
         if heat_sel is not None:
@@ -449,7 +514,7 @@ class RefineEngine:
                     on_iter(it, preds[it])
             return preds, vis, ffeat
 
-        pyr = self.pyramid(B * T, H8, W8, dev)
+        pyr = self.group_pyramids(shapes, dev) if grouped else self.pyramid(B * T, H8, W8, dev)
         preds = torch.empty(iters, B, S, N, 2, dtype=torch.float32, device=dev)
         vis = torch.empty(B, S, N, dtype=torch.float32, device=dev)
         ffeat_out = torch.empty(B, N, LATENT, dtype=torch.float32, device=dev)
@@ -498,6 +563,33 @@ class RefineEngine:
         if loss_target is not None:
             loss_out.copy_(_score_map_loss(neg, pos, loss_target, iters, H8 * W8))
         return preds, vis, ffeat_out
+
+    @staticmethod
+    def _frames2d(fmaps: torch.Tensor) -> torch.Tensor:
+        """(B, T, C, H, W) feature maps as (B*T, C, H, W), NCHW- or channels-last-contiguous."""
+        B, T, Cc, H8, W8 = fmaps.shape
+        fmaps2d = fmaps.reshape(B * T, Cc, H8, W8)                  # a view for both NCHW and channels-last inputs
+        if not fmaps2d.is_contiguous() and not fmaps2d.permute(0, 2, 3, 1).is_contiguous():
+            fmaps2d = fmaps2d.contiguous()
+        return fmaps2d
+
+    @staticmethod
+    def _check_groups(table: torch.Tensor, frame_base: torch.Tensor, B: int, N: int, frames, dev) -> torch.Tensor:
+        """The (B,N,3) table of refine()'s grouped mode as the kernels' (B,N,4) int32 {first, count, group, 0} on
+        ``dev``, after checking 0 <= group < G, 1 <= count, 0 <= first and first + count <= that group's frames."""
+        if not isinstance(table, torch.Tensor) or tuple(table.shape) != (B, N, 3) or table.dtype.is_floating_point \
+                or table.dtype.is_complex:
+            raise L.PipsCudaError(f"pips_b200: the group table must be ({B}, {N}, 3) int32, got "
+                                  f"{tuple(getattr(table, 'shape', ()))} {getattr(table, 'dtype', None)}")
+        c = table.to(device=dev, dtype=torch.long)
+        first, count, group = c[..., 0], c[..., 1], c[..., 2]
+        if bool(((group < 0) | (group >= len(frames))).any()):
+            raise L.PipsCudaError(f"pips_b200: group table names a group outside 0..{len(frames) - 1}")
+        held = torch.tensor(frames, dtype=torch.long, device=dev)[group]
+        if bool(((count < 1) | (first < 0) | (first + count > held)).any()):
+            raise L.PipsCudaError("pips_b200: group table outside its group's frames (need count >= 1, first >= 0, "
+                                  "first + count <= the group's frames)")
+        return torch.cat([c, torch.zeros_like(c[..., :1])], dim=-1).to(torch.int32).contiguous()
 
     @staticmethod
     def _check_clip(clip: torch.Tensor, frame_base: Optional[torch.Tensor], B: int, N: int, frames: int,
