@@ -90,19 +90,22 @@ class _Tracks:
         self.rounds = 0
 
 
-def _run_rounds(model, fmaps: torch.Tensor, tr: _Tracks, iters: int, advance: Optional[int] = None, f0: int = 0,
-                ended: bool = True) -> None:
-    """The round loop shared by track_chain, track_queries and TrackStream.  fmaps (1, F, 128, H8, W8) holds frames
-    f0 .. f0+F-1 of the video.  Every round is one refinement call over all runnable tracks, each reading its window
-    through its frame_base rebased to the held frames; rounds repeat until no track is runnable.  A track is runnable
-    while it is inside its clip and, unless the video has ``ended``, its whole window has arrived.  A window past the
-    last held frame replicates that frame, which is the end-of-clip rule once the video has ended.  A track's first
-    window gathers its own feature; later windows carry it (outs[3], chain_demo.py:57).  With a per-track clip
+def _run_rounds(model, fmaps: torch.Tensor, tr: _Tracks, iters: int, advance: Optional[int] = None, f0=0,
+                ended=True, frames: Optional[torch.Tensor] = None) -> None:
+    """The round loop shared by track_chain, track_queries, TrackStream and MultiStream.  fmaps (1, F, 128, H8, W8)
+    holds frames f0 .. f0+F-1 of the video.  Every round is one refinement call over all runnable tracks, each reading
+    its window through its frame_base rebased to the held frames; rounds repeat until no track is runnable.  A track is
+    runnable while it is inside its clip and, unless the video has ``ended``, its whole window has arrived.  A window
+    past the last held frame replicates that frame, which is the end-of-clip rule once the video has ended.  A track's
+    first window gathers its own feature; later windows carry it (outs[3], chain_demo.py:57).  With a per-track clip
     (tr.clip) the refinement calls pass the runnable tracks' rows of it as ``clip``; without one they pass no clip.
     ``fmaps`` may also be a list of such tensors of different map sizes, one per pyramid group, with a 3-column
-    tr.clip and ``ended``."""
+    tr.clip.  Tracks of several streamed videos take the per-track form: ``f0`` (n,) the video frame of the first held
+    frame of each track's video (its clip's frame 0), ``frames`` (n,) the frames that video has delivered and
+    ``ended`` (n,) bool; the scalars stand for every track, with frames = f0 + F."""
     grouped = isinstance(fmaps, (list, tuple))
-    F = None if grouped else fmaps.shape[1]
+    if frames is None and not grouped:
+        frames = f0 + fmaps.shape[1]
     dev = (fmaps[0] if grouped else fmaps).device
     eng = model.engine
     stride = float(model.stride)
@@ -111,14 +114,16 @@ def _run_rounds(model, fmaps: torch.Tensor, tr: _Tracks, iters: int, advance: Op
     built = False                                                                    # the pyramid of fmaps exists
     while True:
         live = ~tr.done
-        if not ended:
-            live &= tr.base0 + tr.cur + (S_WIN - 1) <= f0 + F - 1
+        if not isinstance(ended, bool):
+            live &= ended | (tr.base0 + tr.cur + (S_WIN - 1) <= frames - 1)
+        elif not ended:
+            live &= tr.base0 + tr.cur + (S_WIN - 1) <= frames - 1
         run = live.nonzero().flatten()
         na = run.numel()
         if na == 0:
             return
         c = tr.cur[run]
-        fb = (tr.base0[run] + c - f0).view(1, na).to(torch.int32)
+        fb = (tr.base0[run] + c - (f0[run] if isinstance(f0, torch.Tensor) else f0)).view(1, na).to(torch.int32)
         coords = (tr.pos[run] / stride).view(1, 1, na, 2).repeat(1, S_WIN, 1, 1)    # zero-velocity init, :453
         new = ~tr.started[run]
         cl = None if tr.clip is None else tr.clip[run].view(1, na, tr.clip.shape[1])
@@ -256,26 +261,49 @@ def _batch_clip(rgbs, i: int) -> torch.Tensor:
     return v
 
 
-def _encode_batch(model, clips, chunk: int = 32) -> torch.Tensor:
+def _encode_batch(model, clips, chunk: int = 32, held=None, frames: Optional[int] = None) -> torch.Tensor:
     """The feature maps (1, F, 128, H8, W8) of all frames of ``clips`` ((T_i, 3, H, W) each) back to back, F = sum T_i.
     Frames are encoded once, ``chunk`` at a time across clip boundaries, so the encoder sees one full-chunk shape and one
     tail; each chunk goes to the model's device only when it is encoded.  The maps are written into one channels-last
-    buffer as they come, so the batch's maps are never held twice."""
+    buffer as they come, so the batch's maps are never held twice.
+
+    ``held`` (streaming): per clip, None or the feature maps (1, h_i, 128, H8, W8) of the frames before it, as
+    ``_encode_clip(held=)`` takes them; the buffer then holds [held_0, clip_0, held_1, clip_1, ...], F = sum h_i + T_i,
+    and T_i == 0 is allowed.  ``frames`` (>= F): the buffer's length, its last frames - F frames zero, so that a buffer
+    whose contents vary keeps one shape."""
     dev = next(iter(model.parameters())).device
+    nh = [0 if h is None else h.shape[1] for h in (held or [None] * len(clips))]
     ends = torch.tensor([c.shape[0] for c in clips]).cumsum(0).tolist()
+    first = torch.tensor([0] + [h + c.shape[0] for h, c in zip(nh, clips)]).cumsum(0).tolist()  # clip i's held maps
     F = ends[-1]
     buf = None
+
+    def alloc(h8, w8, dtype):
+        return torch.empty(first[-1] if frames is None else frames, h8, w8, 128, dtype=dtype, device=dev)
+
     for t0 in range(0, F, chunk):
         t1 = min(F, t0 + chunk)
-        parts = []
-        for c, e in zip(clips, ends):
+        parts, dst = [], []
+        for i, (c, e) in enumerate(zip(clips, ends)):
             s = e - c.shape[0]                                                   # the clip holds frames s .. e-1
-            if s < t1 and e > t0:
-                parts.append(c[max(t0 - s, 0):min(t1, e) - s].to(dev))
+            if s < t1 and e > t0 and s < e:
+                a = max(t0 - s, 0)
+                parts.append(c[a:min(t1, e) - s].to(dev))
+                dst.append(first[i] + nh[i] + a)
         f = model.encode(torch.cat(parts).unsqueeze(0))[0]                          # (k, 128, H8, W8)
         if buf is None:
-            buf = torch.empty(F, f.shape[2], f.shape[3], f.shape[1], dtype=f.dtype, device=dev)
-        buf[t0:t1].copy_(f.permute(0, 2, 3, 1))
+            buf = alloc(f.shape[2], f.shape[3], f.dtype)
+        k = 0
+        for p, d in zip(parts, dst):
+            buf[d:d + p.shape[0]].copy_(f[k:k + p.shape[0]].permute(0, 2, 3, 1))
+            k += p.shape[0]
+    for i, h in enumerate(held or []):
+        if h is not None:
+            if buf is None:
+                buf = alloc(h.shape[3], h.shape[4], h.dtype)
+            buf[first[i]:first[i] + nh[i]].copy_(h[0].permute(0, 2, 3, 1))
+    if frames is not None:
+        buf[first[-1]:].zero_()
     return buf.permute(0, 3, 1, 2).unsqueeze(0)
 
 
