@@ -7,8 +7,12 @@
  *   - takes plain device pointers, sizes and a CUDA stream handle (cudaStream_t as void*),
  *   - launches asynchronously on that stream, never allocates device memory, never synchronises,
  *   - returns 0 on success, non-zero on error with the message available from pips_last_error().
- * All tensors are contiguous unless a leading dimension is given.  S (frames per window) must be 8
- * and the feature dimension 128, as in every caller of the reference (nets/pips.py:401,:408).
+ * All tensors are contiguous unless a leading dimension is given.  The feature dimension is 128
+ * (nets/pips.py:408).  S (frames per window, the model's constructor argument, nets/pips.py:401) is 8 for the
+ * entry points without an S of their own and for training and chained tracking; the inference entry points
+ * (pips_refine_iter, pips_corr_gather, pips_init_gather, pips_update, pips_vis_head, pips_heatmap and the _s /
+ * _window siblings) take any 2 <= S <= PIPS_S_MAX.  Sizes that depend on S: the head GEMM's N = PIPS_HEAD_N(S) = 130*S,
+ * padded to PIPS_HEAD_PAD(S) rows (a multiple of 256).
  *
  * Layouts
  *   fmaps        (B*S, 128, H8, W8) fp32 NCHW              output of fnet           nets/pips.py:444-445
@@ -30,6 +34,12 @@ extern "C" {
 #define PIPS_B200_ABI_VERSION 4
 
 enum { PIPS_S = 8, PIPS_C = 128, PIPS_LEVELS = 4, PIPS_RADIUS = 3 };
+enum { PIPS_S_MAX = 16 };   /* longest window of the inference entry points (S = 2..16) */
+#define PIPS_HEAD_N(S) (130 * (S))
+#define PIPS_HEAD_PAD(S) ((130 * (S) + 255) / 256 * 256)
+/* row stride of delta: 130*S rounded up to a multiple of 4 floats (the head GEMM's fp32 epilogue stores 16-byte
+ * vectors); 130*S for even S */
+#define PIPS_DELTA_LD(S) ((130 * (S) + 3) / 4 * 4)
 enum { PIPS_KITCHEN = 519, PIPS_KITCHEN_PAD = 576, PIPS_DIM = 512, PIPS_HIDDEN = 2048, PIPS_DEPTH = 12, PIPS_HEAD = 1040 };
 
 /* storage type of the correlation pyramid */
@@ -190,16 +200,27 @@ int pips_gemm_f32(const float* a, int lda, const float* w, int ldw, int M, int N
 int pips_tokenmix(float* x, int seqs, const float* ln1_w, const float* ln1_b,
                   const float* w1 /* (32,8) */, const float* b1, const float* w2 /* (8,32) */, const float* b2,
                   const float* ln2_w, const float* ln2_b, void* y_hi, void* y_lo, float* y_f32, void* stream);
+/* pips_tokenmix for windows of 2 <= S <= PIPS_S_MAX frames: x (seqs*S, 512), w1 (4S, S), b1 [4S], w2 (S, 4S), b2 [S]
+ * (Conv1d(S,4S,1) -> GELU -> Conv1d(4S,S,1)).  Only the seqs*S rows of x and y are read or written. */
+int pips_tokenmix_s(float* x, int seqs, int S, const float* ln1_w, const float* ln1_b, const float* w1, const float* b1,
+                    const float* w2, const float* b2, const float* ln2_w, const float* ln2_b, void* y_hi, void* y_lo,
+                    float* y_f32, void* stream);
 
 /* the same with the two contractions as wgmma MMAs (channels as the M dimension, bf16x3 folded into K); bf16
  * outputs only.  Selected inside pips_tokenmix by PIPS_B200_TOKENMIX=tc; see csrc/tokenmix_tc.cu for its status. */
 int pips_tokenmix_tc(float* x, int seqs, const float* ln1_w, const float* ln1_b, const float* w1, const float* b1,
                      const float* w2, const float* b2, const float* ln2_w, const float* ln2_b, void* y_hi, void* y_lo,
                      void* stream);
+int pips_tokenmix_tc_s(float* x, int seqs, int S, const float* ln1_w, const float* ln1_b, const float* w1, const float* b1,
+                       const float* w2, const float* b2, const float* ln2_w, const float* ln2_b, void* y_hi, void* y_lo,
+                       void* stream);
 
 /* nets/pips.py:120-121: final LayerNorm(512) then mean over the S rows of each sequence. */
 int pips_ln_pool(const float* x, int seqs, const float* ln_w, const float* ln_b,
                  void* p_hi, void* p_lo, float* p_f32, void* stream);
+/* the same over x (seqs*S, 512), 2 <= S <= PIPS_S_MAX: the mean is the sum of the S normalised rows divided by S */
+int pips_ln_pool_s(const float* x, int seqs, int S, const float* ln_w, const float* ln_b,
+                   void* p_hi, void* p_lo, float* p_f32, void* stream);
 
 /* ---- results written straight into every rank's memory over NVLink (SURVEY.md section 8e: "fusing the coord
  * all-gather into the update epilogue") ----
@@ -228,7 +249,8 @@ int pips_peer_scatter(const float* src, int rows, int cols, float* const* dst, i
 int pips_peer_barrier(int* const* flags, int rank, int n_peers, int epoch, int timeout_ms, void* stream);
 
 /* nets/pips.py:525-539: split delta, ffeats += GELU(Linear(GroupNorm(1,128)(dfeat))), coords += dcoord,
- * re-lock frame 0, emit coords*stride.  delta is (B*N, S*130). */
+ * re-lock frame 0, emit coords*stride.  delta is (B*N, S*130) with row stride PIPS_DELTA_LD(S) (S*130 for even S),
+ * 2 <= S <= PIPS_S_MAX. */
 int pips_update(const float* delta, float* coords, const float* coords0, float* ffeats,
                 const float* gn_w, const float* gn_b, const float* wu /* (128,128) */, const float* bu,
                 float* out_px /* (B,S,N,2) */, float stride, int B, int S, int N, void* stream);
@@ -264,6 +286,9 @@ int pips_scoremap_splits(int H8, int W8);
 int pips_scoremap_basis(const float* const* lvl_f32, int frames, int H8, int W8, void* G_hi, void* G_lo, void* stream);
 int pips_scoremap_loss(const void* G_hi, const void* G_lo, const float* ffeats, int B, int S, int N, int H8, int W8,
                        const int* target, float* neg_part, float* pos_part, void* stream);
+/* pips_scoremap_loss for windows of 2 <= S <= PIPS_S_MAX frames (pips_scoremap_loss itself takes S == 8 only). */
+int pips_scoremap_loss_window(const void* G_hi, const void* G_lo, const float* ffeats, int B, int S, int N, int H8, int W8,
+                              const int* target, float* neg_part, float* pos_part, void* stream);
 
 /* Backward of the score-map loss over `iters` iterations (csrc/scoremap_grad.cu), without the dense score maps.
  * coef (device, 2 floats) holds g/(eps+K) and g/(eps+K(P-1)): g the upstream gradient, K the kept rows times iters,
@@ -384,8 +409,9 @@ typedef struct pips_weights {
     const float* in_b;
     pips_layer_weights layer[PIPS_DEPTH];
     const float *out_ln_w, *out_ln_b;
-    const void *head_w_hi, *head_w_lo;    /* (1280, 512) bf16, rows zero-padded from 1040              */
-    const float* head_w_f32;              /* (1040, 512)                                               */
+    const void *head_w_hi, *head_w_lo;    /* (PIPS_HEAD_PAD(S), 512) bf16, rows zero-padded from 130*S: */
+                                          /* (1280, 512) for S = 8                                     */
+    const float* head_w_f32;              /* (130*S, 512)                                              */
     const float* head_b;
     const float *gn_w, *gn_b, *upd_w, *upd_b, *vis_w, *vis_b;
 } pips_weights;
@@ -398,11 +424,12 @@ typedef struct pips_workspace {
     void *y_hi, *y_lo;    float* y_f32;   /* (rows_alloc, 512)                                         */
     void *h_hi, *h_lo;    float* h_f32;   /* (rows_alloc, 2048)                                        */
     void *p_hi, *p_lo;    float* p_f32;   /* (seqs_alloc, 512)                                         */
-    float* delta;                         /* (seqs_alloc, 1040)                                        */
+    float* delta;                         /* (seqs_alloc, PIPS_DELTA_LD(S)): 130*S used, 1040 at S = 8  */
 } pips_workspace;
 
 typedef struct pips_problem {
-    int B, S, N, H, W;                    /* H, W of pyramid level 0                                   */
+    int B, S, N, H, W;                    /* H, W of pyramid level 0; 2 <= S <= PIPS_S_MAX (8 with a   */
+                                          /* clip table or groups)                                     */
     int feat_dtype, precision;
     const void* lvl[PIPS_LEVELS];
     const float* times;                   /* [S] = linspace(0,S,S)  nets/pips.py:519                   */
@@ -417,6 +444,8 @@ typedef struct pips_problem {
 
 /* DeltaBlock.forward on prepared input rows (nets/pips.py:304-311, mixer :111-123): x0 -> ws->delta */
 int pips_mixer_forward(const pips_weights* w, const pips_workspace* ws, int seqs, int precision, void* stream);
+/* the same for a model of window length 2 <= S <= PIPS_S_MAX: seqs*S mixer rows, delta (seqs, PIPS_DELTA_LD(S)) */
+int pips_mixer_forward_s(const pips_weights* w, const pips_workspace* ws, int seqs, int S, int precision, void* stream);
 
 /* one refinement iteration; out_px receives coords*stride (B,S,N,2) */
 int pips_refine_iter(const pips_problem* p, const pips_weights* w, const pips_workspace* ws,

@@ -16,8 +16,24 @@ LEVELS = 4
 KPAD = 576
 DIM = 512
 HIDDEN = 2048
-HEAD = 1040
+HEAD = 1040                # head width 130*S and its row padding at S = 8
 HEAD_PAD = 1280
+S_MAX = 16                 # PIPS_S_MAX: longest window of the inference entry points
+
+
+def head_n(S: int) -> int:
+    """PIPS_HEAD_N(S): the head's outputs, 130 per frame."""
+    return 130 * S
+
+
+def delta_ld(S: int) -> int:
+    """PIPS_DELTA_LD(S): row stride of the workspace's delta, 130*S rounded up to a multiple of 4."""
+    return (130 * S + 3) // 4 * 4
+
+
+def head_pad(S: int) -> int:
+    """PIPS_HEAD_PAD(S): rows of the packed head weight, 130*S rounded up to whole 256-row tiles."""
+    return (130 * S + 255) // 256 * 256
 
 FEAT_F32, FEAT_BF16 = 0, 1
 PREC_F32, PREC_BF16X3, PREC_BF16 = 0, 1, 2
@@ -97,6 +113,7 @@ _SIGNATURES = {
     "pips_scoremap_splits": (_i, [_i, _i]),
     "pips_scoremap_basis": (_i, [C.POINTER(_p), _i, _i, _i, _p, _p, _p]),
     "pips_scoremap_loss": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "pips_scoremap_loss_window": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "pips_scoremap_grad_feats": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "pips_scoremap_grad_basis": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "pips_scoremap_basis_grad": (_i, [_p, _i, _i, _i, C.POINTER(_p), _p]),
@@ -113,7 +130,10 @@ _SIGNATURES = {
     "pips_gemm_f32": (_i, [_p, _i, _p, _i, _i, _i, _i, _p, _i, _p, _i, _p]),
     "pips_tokenmix": (_i, [_p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "pips_tokenmix_tc": (_i, [_p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "pips_tokenmix_s": (_i, [_p, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "pips_tokenmix_tc_s": (_i, [_p, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "pips_ln_pool": (_i, [_p, _i, _p, _p, _p, _p, _p, _p]),
+    "pips_ln_pool_s": (_i, [_p, _i, _i, _p, _p, _p, _p, _p, _p]),
     "pips_update": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _p, _f, _i, _i, _i, _p]),
     "pips_vis_head": (_i, [_p, _p, _p, _p, _i, _i, _i, _p]),
     "pips_split_bf16": (_i, [_p, _p, _p, C.c_size_t, _p]),
@@ -136,6 +156,7 @@ _SIGNATURES = {
     "pips_inorm_grad": (_i, [_p, _p, _p, _p, _i, _i, _p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _i, _i, _i, _p, _p]),
     "pips_resize_grad": (_i, [_p, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p]),
     "pips_mixer_forward": (_i, [C.POINTER(Weights), C.POINTER(Workspace), _i, _i, _p]),
+    "pips_mixer_forward_s": (_i, [C.POINTER(Weights), C.POINTER(Workspace), _i, _i, _i, _p]),
     "pips_refine_iter": (_i, [C.POINTER(Problem), C.POINTER(Weights), C.POINTER(Workspace), _p, _p]),
     "pips_refine_iter_clips": (_i, [C.POINTER(Problem), _p, C.POINTER(Weights), C.POINTER(Workspace), _p, _p]),
     "pips_refine_iter_groups": (_i, [C.POINTER(Problem), C.POINTER(Groups), _p, C.POINTER(Weights),

@@ -163,6 +163,14 @@ def _run_rounds(model, fmaps: torch.Tensor, tr: _Tracks, iters: int, advance: Op
         tr.rounds += 1
 
 
+def check_window(model, who: str = "pips_b200.chain") -> None:
+    """Chained tracking moves 8-frame windows along the clip (chain_demo.py:52, test_on_badja.py:81): models of
+    another window length are refused before any work."""
+    S = getattr(model, "S", S_WIN)
+    if S != S_WIN:
+        raise ValueError(f"{who}: chained tracking needs a model of S={S_WIN} frames per window; this model has S={S}")
+
+
 @torch.no_grad()
 def track_chain(model, rgbs: torch.Tensor, xy0: torch.Tensor, iters: int = 6, return_rounds: bool = False,
                 advance: Optional[int] = None):
@@ -170,6 +178,7 @@ def track_chain(model, rgbs: torch.Tensor, xy0: torch.Tensor, iters: int = 6, re
     Returns trajs_e (1, T, N, 2).  Equivalent to chain_demo.py:run_model's per-particle loop.
     ``advance`` (2..7): every track moves on by that many frames per round instead of the visibility-driven
     choice -- a data-independent schedule (ceil((T-1)/advance) rounds) for throughput measurements (SURVEY.md 8d)."""
+    check_window(model)
     if advance is not None and not 2 <= int(advance) <= S_WIN - 1:
         raise ValueError("advance must be in 2..7 (the reference's sweep never picks another frame, chain_demo.py:63-76)")
     B, T, C, H, W = rgbs.shape
@@ -222,6 +231,7 @@ def track_queries(model, rgbs: torch.Tensor, queries: torch.Tensor, iters: int =
 
     The clip is encoded once.  Every query is a forward track, and a backward track when t > 0; all tracks advance
     together, one refinement call per round, each reading its own window of the resident pyramid."""
+    check_window(model)
     t = _check_queries(rgbs, queries)
     T = rgbs.shape[1]
     dev = rgbs.device
@@ -339,6 +349,7 @@ def track_queries_batch(model, clips, queries, iters: int = 6, return_rounds: bo
 def _batch_views(model, clips, queries, who: str):
     """The checks track_queries_batch and track_queries_mixed make before any work; returns the clips as
     (T_i, 3, H_i, W_i) views."""
+    check_window(model)
     shard = getattr(model, "_shard", None)
     if shard is not None and shard[1] > 1:
         raise RuntimeError("pips_b200.chain: chained tracking does not cover particle-sharded models")

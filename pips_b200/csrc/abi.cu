@@ -108,10 +108,12 @@ static int dense(int precision, const void* a_hi, const void* a_lo, const float*
                         out_f32, ldo, out_hi, x3 ? out_lo : nullptr, ldh, stream);
 }
 
-extern "C" int pips_mixer_forward(const pips_weights* w, const pips_workspace* ws, int seqs, int precision, void* stream) {
+extern "C" int pips_mixer_forward_s(const pips_weights* w, const pips_workspace* ws, int seqs, int S, int precision,
+                                    void* stream) {
     if (!w || !ws) return fail("pips_mixer_forward: null argument");
     if (seqs <= 0) return fail("pips_mixer_forward: no sequences");
-    const int M = seqs * PIPS_S;
+    if (S < 2 || S > PIPS_S_MAX) return fail("pips_mixer_forward: S must be in 2..16");
+    const int M = seqs * S;
     if (M > ws->rows_alloc || seqs > ws->seqs_alloc) return fail("pips_mixer_forward: workspace too small");
     const bool f32 = precision == PIPS_PREC_F32;
     const bool x3 = precision == PIPS_PREC_BF16X3;
@@ -124,7 +126,7 @@ extern "C" int pips_mixer_forward(const pips_weights* w, const pips_workspace* w
     for (int l = 0; l < PIPS_DEPTH; ++l) {
         const pips_layer_weights* L = &w->layer[l];
         // :117 token mixing (+ the LayerNorm of :118)
-        rc = pips_tokenmix(ws->x, seqs, L->ln1_w, L->ln1_b, L->tok_w1, L->tok_b1, L->tok_w2, L->tok_b2, L->ln2_w, L->ln2_b,
+        rc = pips_tokenmix_s(ws->x, seqs, S, L->ln1_w, L->ln1_b, L->tok_w1, L->tok_b1, L->tok_w2, L->tok_b2, L->ln2_w, L->ln2_b,
                            f32 ? nullptr : ws->y_hi, x3 ? ws->y_lo : nullptr, f32 ? ws->y_f32 : nullptr, stream);
         if (rc) return rc;
         // :118 channel mixing: Linear(512,2048) -> GELU -> Linear(2048,512) -> + x
@@ -138,14 +140,18 @@ extern "C" int pips_mixer_forward(const pips_weights* w, const pips_workspace* w
         if (rc) return rc;
     }
     // :120-121 LayerNorm + mean over S
-    rc = pips_ln_pool(ws->x, seqs, w->out_ln_w, w->out_ln_b, f32 ? nullptr : ws->p_hi, x3 ? ws->p_lo : nullptr,
+    rc = pips_ln_pool_s(ws->x, seqs, S, w->out_ln_w, w->out_ln_b, f32 ? nullptr : ws->p_hi, x3 ? ws->p_lo : nullptr,
                       f32 ? ws->p_f32 : nullptr, stream);
     if (rc) return rc;
-    // :122 Linear(512 -> 1040)
+    // :122 Linear(512 -> 130 S)
     rc = dense(precision, ws->p_hi, ws->p_lo, ws->p_f32, PIPS_DIM, ws->seqs_alloc,
-               w->head_w_hi, w->head_w_lo, w->head_w_f32, PIPS_DIM, 1280,
-               seqs, PIPS_HEAD, PIPS_DIM, w->head_b, PIPS_EPI_BIAS, ws->delta, PIPS_HEAD, nullptr, nullptr, nullptr, 0, stream);
+               w->head_w_hi, w->head_w_lo, w->head_w_f32, PIPS_DIM, PIPS_HEAD_PAD(S),
+               seqs, PIPS_HEAD_N(S), PIPS_DIM, w->head_b, PIPS_EPI_BIAS, ws->delta, PIPS_DELTA_LD(S), nullptr, nullptr, nullptr, 0, stream);
     return rc;
+}
+
+extern "C" int pips_mixer_forward(const pips_weights* w, const pips_workspace* ws, int seqs, int precision, void* stream) {
+    return pips_mixer_forward_s(w, ws, seqs, PIPS_S, precision, stream);
 }
 
 // pips_refine_iter, _clips and _groups: `groups` (with clip as its [B*N][4] table) selects pips_corr_gather_groups
@@ -155,8 +161,8 @@ static int refine_iter_entry(const char* who, const pips_problem* p, const int* 
         snprintf(g_err, sizeof(g_err), "%s: null argument", who);
         return 1;
     }
-    if (p->S != PIPS_S) {
-        snprintf(g_err, sizeof(g_err), "%s: S must be 8", who);
+    if (clip ? p->S != PIPS_S : (p->S < 2 || p->S > PIPS_S_MAX)) {
+        snprintf(g_err, sizeof(g_err), clip ? "%s: S must be 8" : "%s: S must be in 2..16", who);
         return 1;
     }
     if (clip && !p->frame_base) {
@@ -179,7 +185,7 @@ static int refine_iter_entry(const char* who, const pips_problem* p, const int* 
                                      f32 ? nullptr : ws->x0_hi, x3 ? ws->x0_lo : nullptr, f32 ? ws->x0_f32 : nullptr,
                                      PIPS_KITCHEN_PAD, stream);
     if (rc) return rc;
-    rc = pips_mixer_forward(w, ws, seqs, p->precision, stream);
+    rc = pips_mixer_forward_s(w, ws, seqs, p->S, p->precision, stream);
     if (rc) return rc;
     return pips_update_peer(ws->delta, p->coords, p->coords0, p->ffeats, w->gn_w, w->gn_b, w->upd_w, w->upd_b, out_px,
                             p->stride, p->B, p->S, p->N, &p->peer, stream);

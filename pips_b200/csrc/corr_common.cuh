@@ -78,7 +78,7 @@ struct UnitInfo {
     int ox, oy;        // lane l < 4: TMA box origin (first column, first row) of pyramid level l for this unit
 };
 
-// Unit u = (seq, s) with seq = b*N + n (the mixer's row order); S == 8.  Besides the unit's coordinates every lane
+// Unit u = (seq, s) with seq = b*N + n and s < S (the mixer's row order).  Besides the unit's coordinates every lane
 // computes the box origin of ONE pyramid level (lane & 3), so that issuing a TMA box later costs two shuffles instead
 // of a clamp / floor / convert chain executed by lane 0 alone while 31 lanes wait.  Coordinates are clamped in float
 // so that diverged or non-finite tracks cannot overflow the int conversion (beyond +-8 px of the map all taps are zero).
@@ -90,10 +90,10 @@ __device__ __forceinline__ UnitInfo load_unit(const CgArgs& a, int u, int total,
     ui.valid = u < total;
     ui.cx = 0.f; ui.cy = 0.f; ui.frame = 0; ui.group = 0; ui.b = 0; ui.n = 0; ui.s = 0; ui.ox = 0; ui.oy = 0;
     if (ui.valid) {
-        ui.s = u & 7;
-        const int seq = u >> 3;
+        const int seq = u / a.S;
+        ui.s = u - seq * a.S;
         ui.b = seq / a.N; ui.n = seq - ui.b * a.N;
-        const float2 c = *reinterpret_cast<const float2*>(a.coords + ((static_cast<size_t>(ui.b) * 8 + ui.s) * a.N + ui.n) * 2);
+        const float2 c = *reinterpret_cast<const float2*>(a.coords + ((static_cast<size_t>(ui.b) * a.S + ui.s) * a.N + ui.n) * 2);
         ui.cx = c.x; ui.cy = c.y;
         if constexpr (Maps::kGroups) {
             const int4 e = reinterpret_cast<const int4*>(a.clip)[seq];
@@ -102,7 +102,7 @@ __device__ __forceinline__ UnitInfo load_unit(const CgArgs& a, int u, int total,
         } else if (kClips) {
             ui.frame = clip_window_frame(a.clip, seq, a.frame_base[seq], ui.s);
         } else {
-            ui.frame = a.frame_base ? ui.b * a.T + window_frame(a.frame_base[seq], ui.s, a.T) : ui.b * 8 + ui.s;
+            ui.frame = a.frame_base ? ui.b * a.T + window_frame(a.frame_base[seq], ui.s, a.T) : ui.b * a.S + ui.s;
         }
         const int level = threadIdx.x & 3;
         const float sc = 1.0f / static_cast<float>(1 << level);        // coords / 2**i  (nets/pips.py:373), exact

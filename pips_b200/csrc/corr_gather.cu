@@ -71,7 +71,7 @@ corr_gather_kernel(const __grid_constant__ Maps maps, const CgArgs a) {
     const uint32_t bar0 = smem_u32(dots + 64);
     const uint32_t stage0 = smem_u32(stage_buf);
 
-    const int total = a.B * 8 * a.N;
+    const int total = a.B * a.S * a.N;
     const int nwarps = static_cast<int>(gridDim.x) * CG_WARPS;
     int u = static_cast<int>(blockIdx.x) * CG_WARPS + warp;
     if (u >= total) return;                         // whole warp exits together
@@ -166,7 +166,7 @@ corr_gather_kernel(const __grid_constant__ Maps maps, const CgArgs a) {
 
         // feature copy + motion embedding (utils/misc.py:44-69; flows nets/pips.py:518-520)
         {
-            const float2 c0 = *reinterpret_cast<const float2*>(a.coords + (static_cast<size_t>(cur.b) * 8 * a.N + cur.n) * 2);
+            const float2 c0 = *reinterpret_cast<const float2*>(a.coords + (static_cast<size_t>(cur.b) * a.S * a.N + cur.n) * 2);
             const float flow_x = cur.cx - c0.x, flow_y = cur.cy - c0.y, t = a.times[cur.s];
             *reinterpret_cast<float4*>(rowbuf + lane * 4) = q;
             const float div = static_cast<float>(lane) * 31.25f;          // arange(0,64,2) * (1000/64)
@@ -266,7 +266,7 @@ static int corr_gather_entry(const char* who, const void* const* lvl, int feat_d
         return fail(msg);
     };
     if (!lvl || !coords || !ffeats || !times) return err("null pointer");
-    if (S != PIPS_S) return err("S must be 8");
+    if (clip ? S != PIPS_S : (S < 2 || S > PIPS_S_MAX)) return err(clip ? "S must be 8" : "S must be in 2..16");
     if (B <= 0 || N <= 0) return err("empty problem");
     if (H < 8 || W < 8) return err("level-0 map must be at least 8x8");
     if (!x_hi && !x_f32) return err("no output buffer");

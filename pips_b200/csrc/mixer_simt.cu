@@ -1,6 +1,6 @@
 // CUDA-core parts of the DeltaBlock mixer and the state update:
 //   pips_gemm_f32   exact fp32 dense layer (PIPS_PREC_F32; also the on-device cross-check of the wgmma path)
-//   pips_tokenmix   LN -> token-mixing MLP over the S=8 frames -> +x -> LN   (K = 8/32: not a tensor-core shape)
+//   pips_tokenmix   LN -> token-mixing MLP over the S frames -> +x -> LN   (K = S/4S: not a tensor-core shape)
 //   pips_ln_pool    final LN + mean over S
 //   pips_update     GroupNorm/Linear/GELU feature update + coord update + frame-0 lock
 //   pips_vis_head   Linear(128,1)
@@ -60,8 +60,11 @@ gemm_f32_kernel(const float* __restrict__ a, int lda, const float* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------------ token mixing
-__global__ void __launch_bounds__(TM_THREADS, 4)
-tokenmix_kernel(float* __restrict__ x, const float* __restrict__ ln1_w, const float* __restrict__ ln1_b,
+// S <= 8 frames per track, padded to 8 with zero weights (padded frames are neither loaded nor stored: x = 0 there).
+// kFull: S == 8, compiled without the per-frame guards (which need more than 128 registers).
+template <bool kFull>
+__global__ void __launch_bounds__(TM_THREADS, kFull ? 4 : 3)
+tokenmix_kernel(float* __restrict__ x, int s_arg, const float* __restrict__ ln1_w, const float* __restrict__ ln1_b,
                 const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
                 const float* __restrict__ b2, const float* __restrict__ ln2_w, const float* __restrict__ ln2_b,
                 __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, float* y_f32) {
@@ -69,20 +72,23 @@ tokenmix_kernel(float* __restrict__ x, const float* __restrict__ ln1_w, const fl
     // weights duplicated into (w, w) pairs so that one LDS.128 yields two packed FFMA2 operands
     __shared__ __align__(16) float2 s_w1[32 * 8], s_w2t[32 * 8];  // w1[j][s] and w2 transposed to [j][s]
     __shared__ float s_b1[32], s_b2[8];
+    const int S = kFull ? 8 : s_arg;
     pdl_trigger();
     for (int i = threadIdx.x; i < 256; i += TM_THREADS) {
-        s_w1[i] = bcast2(w1[i]);
-        s_w2t[(i & 31) * 8 + (i >> 5)] = bcast2(w2[i]);  // w2 is (8 s, 32 j)
+        const int j = i >> 3, s = i & 7;
+        const bool in = j < 4 * S && s < S;
+        s_w1[i] = bcast2(in ? w1[j * S + s] : 0.f);        // w1 is (4S j, S s)
+        s_w2t[i] = bcast2(in ? w2[s * 4 * S + j] : 0.f);   // w2 is (S s, 4S j)
     }
-    if (threadIdx.x < 32) s_b1[threadIdx.x] = b1[threadIdx.x];
-    if (threadIdx.x < 8) s_b2[threadIdx.x] = b2[threadIdx.x];
+    if (threadIdx.x < 32) s_b1[threadIdx.x] = static_cast<int>(threadIdx.x) < 4 * S ? b1[threadIdx.x] : 0.f;
+    if (threadIdx.x < 8) s_b2[threadIdx.x] = static_cast<int>(threadIdx.x) < S ? b2[threadIdx.x] : 0.f;
 
-    const size_t base = static_cast<size_t>(blockIdx.x) * 8 * 512 + threadIdx.x * 4;
+    const size_t base = static_cast<size_t>(blockIdx.x) * S * 512 + threadIdx.x * 4;
     float xv[8][4], yv[8][4];
     pdl_wait();                                // x comes from the previous kernel; the weights staged above are constants
 #pragma unroll
     for (int s = 0; s < 8; ++s) {
-        const float4 t = *reinterpret_cast<const float4*>(x + base + s * 512);
+        const float4 t = s < S ? *reinterpret_cast<const float4*>(x + base + s * 512) : make_float4(0.f, 0.f, 0.f, 0.f);
         xv[s][0] = t.x; xv[s][1] = t.y; xv[s][2] = t.z; xv[s][3] = t.w;
     }
     const float4 g1 = *reinterpret_cast<const float4*>(ln1_w + threadIdx.x * 4);
@@ -129,40 +135,118 @@ tokenmix_kernel(float* __restrict__ x, const float* __restrict__ ln1_w, const fl
     for (int s = 0; s < 8; ++s) {
 #pragma unroll
         for (int c = 0; c < 4; ++c) xv[s][c] += z[s][c];
-        *reinterpret_cast<float4*>(x + base + s * 512) = make_float4(xv[s][0], xv[s][1], xv[s][2], xv[s][3]);
+        if (s < S) *reinterpret_cast<float4*>(x + base + s * 512) = make_float4(xv[s][0], xv[s][1], xv[s][2], xv[s][3]);
     }
     const float4 g2 = *reinterpret_cast<const float4*>(ln2_w + threadIdx.x * 4);
     const float4 c2 = *reinterpret_cast<const float4*>(ln2_b + threadIdx.x * 4);
     layernorm8(xv, yv, g2, c2, red);
 #pragma unroll
-    for (int s = 0; s < 8; ++s) store_row4(yv[s], base + s * 512, y_hi, y_lo, y_f32);
+    for (int s = 0; s < 8; ++s)
+        if (s < S) store_row4(yv[s], base + s * 512, y_hi, y_lo, y_f32);
 }
 
-// ------------------------------------------------------------------------------------------ final LN + mean over S
-__global__ void __launch_bounds__(TM_THREADS)
-ln_pool_kernel(const float* __restrict__ x, const float* __restrict__ ln_w, const float* __restrict__ ln_b,
-               __nv_bfloat16* p_hi, __nv_bfloat16* p_lo, float* p_f32) {
-    __shared__ float red[4][8];
-    const size_t base = static_cast<size_t>(blockIdx.x) * 8 * 512 + threadIdx.x * 4;
-    float xv[8][4], yv[8][4];
+// 9 <= S <= 16 frames per track, padded to 16: 256 threads, warpgroup w holds frames 8w..8w+7 for both LayerNorms
+// (thread t: channels 4t..4t+3); the token-mixing MLP runs with every thread on 2 channels of all 16 frames, exchanged
+// through shared memory.
+__global__ void __launch_bounds__(2 * TM_THREADS)
+tokenmix16_kernel(float* __restrict__ x, int S, const float* __restrict__ ln1_w, const float* __restrict__ ln1_b,
+                  const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
+                  const float* __restrict__ b2, const float* __restrict__ ln2_w, const float* __restrict__ ln2_b,
+                  __nv_bfloat16* y_hi, __nv_bfloat16* y_lo, float* y_f32) {
+    __shared__ float red[8][8];
+    __shared__ __align__(16) float s_w1[64 * 16], s_w2t[64 * 16];      // w1[j][s] and w2 transposed to [j][s], zero-padded
+    __shared__ float s_b1[64], s_b2[16];
+    __shared__ __align__(16) float xs[16][512];                        // LN1(x), then z, of the whole track
     pdl_trigger();
+    for (int i = threadIdx.x; i < 64 * 16; i += 2 * TM_THREADS) {
+        const int j = i >> 4, s = i & 15;
+        const bool in = j < 4 * S && s < S;
+        s_w1[i] = in ? w1[j * S + s] : 0.f;
+        s_w2t[i] = in ? w2[s * 4 * S + j] : 0.f;
+    }
+    if (threadIdx.x < 64) s_b1[threadIdx.x] = static_cast<int>(threadIdx.x) < 4 * S ? b1[threadIdx.x] : 0.f;
+    if (threadIdx.x < 16) s_b2[threadIdx.x] = static_cast<int>(threadIdx.x) < S ? b2[threadIdx.x] : 0.f;
+
+    const int t = threadIdx.x & 127, f0 = 8 * (threadIdx.x >> 7);
+    const size_t base = static_cast<size_t>(blockIdx.x) * S * 512 + t * 4;
+    float xv[8][4], yv[8][4];
     pdl_wait();
 #pragma unroll
     for (int s = 0; s < 8; ++s) {
-        const float4 t = *reinterpret_cast<const float4*>(x + base + s * 512);
-        xv[s][0] = t.x; xv[s][1] = t.y; xv[s][2] = t.z; xv[s][3] = t.w;
+        const float4 v = f0 + s < S ? *reinterpret_cast<const float4*>(x + base + (f0 + s) * 512) : make_float4(0.f, 0.f, 0.f, 0.f);
+        xv[s][0] = v.x; xv[s][1] = v.y; xv[s][2] = v.z; xv[s][3] = v.w;
     }
+    const float4 g1 = *reinterpret_cast<const float4*>(ln1_w + t * 4);
+    const float4 c1 = *reinterpret_cast<const float4*>(ln1_b + t * 4);
+    layernorm8_wg(xv, yv, g1, c1, red);
+#pragma unroll
+    for (int s = 0; s < 8; ++s) *reinterpret_cast<float4*>(&xs[f0 + s][t * 4]) = make_float4(yv[s][0], yv[s][1], yv[s][2], yv[s][3]);
+    __syncthreads();
+    {
+        const int c = 2 * threadIdx.x;
+        float2 y2[16], z2[16];
+#pragma unroll
+        for (int s = 0; s < 16; ++s) {
+            y2[s] = *reinterpret_cast<const float2*>(&xs[s][c]);
+            z2[s] = bcast2(s_b2[s]);
+        }
+#pragma unroll 2
+        for (int j = 0; j < 64; ++j) {
+            float2 h = bcast2(s_b1[j]);
+#pragma unroll
+            for (int s = 0; s < 16; ++s) h = fma2(bcast2(s_w1[j * 16 + s]), y2[s], h);
+            h = gelu_fast2(h);
+#pragma unroll
+            for (int s = 0; s < 16; ++s) z2[s] = fma2(bcast2(s_w2t[j * 16 + s]), h, z2[s]);
+        }
+        __syncthreads();                                               // every thread has read its y
+#pragma unroll
+        for (int s = 0; s < 16; ++s) *reinterpret_cast<float2*>(&xs[s][c]) = z2[s];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int s = 0; s < 8; ++s) {
+        const float4 z = *reinterpret_cast<const float4*>(&xs[f0 + s][t * 4]);
+        xv[s][0] += z.x; xv[s][1] += z.y; xv[s][2] += z.z; xv[s][3] += z.w;
+        if (f0 + s < S) *reinterpret_cast<float4*>(x + base + (f0 + s) * 512) = make_float4(xv[s][0], xv[s][1], xv[s][2], xv[s][3]);
+    }
+    const float4 g2 = *reinterpret_cast<const float4*>(ln2_w + t * 4);
+    const float4 c2 = *reinterpret_cast<const float4*>(ln2_b + t * 4);
+    layernorm8_wg(xv, yv, g2, c2, red);
+#pragma unroll
+    for (int s = 0; s < 8; ++s)
+        if (f0 + s < S) store_row4(yv[s], base + (f0 + s) * 512, y_hi, y_lo, y_f32);
+}
+
+// ------------------------------------------------------------------------------------------ final LN + mean over S
+// the S rows of a track are normalised 8 at a time and summed in frame order; the mean is that sum / S
+__global__ void __launch_bounds__(TM_THREADS)
+ln_pool_kernel(const float* __restrict__ x, int S, const float* __restrict__ ln_w, const float* __restrict__ ln_b,
+               __nv_bfloat16* p_hi, __nv_bfloat16* p_lo, float* p_f32) {
+    __shared__ float red[4][8];
+    const size_t base = static_cast<size_t>(blockIdx.x) * S * 512 + threadIdx.x * 4;
+    float xv[8][4], yv[8][4];
+    pdl_trigger();
+    pdl_wait();
     const float4 g = *reinterpret_cast<const float4*>(ln_w + threadIdx.x * 4);
     const float4 c = *reinterpret_cast<const float4*>(ln_b + threadIdx.x * 4);
-    layernorm8(xv, yv, g, c, red);
+    float a[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int f0 = 0; f0 < S; f0 += 8) {
+#pragma unroll
+        for (int s = 0; s < 8; ++s) {
+            const float4 t = f0 + s < S ? *reinterpret_cast<const float4*>(x + base + (f0 + s) * 512) : make_float4(0.f, 0.f, 0.f, 0.f);
+            xv[s][0] = t.x; xv[s][1] = t.y; xv[s][2] = t.z; xv[s][3] = t.w;
+        }
+        layernorm8(xv, yv, g, c, red);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+#pragma unroll
+            for (int s = 0; s < 8; ++s)
+                if (f0 + s < S) a[k] += yv[s][k];
+    }
     float m[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        float a = 0.f;
-#pragma unroll
-        for (int s = 0; s < 8; ++s) a += yv[s][k];
-        m[k] = a * 0.125f;
-    }
+    for (int k = 0; k < 4; ++k) m[k] = __fdiv_rn(a[k], static_cast<float>(S));
     store_row4(m, static_cast<size_t>(blockIdx.x) * 512 + threadIdx.x * 4, p_hi, p_lo, p_f32);
 }
 
@@ -195,7 +279,7 @@ update_kernel(const float* __restrict__ delta, float* __restrict__ coords, const
         float sum = 0.f;
         if (r < rows_total) {
             const int seq = r / S, s = r % S;
-            const float* d = delta + static_cast<size_t>(seq) * (S * 130) + s * 130 + 2 + part * 32;
+            const float* d = delta + static_cast<size_t>(seq) * PIPS_DELTA_LD(S) + s * 130 + 2 + part * 32;
 #pragma unroll
             for (int i = 0; i < 32; ++i) { v[i] = d[i]; sum += v[i]; }
         } else {
@@ -220,7 +304,7 @@ update_kernel(const float* __restrict__ delta, float* __restrict__ coords, const
         if (part == 0 && r < rows_total) {
             const int seq = r / S, s = r % S;
             const int b = seq / N, n = seq % N;
-            const float* d = delta + static_cast<size_t>(seq) * (S * 130) + s * 130;
+            const float* d = delta + static_cast<size_t>(seq) * PIPS_DELTA_LD(S) + s * 130;
             const size_t ci = ((static_cast<size_t>(b) * S + s) * N + n) * 2;
             float cx, cy;
             if (s == 0) { cx = coords0[ci]; cy = coords0[ci + 1]; }        // nets/pips.py:535-536
@@ -280,8 +364,9 @@ __global__ void vis_head_kernel(const float* __restrict__ ffeats, const float* _
 
 }  // namespace pips
 
-int tokenmix_tc_launch(float* x, int seqs, const float* ln1_w, const float* ln1_b, const float* w1, const float* b1, const float* w2,
-                       const float* b2, const float* ln2_w, const float* ln2_b, void* y_hi, void* y_lo, cudaStream_t st);   // tokenmix_tc.cu
+int tokenmix_tc_launch(float* x, int seqs, int S, const float* ln1_w, const float* ln1_b, const float* w1, const float* b1,
+                       const float* w2, const float* b2, const float* ln2_w, const float* ln2_b, void* y_hi, void* y_lo,
+                       cudaStream_t st);   // tokenmix_tc.cu
 
 using namespace pips;
 
@@ -301,45 +386,65 @@ extern "C" int pips_gemm_f32(const float* a, int lda, const float* w, int ldw, i
     return 0;
 }
 
-extern "C" int pips_tokenmix(float* x, int seqs, const float* ln1_w, const float* ln1_b, const float* w1, const float* b1,
-                             const float* w2, const float* b2, const float* ln2_w, const float* ln2_b,
-                             void* y_hi, void* y_lo, float* y_f32, void* stream) {
+extern "C" int pips_tokenmix_s(float* x, int seqs, int S, const float* ln1_w, const float* ln1_b, const float* w1,
+                               const float* b1, const float* w2, const float* b2, const float* ln2_w, const float* ln2_b,
+                               void* y_hi, void* y_lo, float* y_f32, void* stream) {
     if (!x || !ln1_w || !ln1_b || !w1 || !b1 || !w2 || !b2 || !ln2_w || !ln2_b) return fail("pips_tokenmix: null pointer");
     if (seqs <= 0) return fail("pips_tokenmix: no sequences");
     if (!y_hi && !y_f32) return fail("pips_tokenmix: no output buffer");
+    if (S < 2 || S > PIPS_S_MAX) return fail("pips_tokenmix: S must be in 2..16");
     {
         // bf16 / bf16x3 precisions run the tensor-core kernel (tokenmix_tc.cu: both contractions as wgmma MMAs,
-        // pipelined over the four channel tiles, 4 CTAs per SM); PIPS_B200_TOKENMIX=simt keeps the CUDA-core kernel below,
-        // which is also the fp32-precision path.
+        // pipelined over the four channel tiles); PIPS_B200_TOKENMIX=simt keeps the CUDA-core kernels below, which are
+        // also the fp32-precision path.
         static int use_tc = -1;
         if (use_tc < 0) {
             const char* e = getenv("PIPS_B200_TOKENMIX");
             use_tc = (e && e[0] == 's') ? 0 : 1;
         }
         if (use_tc && y_hi && !y_f32)
-            return tokenmix_tc_launch(x, seqs, ln1_w, ln1_b, w1, b1, w2, b2, ln2_w, ln2_b, y_hi, y_lo, static_cast<cudaStream_t>(stream));
+            return tokenmix_tc_launch(x, seqs, S, ln1_w, ln1_b, w1, b1, w2, b2, ln2_w, ln2_b, y_hi, y_lo, static_cast<cudaStream_t>(stream));
     }
     {
-        cudaError_t e = launch_pdl(tokenmix_kernel, dim3(seqs), dim3(TM_THREADS), 0, static_cast<cudaStream_t>(stream), x, ln1_w, ln1_b, w1, b1,
-                                   w2, b2, ln2_w, ln2_b, static_cast<__nv_bfloat16*>(y_hi), static_cast<__nv_bfloat16*>(y_lo), y_f32);
+        cudaError_t e = S == 8 ? launch_pdl(tokenmix_kernel<true>, dim3(seqs), dim3(TM_THREADS), 0, static_cast<cudaStream_t>(stream), x, S,
+                                             ln1_w, ln1_b, w1, b1, w2, b2, ln2_w, ln2_b, static_cast<__nv_bfloat16*>(y_hi),
+                                             static_cast<__nv_bfloat16*>(y_lo), y_f32)
+                      : S < 8 ? launch_pdl(tokenmix_kernel<false>, dim3(seqs), dim3(TM_THREADS), 0, static_cast<cudaStream_t>(stream), x, S,
+                                            ln1_w, ln1_b, w1, b1, w2, b2, ln2_w, ln2_b, static_cast<__nv_bfloat16*>(y_hi),
+                                            static_cast<__nv_bfloat16*>(y_lo), y_f32)
+                               : launch_pdl(tokenmix16_kernel, dim3(seqs), dim3(2 * TM_THREADS), 0, static_cast<cudaStream_t>(stream), x,
+                                            S, ln1_w, ln1_b, w1, b1, w2, b2, ln2_w, ln2_b, static_cast<__nv_bfloat16*>(y_hi),
+                                            static_cast<__nv_bfloat16*>(y_lo), y_f32);
         if (e != cudaSuccess) return fail_cuda("pips_tokenmix", e);
     }
     LAUNCH_CHECK("pips_tokenmix");
     return 0;
 }
 
-extern "C" int pips_ln_pool(const float* x, int seqs, const float* ln_w, const float* ln_b, void* p_hi, void* p_lo,
-                            float* p_f32, void* stream) {
+extern "C" int pips_tokenmix(float* x, int seqs, const float* ln1_w, const float* ln1_b, const float* w1, const float* b1,
+                             const float* w2, const float* b2, const float* ln2_w, const float* ln2_b,
+                             void* y_hi, void* y_lo, float* y_f32, void* stream) {
+    return pips_tokenmix_s(x, seqs, PIPS_S, ln1_w, ln1_b, w1, b1, w2, b2, ln2_w, ln2_b, y_hi, y_lo, y_f32, stream);
+}
+
+extern "C" int pips_ln_pool_s(const float* x, int seqs, int S, const float* ln_w, const float* ln_b, void* p_hi, void* p_lo,
+                              float* p_f32, void* stream) {
     if (!x || !ln_w || !ln_b) return fail("pips_ln_pool: null pointer");
     if (seqs <= 0) return fail("pips_ln_pool: no sequences");
     if (!p_hi && !p_f32) return fail("pips_ln_pool: no output buffer");
+    if (S < 2 || S > PIPS_S_MAX) return fail("pips_ln_pool: S must be in 2..16");
     {
-        cudaError_t e = launch_pdl(ln_pool_kernel, dim3(seqs), dim3(TM_THREADS), 0, static_cast<cudaStream_t>(stream), x, ln_w, ln_b,
+        cudaError_t e = launch_pdl(ln_pool_kernel, dim3(seqs), dim3(TM_THREADS), 0, static_cast<cudaStream_t>(stream), x, S, ln_w, ln_b,
                                    static_cast<__nv_bfloat16*>(p_hi), static_cast<__nv_bfloat16*>(p_lo), p_f32);
         if (e != cudaSuccess) return fail_cuda("pips_ln_pool", e);
     }
     LAUNCH_CHECK("pips_ln_pool");
     return 0;
+}
+
+extern "C" int pips_ln_pool(const float* x, int seqs, const float* ln_w, const float* ln_b, void* p_hi, void* p_lo,
+                            float* p_f32, void* stream) {
+    return pips_ln_pool_s(x, seqs, PIPS_S, ln_w, ln_b, p_hi, p_lo, p_f32, stream);
 }
 
 extern "C" int pips_update(const float* delta, float* coords, const float* coords0, float* ffeats, const float* gn_w,
@@ -363,7 +468,7 @@ extern "C" int pips_update_peer(const float* delta, float* coords, const float* 
             if (!po.out[r] || (reinterpret_cast<uintptr_t>(po.out[r]) & 7)) return fail("pips_update: null or misaligned peer result");
     }
     if (!delta || !coords || !coords0 || !ffeats || !gn_w || !gn_b || !wu || !bu || !out_px) return fail("pips_update: null pointer");
-    if (S != PIPS_S) return fail("pips_update: S must be 8");
+    if (S < 2 || S > PIPS_S_MAX) return fail("pips_update: S must be in 2..16");
     if (B <= 0 || N <= 0) return fail("pips_update: empty problem");
     const int rows = B * N * S;
     const size_t smem = (128 * 129 + UP_ROWS * 132) * sizeof(float);

@@ -169,6 +169,16 @@ __device__ __forceinline__ void wgmma_n8(float (&d)[4], uint64_t a_desc, uint64_
         : "l"(a_desc), "l"(b_desc), "r"(accumulate)
         : "memory");
 }
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+        "%8, %9, p, 1, 1, 0, 0;\n\t}"
+        : PIPS_ACC8(d, 0)
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
 __device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"

@@ -223,11 +223,14 @@ extern "C" int pips_scoremap_basis(const float* const* lvl_f32, int frames, int 
     return e == cudaSuccess ? 0 : fail_cuda("pips_scoremap_basis", e);
 }
 
-extern "C" int pips_scoremap_loss(const void* G_hi, const void* G_lo, const float* ffeats, int B, int S, int N, int H8, int W8,
-                                  const int* target, float* neg_part, float* pos_part, void* stream) {
+// pips_scoremap_loss (S == 8) and pips_scoremap_loss_window (2 <= S <= PIPS_S_MAX): the kernel decodes frame = b*S + s
+static int scoremap_loss_entry(int s_min, int s_max, const void* G_hi, const void* G_lo, const float* ffeats, int B, int S, int N,
+                               int H8, int W8, const int* target, float* neg_part, float* pos_part, void* stream) {
     if (!G_hi || !G_lo || !ffeats || !target || !neg_part || !pos_part) return fail("pips_scoremap_loss: null pointer");
     if (B <= 0 || S <= 0 || N <= 0 || H8 <= 0 || W8 <= 0) return fail("pips_scoremap_loss: empty problem");
-    if (S != PIPS_S) return fail("pips_scoremap_loss: S must be 8");
+    if (S < s_min || S > s_max)
+        return fail(s_min == s_max ? "pips_scoremap_loss: S must be 8 (pips_scoremap_loss_window takes 2..16)"
+                                   : "pips_scoremap_loss_window: S must be in 2..16");
     if ((reinterpret_cast<uintptr_t>(G_hi) | reinterpret_cast<uintptr_t>(G_lo) | reinterpret_cast<uintptr_t>(ffeats)) & 15)
         return fail("pips_scoremap_loss: G_hi, G_lo and ffeats must be 16-byte aligned");
     const long long rows = static_cast<long long>(B) * S * H8 * W8;
@@ -248,4 +251,14 @@ extern "C" int pips_scoremap_loss(const void* G_hi, const void* G_lo, const floa
     // a plain launch: the next iteration's PDL-launched kernels cannot start before this one has read ffeats
     return launch_kernel<scoremap_loss_kernel>("pips_scoremap_loss", false, dim3(a.n_split, (N + BM - 1) / BM, B * S), THREADS,
                                                SMEM_BYTES, static_cast<cudaStream_t>(stream), map_hi, map_lo, a);
+}
+
+extern "C" int pips_scoremap_loss(const void* G_hi, const void* G_lo, const float* ffeats, int B, int S, int N, int H8, int W8,
+                                  const int* target, float* neg_part, float* pos_part, void* stream) {
+    return scoremap_loss_entry(PIPS_S, PIPS_S, G_hi, G_lo, ffeats, B, S, N, H8, W8, target, neg_part, pos_part, stream);
+}
+
+extern "C" int pips_scoremap_loss_window(const void* G_hi, const void* G_lo, const float* ffeats, int B, int S, int N, int H8,
+                                         int W8, const int* target, float* neg_part, float* pos_part, void* stream) {
+    return scoremap_loss_entry(2, PIPS_S_MAX, G_hi, G_lo, ffeats, B, S, N, H8, W8, target, neg_part, pos_part, stream);
 }

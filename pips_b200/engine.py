@@ -14,7 +14,8 @@ import torch
 
 from . import _lib as L
 
-S_FRAMES = 8
+S_FRAMES = 8              # the window of training, chaining and the entry points without an S of their own
+S_MIN, S_MAX = 2, 16      # windows of plain inference (PIPS_S_MAX)
 LATENT = 128
 
 # PIPS_B200_NVTX=1: NVTX ranges around the phases of a forward (encoder, pyramid + initial features, every refinement
@@ -54,7 +55,8 @@ class PackedWeights:
 
     Dense-layer weights are kept as nn.Linear stores them ((out, in) == N x K, K-major), split into a
     bf16 (hi, lo) pair for the wgmma path; the first Linear's K is zero-padded 519 -> 576 and the
-    last Linear's N 1040 -> 1280 so that TMA boxes never leave the allocation.
+    last Linear's N 130*S -> round_up(130*S, 256) (1040 -> 1280 at S = 8) so that TMA boxes never leave the
+    allocation.  ``self.S`` is the window length the weights were trained for (the token-mixing Conv1d's channels).
 
     ``self.t`` holds every tensor under a stable name ("layer3.fc1_w_hi", "head_b", ...); the names are
     the fields of ``pips_weights`` / ``pips_layer_weights`` in include/pips_b200.h, which is also the
@@ -71,6 +73,7 @@ class PackedWeights:
             self.device = self.t["gn_w"].device
         if self.device.type != "cuda":
             raise L.PipsCudaError("pips_b200: the refinement path needs the module on a CUDA device")
+        self.S = int(self.t["layer0.tok_b2"].numel()) if "layer0.tok_b2" in self.t else S_FRAMES
         self._bind()
 
     @staticmethod
@@ -89,6 +92,7 @@ class PackedWeights:
         lib = L.load()
         td = "delta_block.to_delta"
         dev = sd[f"{td}.0.weight"].device
+        S = int(sd[f"{td}.1.0.fn.3.weight"].shape[0])              # Conv1d(4S, S, 1): the model's window length
         if dev.type != "cuda":
             raise L.PipsCudaError("pips_b200: the refinement path needs the module on a CUDA device")
         t: Dict[str, torch.Tensor] = {}
@@ -114,9 +118,9 @@ class PackedWeights:
             p, q = f"{td}.{l + 1}", f"layer{l}."
             f32(q + "ln1_w", sd[p + ".0.norm.weight"])
             f32(q + "ln1_b", sd[p + ".0.norm.bias"])
-            f32(q + "tok_w1", sd[p + ".0.fn.0.weight"].reshape(4 * S_FRAMES, S_FRAMES))
+            f32(q + "tok_w1", sd[p + ".0.fn.0.weight"].reshape(4 * S, S))
             f32(q + "tok_b1", sd[p + ".0.fn.0.bias"])
-            f32(q + "tok_w2", sd[p + ".0.fn.3.weight"].reshape(S_FRAMES, 4 * S_FRAMES))
+            f32(q + "tok_w2", sd[p + ".0.fn.3.weight"].reshape(S, 4 * S))
             f32(q + "tok_b2", sd[p + ".0.fn.3.bias"])
             f32(q + "ln2_w", sd[p + ".1.norm.weight"])
             f32(q + "ln2_b", sd[p + ".1.norm.bias"])
@@ -129,8 +133,8 @@ class PackedWeights:
                 split(q + "fc2_wT", sd[p + ".1.fn.3.weight"].t(), keep_f32=False)
         f32("out_ln_w", sd[f"{td}.13.weight"])
         f32("out_ln_b", sd[f"{td}.13.bias"])
-        wh = torch.zeros(L.HEAD_PAD, L.DIM, dtype=torch.float32, device=dev)
-        wh[:L.HEAD] = sd[f"{td}.15.weight"]
+        wh = torch.zeros(L.head_pad(S), L.DIM, dtype=torch.float32, device=dev)
+        wh[:L.head_n(S)] = sd[f"{td}.15.weight"]
         split("head_w", wh)
         f32("head_b", sd[f"{td}.15.bias"])
         if transposed:
@@ -173,11 +177,11 @@ class PackedWeights:
 
 
 class Workspace:
-    """Mixer activations for up to ``seqs`` particle tracks ((b, n) pairs)."""
+    """Mixer activations for up to ``seqs`` particle tracks ((b, n) pairs) of ``S`` frames each."""
 
-    def __init__(self, seqs: int, precision: int, device):
-        self.seqs = seqs
-        rows = _round_up(seqs * S_FRAMES, 256)        # whole 256-row CTA-pair tiles
+    def __init__(self, seqs: int, precision: int, device, S: int = S_FRAMES):
+        self.seqs, self.S = seqs, S
+        rows = _round_up(seqs * S, 256)               # whole 256-row CTA-pair tiles
         sq = _round_up(seqs, 256)
         self.c = L.Workspace()
         self.c.rows_alloc, self.c.seqs_alloc = rows, sq
@@ -189,7 +193,7 @@ class Workspace:
             setattr(self.c, name, L.ptr(t))
 
         alloc("x", rows, L.DIM, torch.float32)
-        alloc("delta", sq, L.HEAD, torch.float32)
+        alloc("delta", sq, L.delta_ld(S), torch.float32)
         if precision == L.PREC_F32:
             alloc("x0_f32", rows, L.KPAD, torch.float32)
             alloc("y_f32", rows, L.DIM, torch.float32)
@@ -275,7 +279,7 @@ class RefineEngine:
         self._ws: Optional[Workspace] = None
         self._pyr: Optional[Pyramid] = None
         self._gpyr: Optional[GroupPyramids] = None
-        self._times = None
+        self._times = None                    # linspace(0, S, S) of the last S asked for
         self._plans: Dict[tuple, "_GraphPlan"] = {}
         self.use_graph = os.environ.get("PIPS_B200_GRAPH", "1") != "0"
         self.launches = 0                       # kernels launched by the last refine() call
@@ -285,8 +289,12 @@ class RefineEngine:
     def _stream() -> int:
         return torch.cuda.current_stream().cuda_stream
 
+    @staticmethod
+    def _pack_key(module):
+        return (getattr(module, "S", S_FRAMES),) + tuple((p.data_ptr(), p._version) for p in module.parameters())
+
     def weights(self, module) -> PackedWeights:
-        key = tuple((p.data_ptr(), p._version) for p in module.parameters())
+        key = self._pack_key(module)
         if self._weights is None or key != self._weights_key:
             self._plans.clear()                                   # captured graphs point into the old pack
             self._weights = PackedWeights(module, self._stream())
@@ -305,13 +313,16 @@ class RefineEngine:
     def adopt_weights(self, module, packed: PackedWeights) -> None:
         """Use an already packed weight set (pips_b200/pack.py) for ``module``'s current parameters."""
         self._plans.clear()
+        S = getattr(module, "S", S_FRAMES)
+        if packed.S != S:
+            raise L.PipsCudaError(f"pips_b200: the weight pack is for windows of S={packed.S} frames, the model's S is {S}")
         self._weights = packed
-        self._weights_key = tuple((p.data_ptr(), p._version) for p in module.parameters())
+        self._weights_key = self._pack_key(module)
 
-    def workspace(self, seqs: int, device) -> Workspace:
-        if self._ws is None or self._ws.seqs < seqs or next(iter(self._ws.keep.values())).device != device:
+    def workspace(self, seqs: int, device, S: int = S_FRAMES) -> Workspace:
+        if self._ws is None or self._ws.seqs < seqs or self._ws.S != S or next(iter(self._ws.keep.values())).device != device:
             self._ws = None
-            self._ws = Workspace(seqs, self.precision, device)
+            self._ws = Workspace(seqs, self.precision, device, S)
         return self._ws
 
     def pyramid(self, frames: int, H: int, W: int, device) -> Pyramid:
@@ -329,11 +340,11 @@ class RefineEngine:
             self._gpyr = GroupPyramids(shapes, self.feat_dtype, device)
         return self._gpyr
 
-    def times(self, device) -> torch.Tensor:
-        if self._times is None or self._times.device != device:
+    def times(self, device, S: int = S_FRAMES) -> torch.Tensor:
+        if self._times is None or self._times.device != device or self._times.numel() != S:
             # computed on the host exactly as the reference does (nets/pips.py:519); the sin/cos
             # embedding multiplies it by up to 968.75, so the fp32 bit pattern matters
-            self._times = torch.linspace(0, S_FRAMES, S_FRAMES, dtype=torch.float32).to(device)
+            self._times = torch.linspace(0, S, S, dtype=torch.float32).to(device)
         return self._times
 
     # ------------------------------------------------------------------ the loop
@@ -379,7 +390,7 @@ class RefineEngine:
             lvl = pyr.levels()
             for i in range(L.LEVELS):
                 prob.lvl[i] = L.ptr(lvl[i])
-        prob.times, prob.coords, prob.coords0, prob.ffeats = L.ptr(self.times(c.device)), L.ptr(c), L.ptr(c0), L.ptr(ffeats)
+        prob.times, prob.coords, prob.coords0, prob.ffeats = L.ptr(self.times(c.device, S)), L.ptr(c), L.ptr(c0), L.ptr(ffeats)
         prob.stride = float(stride)
         prob.frame_base, prob.frames_per_batch = L.ptr(frame_base), T
         if heat is not None:
@@ -401,8 +412,9 @@ class RefineEngine:
                 launches += 1 + (sel.numel() + 31) // 32
             if loss is not None:                    # plain launch: the iteration's kernels wait until ffeats is read
                 g_hi, g_lo, target, neg, pos = loss
-                L.check(lib.pips_scoremap_loss(L.ptr(g_hi), L.ptr(g_lo), L.ptr(ffeats), B, S, nc, H8, W8, L.ptr(target),
-                                               L.ptr(neg[it]), L.ptr(pos[it]), st), "pips_scoremap_loss")
+                L.check(lib.pips_scoremap_loss_window(L.ptr(g_hi), L.ptr(g_lo), L.ptr(ffeats), B, S, nc, H8, W8,
+                                                      L.ptr(target), L.ptr(neg[it]), L.ptr(pos[it]), st),
+                        "pips_scoremap_loss_window")
                 launches += 1
             with nvtx_range(f"pips/iter{it}"):
                 if grouped:
@@ -470,8 +482,13 @@ class RefineEngine:
             B, T, Cc, H8, W8 = fmaps.shape
             dev = fmaps.device
         S = coords.shape[1]
-        if S != S_FRAMES or Cc != LATENT or (frame_base is None and T != S):
-            raise L.PipsCudaError(f"pips_b200 CUDA path supports S=8, C=128 (got S={S}, T={T}, C={Cc})")
+        S_model = getattr(module, "S", S_FRAMES)
+        if not S_MIN <= S <= S_MAX or Cc != LATENT or (frame_base is None and T != S):
+            raise L.PipsCudaError(f"pips_b200 CUDA path supports {S_MIN} <= S <= {S_MAX}, C=128 (got S={S}, T={T}, C={Cc})")
+        if S != S_model:
+            raise L.PipsCudaError(f"pips_b200: the clip's windows have S={S} frames, the model was built for S={S_model}")
+        if S != S_FRAMES and (frame_base is not None or grouped or clip is not None or peer is not None):
+            raise L.PipsCudaError(f"pips_b200: chained windows, clip tables and sharded runs need S=8 (the model's S is {S})")
         if frame_base is not None:
             frame_base = frame_base.to(device=dev, dtype=torch.int32).contiguous()
         N = coords.shape[2]
@@ -484,7 +501,7 @@ class RefineEngine:
             fmaps2d = [self._frames2d(f) for f in fmaps]
         else:
             fmaps2d = self._frames2d(fmaps)
-        chunk = max(1, self.max_seqs // B)
+        chunk = max(1, self.max_seqs * S_FRAMES // S // B)           # tracks per call: max_seqs * 8 mixer rows
 
         if heat_sel is not None:
             if frame_base is not None:
@@ -533,7 +550,7 @@ class RefineEngine:
             ffeat = torch.empty(B * nc, LATENT, dtype=torch.float32, device=dev)
             ffeats = torch.empty(B * nc, S, LATENT, dtype=torch.float32, device=dev)
             fi = None if feat_init is None else (feat_init if whole else feat_init[:, n0:n1])
-            ws = self.workspace(B * nc, dev)
+            ws = self.workspace(B * nc, dev, S)
             out = preds if whole else torch.empty(iters, B, S, nc, 2, dtype=torch.float32, device=dev)
             v = vis if whole else torch.empty(B, S, nc, dtype=torch.float32, device=dev)
             fb = None if frame_base is None else (frame_base if whole else frame_base[:, n0:n1].contiguous())
@@ -644,8 +661,8 @@ class RefineEngine:
         ffeat = torch.empty(B * N, LATENT, dtype=torch.float32, device=dev)
         ffeats = torch.empty(B * N, S, LATENT, dtype=torch.float32, device=dev)
         L.check(lib.pips_init_gather(L.ptr(pyr.f32[0]), B, S, N, H8, W8, L.ptr(c), None, 0, L.ptr(ffeat), L.ptr(ffeats), st))
-        ws = self.workspace(B * N, dev).c
-        times = self.times(dev)
+        ws = self.workspace(B * N, dev, S).c
+        times = self.times(dev, S)
         out = torch.empty(B, S, N, 2, dtype=torch.float32, device=dev)
         seqs, M = B * N, B * N * S
         f32, x3 = self.precision == L.PREC_F32, self.precision == L.PREC_BF16X3
@@ -675,17 +692,17 @@ class RefineEngine:
                   L.DIM, M, L.DIM, L.KPAD, w.in_b, L.EPI_BIAS, ws.x, L.DIM, (None, None, None), 0)
             for l in range(L.DEPTH):
                 lw = w.layer[l]
-                timed("tokenmix", lambda: lib.pips_tokenmix(
-                    ws.x, seqs, lw.ln1_w, lw.ln1_b, lw.tok_w1, lw.tok_b1, lw.tok_w2, lw.tok_b2, lw.ln2_w, lw.ln2_b,
+                timed("tokenmix", lambda: lib.pips_tokenmix_s(
+                    ws.x, seqs, S, lw.ln1_w, lw.ln1_b, lw.tok_w1, lw.tok_b1, lw.tok_w2, lw.tok_b2, lw.ln2_w, lw.ln2_b,
                     None if f32 else ws.y_hi, ws.y_lo if x3 else None, ws.y_f32 if f32 else None, st))
                 dense("gemm_fc1", (ws.y_hi, ws.y_lo, ws.y_f32), L.DIM, ws.rows_alloc, (lw.fc1_w_hi, lw.fc1_w_lo, lw.fc1_w_f32),
                       L.DIM, L.HIDDEN, M, L.HIDDEN, L.DIM, lw.fc1_b, L.EPI_BIAS_GELU, None, 0, (ws.h_hi, ws.h_lo, ws.h_f32), L.HIDDEN)
                 dense("gemm_fc2", (ws.h_hi, ws.h_lo, ws.h_f32), L.HIDDEN, ws.rows_alloc, (lw.fc2_w_hi, lw.fc2_w_lo, lw.fc2_w_f32),
                       L.HIDDEN, L.DIM, M, L.DIM, L.HIDDEN, lw.fc2_b, L.EPI_BIAS_RESID, ws.x, L.DIM, (None, None, None), 0)
-            timed("ln_pool", lambda: lib.pips_ln_pool(ws.x, seqs, w.out_ln_w, w.out_ln_b, None if f32 else ws.p_hi,
+            timed("ln_pool", lambda: lib.pips_ln_pool_s(ws.x, seqs, S, w.out_ln_w, w.out_ln_b, None if f32 else ws.p_hi,
                                                       ws.p_lo if x3 else None, ws.p_f32 if f32 else None, st))
             dense("gemm_head", (ws.p_hi, ws.p_lo, ws.p_f32), L.DIM, ws.seqs_alloc, (w.head_w_hi, w.head_w_lo, w.head_w_f32), L.DIM,
-                  L.HEAD_PAD, seqs, L.HEAD, L.DIM, w.head_b, L.EPI_BIAS, ws.delta, L.HEAD, (None, None, None), 0)
+                  L.head_pad(S), seqs, L.head_n(S), L.DIM, w.head_b, L.EPI_BIAS, ws.delta, L.delta_ld(S), (None, None, None), 0)
             timed("update", lambda: lib.pips_update(ws.delta, L.ptr(c), L.ptr(c0), L.ptr(ffeats), w.gn_w, w.gn_b, w.upd_w, w.upd_b,
                                                     L.ptr(out), float(stride), B, S, N, st))
         torch.cuda.synchronize()
@@ -704,7 +721,7 @@ class _GraphPlan:
         self.peer = peer                              # the captured update kernels store into these slabs
         self.iters = iters
         self.pyr = Pyramid(B * S, H8, W8, eng.feat_dtype, dev)
-        self.ws = Workspace(B * N, eng.precision, dev)
+        self.ws = Workspace(B * N, eng.precision, dev, S)
         f32 = dict(dtype=torch.float32, device=dev)
         self.fmaps_nchw = torch.zeros(B * S, LATENT, H8, W8, **f32)
         self.fmaps_nhwc = self.fmaps_nchw.view(B * S, H8, W8, LATENT).permute(0, 3, 1, 2)   # same storage, NHWC strides
@@ -716,7 +733,7 @@ class _GraphPlan:
         self.preds = torch.zeros(iters, B, S, N, 2, **f32)
         self.vis = torch.zeros(B, S, N, **f32)
         self.shape = (B, N)
-        eng.times(dev)
+        eng.times(dev, S)
 
         self.nhwc = nhwc
         loss = None

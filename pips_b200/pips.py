@@ -7,6 +7,12 @@ per-iteration refinement loop (nets/pips.py:459-559) runs in hand-written sm_90a
 (libpips_b200.so) instead of ~150 eager torch ops per iteration, and the all-pairs correlation
 volume is never materialised.
 
+Window length: plain inference (forward, refine, score_maps) and evaluation with ground truth under no_grad with
+loss_path 'cuda' / 'fused' run models of any S from 2 to 16 on the CUDA path (the token-mixing kernels pad the frame
+axis to 8 or 16).  Training with mixer_path='cuda', chained tracking and streaming (pips_b200.chain /
+pips_b200.stream) and particle-sharded models need S = 8 and raise ValueError otherwise; a clip whose frame count
+differs from the model's S, S = 1 and S > 16 raise PipsCudaError on the CUDA path.
+
 Extra, optional knobs (keyword-only; the reference signature is unchanged):
   precision   'bf16x3' (default; wgmma with hi/lo-split bf16 operands, fp32-class accuracy, meets
               the 1e-3 px parity target), 'bf16' (fast, ~1e-2 px), 'fp32' (CUDA-core GEMMs, exact)
@@ -40,7 +46,8 @@ Extra, optional knobs (keyword-only; the reference signature is unchanged):
               taps by grid_sample, every volume kept until the backward (whose grid_sample adjoint accumulates with
               atomics).  'cuda' is torch_path.local_corr_cuda: pips_corr_gather's 8x8 footprints forward and
               deterministic gather kernels backward, with no volume; volumes are then built only for the dense score
-              maps (loss_path other than 'fused').  CPU tensors, S != 8 and maps under 8x8 keep the torch formulation;
+              maps (loss_path other than 'fused').  CPU tensors, S != 8 (the gradient kernels are written for 8-frame
+              windows) and maps under 8x8 keep the torch formulation;
               plain inference is unaffected.  Independent of the other paths
 Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET, PIPS_B200_LOSSES, PIPS_B200_MIXER,
 PIPS_B200_ENCODER, PIPS_B200_CORR.
@@ -239,6 +246,11 @@ class Pips(nn.Module):
                        and all(t is not None and t.is_cuda for t in (rgbs, trajs_g, vis_g, valids))
                        and not torch.is_grad_enabled() and (self._shard is None or self._shard[1] == 1))
         slow = not cuda_losses and (trajs_g is not None or is_train or save_this)
+        if S != 8 and rgbs.is_cuda:                 # what stays S = 8, refused before the encoder runs
+            if self._shard is not None and self._shard[1] > 1:
+                raise ValueError(f"pips_b200.Pips: particle-sharded models need S=8; this model has S={self.S}")
+            if slow and self.mixer_path == "cuda" and (is_train or torch.is_grad_enabled()):
+                raise ValueError(f"pips_b200.Pips: mixer_path='cuda' trains models of S=8 only; this model has S={self.S}")
         if slow:
             from .torch_path import forward_torch
             return forward_torch(self, xys, rgbs, coords_init=coords_init, feat_init=feat_init, iters=iters,
@@ -251,6 +263,7 @@ class Pips(nn.Module):
         if not rgbs.is_cuda:
             raise RuntimeError("pips_b200.Pips: the inference path is CUDA-only (sm_90a); move the model and "
                                "inputs to a CUDA device. There is no CPU fallback.")
+        self._check_frames(S)
         with torch.no_grad():
             if self._shard is not None and self._shard[1] > 1 and self.shard_fnet and self.fnet_mode == "tc":
                 from .sharding import encode_sharded
@@ -274,6 +287,7 @@ class Pips(nn.Module):
         B, N, D = xys.shape
         assert (D == 2)
         S = rgbs.shape[1]
+        self._check_frames(S)
         fmaps = self.encode(rgbs)
         stride = float(self.stride)
         if coords_init is None:
@@ -288,6 +302,16 @@ class Pips(nn.Module):
                                               heat_sel=sel, heat_out=fcps)
         return fcps, [preds[i] for i in range(iters)], vis_e
 
+    def _check_frames(self, S: int) -> None:
+        """The CUDA path's window: 2 <= S <= 16 frames, as many as the model was built for (its token mixing)."""
+        from ._lib import PipsCudaError
+        if not 2 <= S <= 16:
+            raise PipsCudaError(f"pips_b200 CUDA path supports 2 <= S <= 16 frames per window (got S={S})")
+        if S != self.S:
+            raise PipsCudaError(f"pips_b200: the clip has S={S} frames, the model was built for S={self.S}")
+        if S != 8 and self._shard is not None and self._shard[1] > 1:
+            raise ValueError(f"pips_b200.Pips: particle-sharded models need S=8; this model has S={self.S}")
+
     def refine(self, xys, fmaps, coords_init=None, feat_init=None, iters=3, return_feat=False, trajs_g=None, vis_g=None,
                valids=None):
         """Everything after fnet (nets/pips.py:450-611) given precomputed feature maps.  With ground truth
@@ -296,6 +320,7 @@ class Pips(nn.Module):
         loss comes from pips_scoremap_loss.  Not for particle-sharded models."""
         B, N, _ = xys.shape
         S = fmaps.shape[1]
+        self._check_frames(S)
         stride = float(self.stride)
         loss_target = score = None
         if trajs_g is not None:

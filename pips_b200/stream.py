@@ -58,6 +58,8 @@ def _as_clip(chunk) -> torch.Tensor:
 
 
 def _check_model(model) -> None:
+    from .chain import check_window
+    check_window(model, "pips_b200.stream")
     shard = getattr(model, "_shard", None)
     if shard is not None and shard[1] > 1:
         raise RuntimeError("pips_b200.stream: chained tracking does not cover particle-sharded models")
