@@ -108,6 +108,22 @@ __device__ __forceinline__ uint32_t staged(int row, int byte) {
     return o ^ (((o >> 7) & (PITCH / 16 - 1)) << 4);
 }
 
+// Columns of the output that its tensor map covers.  A TMA store writes whole 16-byte units of a row, so an fp32 map N
+// wide would also write the up to 3 columns past N that share the last unit (the pad columns of a row of delta at odd S,
+// PIPS_DELTA_LD); the fp32 map stops at N rounded down to a multiple of 4, and the epilogue threads store the last N % 4
+// columns themselves (store_tail).
+__host__ __device__ __forceinline__ int tma_cols(const GemmArgs& args) {
+    return bf16_epilogue(args.epilogue) ? args.N : (args.N & ~3);
+}
+
+// fp32 value v of (row, col) when col is one of the last N % 4 columns, which the output map does not cover
+__device__ __forceinline__ void store_tail(const GemmArgs& args, int row, int col, float v) {
+    if (row < args.M && col >= (args.N & ~3) && col < args.N) {
+        float* o = args.out_f32 + static_cast<size_t>(row) * args.ldo + col;
+        *o = args.epilogue == PIPS_EPI_BIAS_RESID ? *o + v : v;                  // as the reduce-add: the bits of (acc + b) + x
+    }
+}
+
 // Epilogue of a warpgroup's 64 x BN accumulator (wgmma fragment layout, ptx.cuh).  `row0` is the first of the
 // warpgroup's rows, `n0` the tile's first column, `staging` its two EPI_BUF_BYTES buffers; `chunk` counts the chunks
 // this warpgroup has staged so far (it picks the buffer and tells when a buffer has had a store issued from it).
@@ -163,12 +179,16 @@ __device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArg
                     }
                 } else {
                     st_shared_f32x2(buf + staged<EPI_COLS * 4>(r + 8 * h, (8 * jj + cq) * 4), f);
+                    if (col + 1 >= (args.N & ~3)) {
+                        store_tail(args, row0 + r + 8 * h, col, f.x);
+                        store_tail(args, row0 + r + 8 * h, col + 1, f.y);
+                    }
                 }
             }
         }
         fence_proxy_async_smem();                                         // make the writes visible to the TMA unit
         named_bar_sync(1 + wg, 128);
-        if (issuer) {
+        if (issuer && col0 < tma_cols(args)) {
             if (gelu) {
                 tma_store_2d(&maps.out_hi, buf, col0, row0);
                 if (args.out_lo) tma_store_2d(&maps.out_lo, buf + EPI_BUF_BYTES / 2, col0, row0);
@@ -232,11 +252,18 @@ __device__ __forceinline__ void epilogue_handoff(const GemmMaps& maps, const Gem
                 if ((t >> 3) + EPI_ROWS * i >= 64) break;
                 const float2 f01 = add2(make_float2(v[i].x, v[i].y), b01), f23 = add2(make_float2(v[i].z, v[i].w), b23);
                 st_shared_f32x4(chunk + staged<EPI_COLS * 4>((t >> 3) + EPI_ROWS * i, 16 * u), make_float4(f01.x, f01.y, f23.x, f23.y));
+                if (col + 3 >= (args.N & ~3)) {
+                    const int row = row0 + (t >> 3) + EPI_ROWS * i;
+                    store_tail(args, row, col, f01.x);
+                    store_tail(args, row, col + 1, f01.y);
+                    store_tail(args, row, col + 2, f23.x);
+                    store_tail(args, row, col + 3, f23.y);
+                }
             }
         }
         fence_proxy_async_smem();                                         // make the writes visible to the TMA unit
         named_bar_sync(1, EPI_THREADS);
-        if (issuer) {
+        if (issuer && col0 < tma_cols(args)) {
             if (gelu) {
                 tma_store_2d(&maps.out_hi, chunk, col0, row0);
                 if (args.out_lo) tma_store_2d(&maps.out_lo, chunk + EPI_BUF_BYTES / 2, col0, row0);
@@ -537,10 +564,11 @@ static bool make_operand_maps(CUtensorMap* map_hi, CUtensorMap* map_lo, const vo
     return encode_tiled_pair(map_hi, map_lo, hi, lo, 2, gdim, gstride, box, estr, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
-// Output tensor {N, M} with row stride `ld` elements; box {EPI_COLS, 64} (one warpgroup's chunk), swizzled like the
-// staging buffer.  The bounds are the problem's, so TMA drops the rows and columns of a tile beyond M and N.
+// Output tensor {tma_cols, M} with row stride `ld` elements; box {EPI_COLS, 64} (one warpgroup's chunk), swizzled like
+// the staging buffer.  The bounds are the problem's, so TMA drops the rows and columns of a tile beyond M and tma_cols.
 static bool make_output_map(CUtensorMap* map, void* ptr, const GemmArgs& args, int ld, bool f32) {
-    cuuint64_t gdim[2] = {static_cast<cuuint64_t>(args.N), static_cast<cuuint64_t>(args.M)};
+    const int cols = tma_cols(args) > 0 ? tma_cols(args) : args.N;        // N < 4: the map is never stored through
+    cuuint64_t gdim[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(args.M)};
     cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ld) * (f32 ? 4 : 2)};
     cuuint32_t box[2] = {static_cast<cuuint32_t>(EPI_COLS), 64};
     cuuint32_t estr[2] = {1, 1};

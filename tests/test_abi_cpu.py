@@ -69,6 +69,69 @@ def test_edge_shapes_are_rejected_by_the_c_abi():
     assert lib.pips_pyramid_build(1, 8, 4, 4, None, None, 0) != 0                            # map too small for 4 levels
 
 
+def test_window_size_macros_match_the_binding():
+    """PIPS_HEAD_N, PIPS_HEAD_PAD and PIPS_DELTA_LD of the header, evaluated from their text, and PIPS_S_MAX equal the
+    sizes pips_b200/_lib.py allocates with, for every window length."""
+    hdr = open(os.path.join(ROOT, "include", "pips_b200.h")).read()
+    assert int(re.search(r"\bPIPS_S_MAX\s*=\s*(\d+)", hdr).group(1)) == L.S_MAX == 16
+    for macro, fn in (("PIPS_HEAD_N", L.head_n), ("PIPS_HEAD_PAD", L.head_pad), ("PIPS_DELTA_LD", L.delta_ld)):
+        body = re.search(rf"^#define {macro}\(S\) (.+)$", hdr, flags=re.M).group(1)
+        assert re.fullmatch(r"[\d\s()+*/S]+", body), body                  # integer arithmetic on S only
+        for S in range(2, L.S_MAX + 1):
+            assert eval(body.replace("/", "//"), {"S": S}) == fn(S), (macro, S)
+    assert [L.delta_ld(S) - L.head_n(S) for S in (5, 8, 9)] == [2, 0, 2]
+
+
+def test_window_entry_points_reject_other_lengths_without_gpu():
+    """S = 1 and S = 17 are refused by every entry point that takes 2 <= S <= 16, before any launch; pips_scoremap_loss
+    takes S = 8 only and names its _window sibling; the clip-table and grouped entry points take S = 8 only."""
+    import ctypes as C
+    lib = L.load()
+    p = C.c_void_p(256)
+    lv = (C.c_void_p * 4)(256, 256, 256, 256)
+    w, ws = L.Weights(), L.Workspace()
+    ws.rows_alloc = ws.seqs_alloc = 1 << 20
+
+    def problem(S):
+        prob = L.Problem()
+        prob.B, prob.S, prob.N, prob.H, prob.W = 1, S, 4, 16, 16
+        prob.frame_base, prob.frames_per_batch = 256, 4
+        return prob
+
+    calls = {
+        "pips_tokenmix": lambda S: lib.pips_tokenmix_s(p, 1, S, *[p] * 8, None, None, p, None),
+        "pips_tokenmix_tc": lambda S: lib.pips_tokenmix_tc_s(p, 1, S, *[p] * 8, p, p, None),
+        "pips_ln_pool": lambda S: lib.pips_ln_pool_s(p, 1, S, p, p, None, None, p, None),
+        "pips_mixer_forward": lambda S: lib.pips_mixer_forward_s(C.byref(w), C.byref(ws), 1, S, L.PREC_F32, None),
+        "pips_scoremap_loss_window": lambda S: lib.pips_scoremap_loss_window(p, p, p, 1, S, 4, 8, 8, p, p, p, None),
+        "pips_update": lambda S: lib.pips_update(*[p] * 9, 8.0, 1, S, 4, None),
+        "pips_corr_gather": lambda S: lib.pips_corr_gather(lv, 0, 1, S, 4, 16, 16, p, p, p, None, 0, p, p, p, 576, None),
+        "pips_refine_iter": lambda S: lib.pips_refine_iter(C.byref(problem(S)), C.byref(w), C.byref(ws), p, None),
+    }
+    for who, call in calls.items():
+        for S in (1, 17):
+            assert call(S) != 0, (who, S)
+            assert lib.pips_last_error() == f"{who}: S must be in 2..16".encode(), (who, S, lib.pips_last_error())
+
+    assert lib.pips_scoremap_loss(p, p, p, 1, 5, 4, 8, 8, p, p, p, None) != 0
+    assert b"S must be 8 (pips_scoremap_loss_window takes 2..16)" in lib.pips_last_error()
+
+    groups = L.Groups()
+    groups.G = 1
+    clips = {
+        "pips_corr_gather_clips": lambda: lib.pips_corr_gather_clips(lv, 0, 1, 9, 4, 16, 16, p, p, p, p, 4, p, p, p, p, 576,
+                                                                     None),
+        "pips_corr_gather_groups": lambda: lib.pips_corr_gather_groups(C.byref(groups), 0, 1, 9, 4, p, p, p, p, p, p, p, p,
+                                                                       576, None),
+        "pips_refine_iter_clips": lambda: lib.pips_refine_iter_clips(C.byref(problem(9)), p, C.byref(w), C.byref(ws), p, None),
+        "pips_refine_iter_groups": lambda: lib.pips_refine_iter_groups(C.byref(problem(9)), C.byref(groups), p, C.byref(w),
+                                                                       C.byref(ws), p, None),
+    }
+    for who, call in clips.items():
+        assert call() != 0, who
+        assert lib.pips_last_error() == f"{who}: S must be 8".encode(), (who, lib.pips_last_error())
+
+
 def test_peer_entry_points_validate_arguments_without_gpu():
     import ctypes as C
     lib = L.load()

@@ -50,6 +50,14 @@ def _st():
     return torch.cuda.current_stream().cuda_stream
 
 
+def _windows(cases, other, windows):
+    """pytest params (*case, S): `cases` at S = 8 under their plain ids, `other` at each of the other window lengths"""
+    tup = lambda c: c if isinstance(c, tuple) else (c,)
+    name = lambda c: "-".join(map(str, tup(c)))
+    return ([pytest.param(*tup(c), S, id=name(c)) for c in cases]
+            + [pytest.param(*tup(c), s, id=f"{name(c)}-S{s}") for s in windows for c in other])
+
+
 def _nan(*shape, dtype=torch.float32):
     return torch.full(shape, float("nan"), dtype=dtype, device=DEV)
 
@@ -132,20 +140,33 @@ def _frame_base(B, N, T, seed):
 def test_init_gather_chained(T):
     """pips_init_gather with frame_base: track (b, n) samples frame b*T + min(frame_base, T-1) at its frame-0 query
     (utils/samp.py: indices clamped, weights not), and broadcasts the row over the S rows of ffeats."""
+    _check_init_gather(T, chained=True)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("S", [2, 5, 16])
+def test_init_gather_window(S):
+    """pips_init_gather without frame_base: track (b, n) samples frame b*S of a pyramid of B*S frames."""
+    _check_init_gather(S, chained=False, S=S)
+
+
+def _check_init_gather(T, chained, S=S):
     lib = L.load()
     torch.manual_seed(102)
     B, N, H, W = 2, 24, 11, 19
     fm = torch.randn(B * T, 128, H, W)
     f32, _ = _pyramid(fm)
-    fb = _frame_base(B, N, T, 103)
+    fb = _frame_base(B, N, T, 103) if chained else torch.zeros(B, N, dtype=torch.int32)
     coords = torch.rand(B, S, N, 2) * torch.tensor([W + 6.0, H + 6.0]) - 3.0
     c0 = coords[:, 0].reshape(-1, 2)
     c0[:6] = torch.tensor([[W - 1.0, H - 1.0], [0.0, 0.0], [W - 1.0, 2.0], [3.0, H - 1.0], [-0.5, H - 0.5], [W + 2.25, -2.75]])
     c0[6:8] = torch.tensor([[5.0, 7.0], [W - 1.5, H - 1.5]])
     coords[:, 0] = c0.reshape(B, N, 2)
     ffeat, ffeats = _nan(B * N + 1, 128), _nan(B * N + 1, S, 128)           # one row past the end stays NaN
-    cd, fbd = coords.to(DEV).contiguous(), fb.to(DEV).contiguous()
-    L.check(lib.pips_init_gather(L.ptr(f32[0]), B, S, N, H, W, L.ptr(cd), L.ptr(fbd), T, L.ptr(ffeat), L.ptr(ffeats), _st()))
+    cd = coords.to(DEV).contiguous()
+    fbd = fb.to(DEV).contiguous() if chained else None
+    L.check(lib.pips_init_gather(L.ptr(f32[0]), B, S, N, H, W, L.ptr(cd), L.ptr(fbd), T if chained else 0, L.ptr(ffeat),
+                                 L.ptr(ffeats), _st()))
     torch.cuda.synchronize()
     frame = (torch.arange(B).view(B, 1) * T + fb.clamp(max=T - 1)).reshape(-1).long()
     img = f32[0].cpu().double()[frame].permute(0, 3, 1, 2)                    # (B*N, 128, H, W): each track's frame
@@ -154,7 +175,8 @@ def test_init_gather_chained(T):
     ref = torch_path.sample_clamped(img, x, y)[:, 0]
     mag = torch_path.sample_clamped(img.abs(), x, y)[:, 0]                    # weights are >= 0
     got = ffeat[:B * N].cpu()
-    _report(f"init_gather T={T}: err / (U sum|terms|)", _ratio(got, ref, mag), C_INIT)
+    tag = f"T={T}" if chained else f"S={S}"
+    _report(f"init_gather {tag}: err / (U sum|terms|)", _ratio(got, ref, mag), C_INIT)
     assert torch.isnan(ffeat[B * N]).all() and torch.isnan(ffeats[B * N]).all()
     assert torch.equal(_bits(ffeats[:B * N]), _bits(got.unsqueeze(1).expand(-1, S, -1)))
 
@@ -237,7 +259,7 @@ def _special_coords(H, W):
     return torch.tensor(pts, dtype=torch.float32), torch.tensor(far, dtype=torch.float32)
 
 
-def _corr_gather(lv, feat, B, N, H, W, coords, ff_rows, times, fb=None, T=0, outs=("f32",), ldx=576):
+def _corr_gather(lv, feat, B, N, H, W, coords, ff_rows, times, fb=None, T=0, outs=("f32",), ldx=576, S=S):
     """One pips_corr_gather call into NaN-filled buffers with one unit's rows of slack; returns {name: (M+8, ldx)}."""
     lib = L.load()
     M = B * N * S
@@ -261,9 +283,12 @@ def _same(a, b):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("feat", ["fp32", "bf16"])
-@pytest.mark.parametrize("H,W,ldx", [(8, 8, 576), (9, 40, 584), (15, 8, 640), (45, 80, 576)])
-def test_corr_gather_against_allpairs(feat, H, W, ldx):
-    B, N = 2, 12
+@pytest.mark.parametrize("H,W,ldx,S", _windows([(8, 8, 576), (9, 40, 584), (15, 8, 640), (45, 80, 576)],
+                                               [(9, 40, 584), (45, 80, 576)], [2, 5, 9, 16]))
+def test_corr_gather_against_allpairs(feat, H, W, ldx, S):
+    """Other window lengths at N = 37: B*S*N is no multiple of a CTA's 8 warps, and at S = 16 it exceeds the warps of
+    the persistent grid (8 per SM), so warps take a second unit."""
+    B, N = 2, 12 if S == 8 else 37
     torch.manual_seed(104)
     f32, bf = _pyramid(torch.randn(B * S, 128, H, W))
     lv = bf if feat == "bf16" else f32
@@ -274,9 +299,9 @@ def test_corr_gather_against_allpairs(feat, H, W, ldx):
     flat[-len(far):] = far
     ff_rows = torch.randn(B * N, S, 128)
     times = po.times_axis(S)
-    out = _corr_gather(lv, feat, B, N, H, W, coords, ff_rows, times, outs=("f32",), ldx=ldx)["f32"]
-    pair = _corr_gather(lv, feat, B, N, H, W, coords, ff_rows, times, outs=("hi", "lo"), ldx=ldx)
-    plain = _corr_gather(lv, feat, B, N, H, W, coords, ff_rows, times, outs=("hi",), ldx=ldx)["hi"]
+    out = _corr_gather(lv, feat, B, N, H, W, coords, ff_rows, times, outs=("f32",), ldx=ldx, S=S)["f32"]
+    pair = _corr_gather(lv, feat, B, N, H, W, coords, ff_rows, times, outs=("hi", "lo"), ldx=ldx, S=S)
+    plain = _corr_gather(lv, feat, B, N, H, W, coords, ff_rows, times, outs=("hi",), ldx=ldx, S=S)["hi"]
     M = B * N * S
     assert torch.isnan(out[M:]).all() and torch.isnan(pair["hi"][M:]).all() and torch.isnan(pair["lo"][M:]).all()
     x = out[:M]
@@ -290,13 +315,14 @@ def test_corr_gather_against_allpairs(feat, H, W, ldx):
     diverged = (coords.abs() >= 1e9).any(-1).permute(0, 2, 1).reshape(M)
     assert (x[diverged, 128:324] == 0).all(), "a diverged track's correlation is not exactly 0"
     r = _ratio(x[:, 128:324], ref, mag)
-    _report(f"corr_gather {feat} {H}x{W}: corr err / (U sum|terms|)", r, C_CORR)
+    tag = f"corr_gather {feat} {H}x{W}" + ("" if S == 8 else f" S={S}")
+    _report(f"{tag}: corr err / (U sum|terms|)", r, C_CORR)
 
     emb, flow = _embed_ref(coords, times)
     flow = flow.reshape(M, 3)
     ok = torch.isfinite(flow).all(-1)
     e_emb = (x[ok, 324:516].double() - emb.reshape(M, 195)[ok, :192]).abs().max().item()
-    _report(f"corr_gather {feat} {H}x{W}: embedding abs err", e_emb, E_EMB)
+    _report(f"{tag}: embedding abs err", e_emb, E_EMB)
     assert _same(x[:, 516:519], flow), "flow / time columns differ"
 
     hi, lo = _split_bf16(x[:, :576])
@@ -306,7 +332,7 @@ def test_corr_gather_against_allpairs(feat, H, W, ldx):
     assert torch.isnan(plain[:, 576:].float()).all()
 
 
-def _chained_case(B, N, H, W, T, seed):
+def _chained_case(B, N, H, W, T, seed, S=S):
     torch.manual_seed(seed)
     fm = torch.randn(B * T, 128, H, W)
     fb = _frame_base(B, N, T, seed + 1)
@@ -347,7 +373,7 @@ def _module(sd):
 
 def _update_ref(sd64, delta, coords, coords0, ff_rows):
     """nets/pips.py:525-536 in fp64: delta (B*N, S, 130) -> new coords (B,S,N,2) and ffeats rows (B*N, S, 128)."""
-    B, _, N, _ = coords.shape
+    B, S, N, _ = coords.shape
     dfeat = delta[:, :, 2:].reshape(-1, 128)
     g = F.group_norm(dfeat, 1, sd64["norm.weight"], sd64["norm.bias"], 1e-5)
     ff = F.gelu(F.linear(g, sd64["ffeat_updater.0.weight"], sd64["ffeat_updater.0.bias"])) + ff_rows.double().reshape(-1, 128)
@@ -357,21 +383,21 @@ def _update_ref(sd64, delta, coords, coords0, ff_rows):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("precision", ["fp32", "bf16x3", "bf16"])
-def test_refine_iter_chained(precision):
+@pytest.mark.parametrize("precision,S", _windows(["fp32", "bf16x3", "bf16"], ["fp32", "bf16x3", "bf16"], [5, 16]))
+def test_refine_iter_chained(precision, S):
     """One pips_refine_iter on chained windows against the loop body (nets/pips.py:499-536) in fp64 on the same
     frames min(frame_base + s, T-1): all-pairs correlation, embedding, the oracle mixer, the state update."""
     lib = L.load()
     B, N, H, W, T, stride = 2, 10, 16, 24, 13, 8.0
-    fm, fb, coords, ff_rows, fidx = _chained_case(B, N, H, W, T, 106)
+    fm, fb, coords, ff_rows, fidx = _chained_case(B, N, H, W, T, 106, S=S)
     coords = torch.rand(B, S, N, 2) * torch.tensor([W - 1.0, H - 1.0])
     coords0 = coords.clone()
     coords0[:, 0] += 0.25                                      # the frame-0 lock must restore coords0, not keep coords
     f32, _ = _pyramid(fm)
-    sd = po.init_state_dict(seed=5, head_scale=1.0)
+    sd = po.init_state_dict(seed=5, head_scale=1.0, S=S)
     w = engine.PackedWeights(_module(sd), _st())
     prec = L.PRECISIONS[precision]
-    ws = engine.Workspace(B * N, prec, DEV)
+    ws = engine.Workspace(B * N, prec, DEV, S=S)
     times = po.times_axis(S).to(DEV)
     cd, c0d = coords.to(DEV).contiguous(), coords0.to(DEV).contiguous()
     fd, fbd = ff_rows.to(DEV).contiguous(), fb.to(DEV).contiguous()
@@ -397,10 +423,10 @@ def test_refine_iter_chained(precision):
     e_ff = (fd.cpu().double() - ff_ref).abs().max().item() / ff_ref.abs().max().item()
     assert torch.equal(_bits(cd), _bits(out / stride)), "coords state and out_px disagree"
     assert torch.equal(_bits(cd[:, 0]), _bits(coords0[:, 0].to(DEV))), "frame 0 is not re-locked to coords0"
-    print(f"refine_iter chained {precision}: max|dpos| {e_px:.3g} px (|delta| max {delta[..., :2].abs().max().item():.3g} px), "
-          f"ffeats rel err {e_ff:.3g}")
-    _report(f"refine_iter chained {precision}: out_px err (px)", e_px, REFINE_PX[precision])
-    _report(f"refine_iter chained {precision}: ffeats rel err", e_ff, REFINE_FF[precision])
+    tag = f"refine_iter chained {precision}" + ("" if S == 8 else f" S={S}")
+    print(f"{tag}: max|dpos| {e_px:.3g} px (|delta| max {delta[..., :2].abs().max().item():.3g} px), ffeats rel err {e_ff:.3g}")
+    _report(f"{tag}: out_px err (px)", e_px, REFINE_PX[precision])
+    _report(f"{tag}: ffeats rel err", e_ff, REFINE_FF[precision])
 
 
 # ------------------------------------------------------------------------------------------------ 4. heat map
@@ -427,8 +453,8 @@ def _heat_ref(levels, q, H8, W8):
 @pytest.mark.gpu
 @pytest.mark.parametrize("feat", ["fp32", "bf16"])
 @pytest.mark.parametrize("n_sel", [1, 33, 70])
-@pytest.mark.parametrize("H8,W8", [(8, 8), (9, 15), (45, 80)])
-def test_heatmap_against_allpairs(H8, W8, n_sel, feat):
+@pytest.mark.parametrize("H8,W8,S", _windows([(8, 8), (9, 15), (45, 80)], [(9, 15), (45, 80)], [2, 5, 12]))
+def test_heatmap_against_allpairs(H8, W8, S, n_sel, feat):
     """n_sel 33 and 70 need two and three heat_corr launches.  Selections repeat and are unsorted.  n_sel 1: identity
     slots with a gap between frames; 33: a slot map with unused slots; 70: both."""
     lib = L.load()
@@ -464,7 +490,8 @@ def test_heatmap_against_allpairs(H8, W8, n_sel, feat):
     assert torch.isnan(frames[~live]).all(), "unused slots / the gap between frames were written"
     assert torch.isnan(got[B * S * stride:]).all()
     g = frames[:, :n_slots * P].reshape(B * S, n_slots, H8, W8)[:, slots]
-    _report(f"heatmap {feat} {H8}x{W8} n_sel={n_sel}: err / (U sum|terms|)", _ratio(g, ref, mag), C_HEAT)
+    tag = f"heatmap {feat} {H8}x{W8} n_sel={n_sel}" + ("" if S == 8 else f" S={S}")
+    _report(f"{tag}: err / (U sum|terms|)", _ratio(g, ref, mag), C_HEAT)
 
 
 # ------------------------------------------------------------------------------------------------ 5. token mixing, pooling
@@ -501,7 +528,7 @@ def _tokenmix_ref(x, lw):
     return xn, y2, xmag, y2mag
 
 
-def _tokenmix_inputs(seqs, offset, seed):
+def _tokenmix_inputs(seqs, offset, seed, S=S):
     g = torch.Generator().manual_seed(seed)
     x = torch.randn(seqs, S, 512, generator=g)
     if offset:
@@ -509,22 +536,27 @@ def _tokenmix_inputs(seqs, offset, seed):
     return x
 
 
-def _tokenmix_seqs():
-    """1, 37, 4 x SMs + 1 (one track more than the wgmma kernel's persistent grid: its prefetch path), 700."""
-    return [1, 37, 4 * torch.cuda.get_device_properties(0).multi_processor_count + 1 if torch.cuda.is_available() else 529, 700]
+def _tokenmix_seqs(S=S):
+    """1, 37, one track more than the wgmma kernel's persistent grid (its next-track prefetch and residual loop), 700.
+    The grid is 4 CTAs per SM at S = 8, 3 at S < 8 (the frame guards need more registers) and 1 above 8 (two
+    warpgroups)."""
+    per_sm = 4 if S == 8 else 3 if S < 8 else 1
+    sms = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else 132
+    return [1, 37, per_sm * sms + 1, 700]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("offset", [False, True])
-@pytest.mark.parametrize("which", range(4))
-def test_tokenmix_outputs(which, offset):
+@pytest.mark.parametrize("which,S", _windows(range(4), range(4), [2, 5, 9, 16]))
+def test_tokenmix_outputs(which, S, offset):
     """pips_tokenmix as (hi, lo) [bf16x3: the wgmma kernel], (hi, NULL) [bf16: the wgmma kernel], f32 [the CUDA-core
-    kernel], and pips_tokenmix_tc itself; x is updated in place.  A sequence past the end stays NaN."""
+    kernel], and pips_tokenmix_tc itself; x is updated in place.  A sequence past the end stays NaN.  Other window
+    lengths go through pips_tokenmix_s and pips_tokenmix_tc_s: P = 8 padded below 8, P = 16 above."""
     lib = L.load()
-    seqs = _tokenmix_seqs()[which]
-    sd = po.init_state_dict(3)
+    seqs = _tokenmix_seqs(S)[which]
+    sd = po.init_state_dict(3, S=S)
     lw = _layer(sd)
-    x = _tokenmix_inputs(seqs, offset, 108 + seqs)
+    x = _tokenmix_inputs(seqs, offset, 108 + seqs, S=S)
     d = {k: v.to(DEV).contiguous() for k, v in lw.items()}
     w = (L.ptr(d["ln1_w"]), L.ptr(d["ln1_b"]), L.ptr(d["w1"]), L.ptr(d["b1"]), L.ptr(d["w2"]), L.ptr(d["b2"]),
          L.ptr(d["ln2_w"]), L.ptr(d["ln2_b"]))
@@ -535,17 +567,19 @@ def test_tokenmix_outputs(which, offset):
         xd[:seqs * S] = x.reshape(-1, 512).to(DEV)
         bufs = {"hi": _nan(R, 512, dtype=torch.bfloat16) if hi else None, "lo": _nan(R, 512, dtype=torch.bfloat16) if lo else None,
                 "f32": _nan(R, 512) if f32 else None}
-        args = (L.ptr(xd), seqs, *w, L.ptr(bufs["hi"]), L.ptr(bufs["lo"]))
-        L.check(fn(*args, _st()) if fn is lib.pips_tokenmix_tc else fn(*args, L.ptr(bufs["f32"]), _st()))
+        args = (L.ptr(xd), seqs, *w, L.ptr(bufs["hi"]), L.ptr(bufs["lo"])) if S == 8 else \
+            (L.ptr(xd), seqs, S, *w, L.ptr(bufs["hi"]), L.ptr(bufs["lo"]))
+        L.check(fn(*args, _st()) if fn in (lib.pips_tokenmix_tc, lib.pips_tokenmix_tc_s) else fn(*args, L.ptr(bufs["f32"]), _st()))
         torch.cuda.synchronize()
         for t in [xd] + [v for v in bufs.values() if v is not None]:
             assert torch.isnan(t[seqs * S:].float()).all(), "a row past seqs was written"
         return xd[:seqs * S].cpu(), {k: v[:seqs * S].cpu() for k, v in bufs.items() if v is not None}
 
-    x_pair, pair = run(lib.pips_tokenmix, True, True, False)
-    x_hi, plain = run(lib.pips_tokenmix, True, False, False)
-    x_f, f32 = run(lib.pips_tokenmix, False, False, True)
-    x_tc, tc = run(lib.pips_tokenmix_tc, True, True, False)
+    tm, tm_tc = (lib.pips_tokenmix, lib.pips_tokenmix_tc) if S == 8 else (lib.pips_tokenmix_s, lib.pips_tokenmix_tc_s)
+    x_pair, pair = run(tm, True, True, False)
+    x_hi, plain = run(tm, True, False, False)
+    x_f, f32 = run(tm, False, False, True)
+    x_tc, tc = run(tm_tc, True, True, False)
     assert torch.equal(_bits(x_pair), _bits(x_tc)) and torch.equal(_bits(pair["hi"]), _bits(tc["hi"])) \
         and torch.equal(_bits(pair["lo"]), _bits(tc["lo"])), "pips_tokenmix (hi, lo) and pips_tokenmix_tc differ"
     assert torch.equal(_bits(x_hi), _bits(x_pair)) and torch.equal(_bits(plain["hi"]), _bits(pair["hi"])), \
@@ -553,7 +587,7 @@ def test_tokenmix_outputs(which, offset):
 
     xn, y2, xmag, y2mag = _tokenmix_ref(x.double(), lw)
     xn, y2, xmag, y2mag = (t.reshape(-1, 512) for t in (xn, y2, xmag, y2mag))
-    tag = f"tokenmix seqs={seqs} offset={offset}"
+    tag = f"tokenmix seqs={seqs} offset={offset}" + ("" if S == 8 else f" S={S}")
     _report(f"{tag} wgmma: x err / (U sum|terms|)", _ratio(x_pair, xn, xmag), C_TM_TC)
     _report(f"{tag} wgmma: hi+lo err / (U sum|terms|)", _ratio(pair["hi"].double() + pair["lo"].double(), y2, y2mag), C_TM_Y)
     _report(f"{tag} fp32: x err / (U sum|terms|)", _ratio(x_f, xn, xmag), C_TM_F32)
@@ -564,19 +598,20 @@ def test_tokenmix_outputs(which, offset):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("offset", [False, True])
-@pytest.mark.parametrize("seqs", [1, 37, 700])
-def test_ln_pool_outputs(seqs, offset):
-    """pips_ln_pool (nets/pips.py:120-121) as (hi, lo), (hi, NULL) and f32."""
+@pytest.mark.parametrize("seqs,S", _windows([1, 37, 700], [1, 37, 700], [2, 5, 9, 16]))
+def test_ln_pool_outputs(seqs, S, offset):
+    """pips_ln_pool (nets/pips.py:120-121) as (hi, lo), (hi, NULL) and f32; pips_ln_pool_s at the other window lengths."""
     lib = L.load()
-    lw = _layer(po.init_state_dict(3))
-    x = _tokenmix_inputs(seqs, offset, 109 + seqs)
+    lw = _layer(po.init_state_dict(3, S=S))
+    x = _tokenmix_inputs(seqs, offset, 109 + seqs, S=S)
     xd = x.reshape(-1, 512).to(DEV).contiguous()
     gw, gb = lw["out_w"].to(DEV), lw["out_b"].to(DEV)
     outs = {}
     for name, parts in (("pair", ("hi", "lo")), ("plain", ("hi",)), ("f32", ("f32",))):
         b = {k: _nan(seqs + 1, 512, dtype=torch.float32 if k == "f32" else torch.bfloat16) if k in parts else None
              for k in ("hi", "lo", "f32")}
-        L.check(lib.pips_ln_pool(L.ptr(xd), seqs, L.ptr(gw), L.ptr(gb), L.ptr(b["hi"]), L.ptr(b["lo"]), L.ptr(b["f32"]), _st()))
+        outs_ = (L.ptr(gw), L.ptr(gb), L.ptr(b["hi"]), L.ptr(b["lo"]), L.ptr(b["f32"]), _st())
+        L.check(lib.pips_ln_pool(L.ptr(xd), seqs, *outs_) if S == 8 else lib.pips_ln_pool_s(L.ptr(xd), seqs, S, *outs_))
         torch.cuda.synchronize()
         for v in b.values():
             if v is not None:
@@ -588,16 +623,17 @@ def test_ln_pool_outputs(seqs, offset):
     mag, _ = _ln_mag(xd64, w64, b64)
     mag = mag.mean(1)
     pf = outs["f32"]["f32"]
-    _report(f"ln_pool seqs={seqs} offset={offset}: f32 err / (U sum|terms|)", _ratio(pf, ref, mag), C_POOL)
+    tag = f"ln_pool seqs={seqs} offset={offset}" + ("" if S == 8 else f" S={S}")
+    _report(f"{tag}: f32 err / (U sum|terms|)", _ratio(pf, ref, mag), C_POOL)
     hi, lo = outs["pair"]["hi"].float(), outs["pair"]["lo"].float()
     rec = ((hi.double() + lo.double()) - pf.double()).abs() / pf.double().abs().clamp_min(1e-30)
-    _report(f"ln_pool seqs={seqs} offset={offset}: hi+lo vs f32, relative", rec.max().item(), 2.0 ** -16)
+    _report(f"{tag}: hi+lo vs f32, relative", rec.max().item(), 2.0 ** -16)
     assert torch.equal(_bits(outs["plain"]["hi"]), _bits(outs["pair"]["hi"])), "(hi, NULL) is not the hi half of (hi, lo)"
 
 
 # ------------------------------------------------------------------------------------------------ 6. update, peers, vis head
 
-def _update_case(B, N, seed):
+def _update_case(B, N, seed, S=S):
     torch.manual_seed(seed)
     delta = torch.randn(B * N, S, 130)
     delta[: (B * N) // 3, :, 2:] += 50.0                     # GroupNorm rows with a large common offset
@@ -609,10 +645,13 @@ def _update_case(B, N, seed):
 
 
 def _upd_call(sd, delta, coords, coords0, ffeats, stride, peer=None):
+    """pips_update_peer with delta in rows of PIPS_DELTA_LD(S) floats, NaN in the pad columns of odd S."""
     lib = L.load()
-    B, _, N, _ = coords.shape
+    B, S, N, _ = coords.shape
     d = lambda t: t.to(DEV).contiguous()
-    dd, cd, c0d, fd = d(delta.reshape(B * N, S * 130)), d(coords), d(coords0), d(ffeats)
+    dd = _nan(B * N, L.delta_ld(S))
+    dd[:, :S * 130] = d(delta.reshape(B * N, S * 130))
+    cd, c0d, fd = d(coords), d(coords0), d(ffeats)
     gw, gb, wu, bu = d(sd["norm.weight"]), d(sd["norm.bias"]), d(sd["ffeat_updater.0.weight"]), d(sd["ffeat_updater.0.bias"])
     out = _nan(B, S, N, 2)
     L.check(lib.pips_update_peer(L.ptr(dd), L.ptr(cd), L.ptr(c0d), L.ptr(fd), L.ptr(gw), L.ptr(gb), L.ptr(wu), L.ptr(bu),
@@ -623,11 +662,23 @@ def _upd_call(sd, delta, coords, coords0, ffeats, stride, peer=None):
 
 @pytest.mark.gpu
 def test_update_and_vis_head_fp64():
+    _check_update_and_vis_head()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("S", [2, 5, 9, 16])
+def test_update_and_vis_head_fp64_window(S):
+    """pips_update reads delta rows PIPS_DELTA_LD(S) floats apart (2 pad columns at odd S); pips_vis_head decodes the
+    warp of (b, s, n) by S."""
+    _check_update_and_vis_head(S)
+
+
+def _check_update_and_vis_head(S=S):
     lib = L.load()
     sd = po.init_state_dict(4)
     sd64 = {k: v.double() for k, v in sd.items()}
     B, N, stride = 2, 45, 4.0
-    delta, coords, coords0, ffeats = _update_case(B, N, 110)
+    delta, coords, coords0, ffeats = _update_case(B, N, 110, S=S)
     c, ff, out = _upd_call(sd, delta, coords, coords0, ffeats, stride)
     # coordinates: one fp32 add (frame 0: the copy of coords0), then one fp32 multiply -- exactly torch's fp32 results
     c_ref = coords + delta[:, :, :2].reshape(B, N, S, 2).permute(0, 2, 1, 3)
@@ -637,7 +688,8 @@ def test_update_and_vis_head_fp64():
     v = delta[:, :, 2:].double().reshape(-1, 128)
     gmag, _ = _ln_mag(v, sd64["norm.weight"], sd64["norm.bias"])                    # GroupNorm(1, 128) = LN over 128
     fmag = gmag @ sd64["ffeat_updater.0.weight"].abs().t() + sd64["ffeat_updater.0.bias"].abs() + ffeats.double().reshape(-1, 128).abs()
-    _report("update: ffeats err / (U sum|terms|)", _ratio(ff.reshape(-1, 128), ff_ref.reshape(-1, 128), fmag), C_UPD)
+    tag = "" if S == 8 else f" S={S}"
+    _report(f"update{tag}: ffeats err / (U sum|terms|)", _ratio(ff.reshape(-1, 128), ff_ref.reshape(-1, 128), fmag), C_UPD)
 
     vis = _nan(B, S, N + 1)
     fd = ff.to(DEV).contiguous()
@@ -648,7 +700,7 @@ def test_update_and_vis_head_fp64():
     v_ref = f64 @ sd64["vis_predictor.0.weight"].reshape(-1) + sd64["vis_predictor.0.bias"]
     v_mag = f64.abs() @ sd64["vis_predictor.0.weight"].abs().reshape(-1) + sd64["vis_predictor.0.bias"].abs()
     got = vis.cpu().view(-1)[:B * S * N].view(B, S, N)
-    _report("vis_head: err / (U sum|terms|)", _ratio(got, v_ref, v_mag), C_VIS)
+    _report(f"vis_head{tag}: err / (U sum|terms|)", _ratio(got, v_ref, v_mag), C_VIS)
     assert torch.isnan(vis.cpu().view(-1)[B * S * N:]).all()
 
 
@@ -698,23 +750,23 @@ def test_peer_scatter_column_offset(cols, cols_total, col_offset):
 _MIXER = {}
 
 
-def _mixer_case():
+def _mixer_case(S=S):
     """Weights with head_scale 1 (the head does not shrink errors), 300 sequences of mixer input and the fp64 oracle
     mixer's delta for them.  Sequences are independent, so the first k rows serve every seqs = k."""
-    if not _MIXER:
-        sd = po.init_state_dict(seed=9, head_scale=1.0)
+    if S not in _MIXER:
+        sd = po.init_state_dict(seed=9, head_scale=1.0, S=S)
         g = torch.Generator().manual_seed(113)
         x0 = torch.randn(300, S, 519, generator=g)
-        _MIXER.update(sd=sd, x0=x0, ref=po.mixer({k: v.double() for k, v in sd.items()}, x0.double()))
-    return _MIXER
+        _MIXER[S] = dict(sd=sd, x0=x0, ref=po.mixer({k: v.double() for k, v in sd.items()}, x0.double()))
+    return _MIXER[S]
 
 
 _WS_ROWS = {"x0": "M", "x": "M", "y": "M", "h": "M", "p": "seqs", "delta": "seqs"}
 
 
-def _mixer_run(w, ws, x0, seqs, prec, tail):
+def _mixer_run(w, ws, x0, seqs, prec, tail, S=S):
     """Fill the workspace's live rows with x0 and every row at or beyond M (beyond seqs for p / delta) with `tail`,
-    run pips_mixer_forward, return delta (all rows)."""
+    run pips_mixer_forward (pips_mixer_forward_s at S != 8), return delta (all rows, PIPS_DELTA_LD(S) columns)."""
     lib = L.load()
     M = seqs * S
     for name, t in ws.keep.items():
@@ -732,44 +784,54 @@ def _mixer_run(w, ws, x0, seqs, prec, tail):
         ws.keep["x0_hi"][:M, :519] = hi
         if prec == L.PREC_BF16X3:
             ws.keep["x0_lo"][:M, :519] = lo
-    L.check(lib.pips_mixer_forward(C.byref(w.c), C.byref(ws.c), seqs, prec, _st()), "pips_mixer_forward")
+    if S == 8:
+        L.check(lib.pips_mixer_forward(C.byref(w.c), C.byref(ws.c), seqs, prec, _st()), "pips_mixer_forward")
+    else:
+        L.check(lib.pips_mixer_forward_s(C.byref(w.c), C.byref(ws.c), seqs, S, prec, _st()), "pips_mixer_forward_s")
     torch.cuda.synchronize()
     return ws.keep["delta"].cpu()
 
 
+_PRECISIONS = ["fp32", "bf16x3", "bf16"]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("precision", ["fp32", "bf16x3", "bf16"])
-def test_mixer_forward_against_fp64(precision):
+@pytest.mark.parametrize("precision,S", _windows(_PRECISIONS, _PRECISIONS, [2, 5, 9, 16]))
+def test_mixer_forward_against_fp64(precision, S):
     """pips_mixer_forward (1 + 12 x 3 + 1 dense layers, token mixing, pooling) against the oracle mixer in fp64, at
-    seqs 1, 37, 300; error relative to max|delta|."""
-    case = _mixer_case()
+    seqs 1, 37, 300; error relative to max|delta|.  At odd S the 2 pad columns of every delta row stay NaN."""
+    case = _mixer_case(S)
     prec = L.PRECISIONS[precision]
     w = engine.PackedWeights(_module(case["sd"]), _st())
-    ws = engine.Workspace(300, prec, DEV)
+    ws = engine.Workspace(300, prec, DEV, S=S)
+    n = L.head_n(S)
     for seqs in (1, 37, 300):
-        d = _mixer_run(w, ws, case["x0"], seqs, prec, 0.0)
+        d = _mixer_run(w, ws, case["x0"], seqs, prec, 0.0, S=S)
         ref = case["ref"][:seqs]
-        rel = (d[:seqs].double() - ref).abs().max().item() / ref.abs().max().item()
-        _report(f"mixer {precision} seqs={seqs}: max|err| / max|delta| (max|delta| {ref.abs().max().item():.3g})", rel,
-                MIXER_REL[precision])
+        assert torch.isnan(d[:seqs, n:]).all(), "pad columns of delta were written"
+        rel = (d[:seqs, :n].double() - ref).abs().max().item() / ref.abs().max().item()
+        tag = f"mixer {precision} seqs={seqs}" + ("" if S == 8 else f" S={S}")
+        _report(f"{tag}: max|err| / max|delta| (max|delta| {ref.abs().max().item():.3g})", rel, MIXER_REL[precision])
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("precision", ["fp32", "bf16x3", "bf16"])
-def test_mixer_forward_tails_and_prefix(precision):
+@pytest.mark.parametrize("precision,S", _windows(_PRECISIONS, _PRECISIONS, [2, 5, 9, 16]))
+def test_mixer_forward_tails_and_prefix(precision, S):
     """Rows past M (past seqs for p / delta) hold stale data when a workspace is reused for a smaller chunk: NaN there
     must not reach a live row, and delta rows >= seqs must not be written.  A sequence's delta must not depend on how
     many other sequences share the call (particle chunking relies on it)."""
-    case = _mixer_case()
+    case = _mixer_case(S)
     prec = L.PRECISIONS[precision]
     w = engine.PackedWeights(_module(case["sd"]), _st())
-    ws = engine.Workspace(300, prec, DEV)
-    zero = _mixer_run(w, ws, case["x0"], 37, prec, 0.0)
-    poisoned = _mixer_run(w, ws, case["x0"], 37, prec, float("nan"))
+    ws = engine.Workspace(300, prec, DEV, S=S)
+    n = L.head_n(S)
+    zero = _mixer_run(w, ws, case["x0"], 37, prec, 0.0, S=S)
+    poisoned = _mixer_run(w, ws, case["x0"], 37, prec, float("nan"), S=S)
     assert torch.equal(_bits(poisoned[:37]), _bits(zero[:37])), "stale rows past M changed live rows"
     assert torch.isnan(poisoned[37:]).all(), "delta rows >= seqs were written"
-    assert not torch.isnan(zero[:37]).any()
-    full = _mixer_run(w, ws, case["x0"], 300, prec, 0.0)
+    assert not torch.isnan(zero[:37, :n]).any()
+    assert torch.isnan(zero[:37, n:]).all() and torch.isnan(poisoned[:37, n:]).all(), "pad columns of delta were written"
+    full = _mixer_run(w, ws, case["x0"], 300, prec, 0.0, S=S)
     assert torch.equal(_bits(full[:37]), _bits(zero[:37])), "delta of the first 37 sequences depends on seqs"
 
 

@@ -60,10 +60,19 @@ C_DG = 512.0          # pips_scoremap_grad_basis on randn (measured 177)
 CASES = [(8, 8, 1, 1), (8, 9, 63, 2), (9, 15, 64, 1), (15, 8, 65, 2), (16, 32, 129, 1), (23, 23, 300, 2),
          (45, 80, 65, 1), (48, 64, 129, 2)]
 RANDN_CASES = [(9, 15, 129, 1), (23, 23, 65, 2), (45, 80, 300, 1), (48, 64, 129, 2)]
+# other window lengths (pips_scoremap_loss_window), all with B = 2 so that a wrong b*S frame stride shows
+WINDOWS = [2, 5, 12, 16]
+WINDOW_CASES = [CASES[1], CASES[5], CASES[7]]
 
 
 def _ids(cases):
     return [f"{h}x{w}-N{n}-B{b}" for h, w, n, b in cases]
+
+
+def _windows(cases, other, windows):
+    """pytest params (H8, W8, N, B, S): `cases` at S = 8 under their plain ids, `other` at each of `windows`"""
+    return ([pytest.param(*c, S, id=i) for c, i in zip(cases, _ids(cases))]
+            + [pytest.param(*c, s, id=f"{i}-S{s}") for s in windows for c, i in zip(other, _ids(other))])
 
 
 # ------------------------------------------------------------------------------------------------ problems
@@ -78,10 +87,11 @@ class Problem(NamedTuple):
     f_hi: torch.Tensor        # (I, frames, N, C) bf16; the fp32 ffeats are hi + lo
     f_lo: torch.Tensor
     target: torch.Tensor      # (frames, N) int32: pixel, or -1
+    S: int = S                # window length: frame b*S + s of the basis serves row ((b N + n), s)
 
     @property
     def frames(self):
-        return self.B * S
+        return self.B * self.S
 
     @property
     def P(self):
@@ -127,7 +137,7 @@ def _targets(P, N, frames, strong, g):
     return target
 
 
-def exact_problem(H8, W8, N, B, I, seed):
+def exact_problem(H8, W8, N, B, I, seed, S=S):
     """the tail operands of the module docstring, on the host"""
     g = torch.Generator().manual_seed(seed)
     frames, P = B * S, H8 * W8
@@ -145,10 +155,10 @@ def exact_problem(H8, W8, N, B, I, seed):
     f_hi[..., :MAIN] *= -tau * u[:MAIN]
     _, f_lo = Spec(0, 1).draw((I, frames, N, C), g)
     return Problem(H8, W8, N, B, g_hi.to(torch.bfloat16), g_lo, f_hi.to(torch.bfloat16), f_lo,
-                   _targets(P, N, frames, strong, g))
+                   _targets(P, N, frames, strong, g), S)
 
 
-def randn_problem(H8, W8, N, B, I, seed):
+def randn_problem(H8, W8, N, B, I, seed, S=S):
     """randn G and F scaled so that the scores are about N(0, 4^2): in the sigmoid's live range"""
     g = torch.Generator().manual_seed(seed)
     frames, P = B * S, H8 * W8
@@ -158,7 +168,7 @@ def randn_problem(H8, W8, N, B, I, seed):
     target = torch.randint(0, P, (frames, N), generator=g, dtype=torch.int32)
     target[torch.rand(frames, N, generator=g) < 0.2] = -1
     return Problem(H8, W8, N, B, g_hi, (G - g_hi.float()).to(torch.bfloat16), f_hi, (Fv - f_hi.float()).to(torch.bfloat16),
-                   target)
+                   target, S)
 
 
 # ------------------------------------------------------------------------------------------------ fp64 references
@@ -321,7 +331,7 @@ def _slack_ok(whole, n):
     return bool(torch.isnan(whole[n:]).all())
 
 
-def _rows_layout(f):
+def _rows_layout(f, S=S):
     """(frames, N, C) ffeats of one iteration -> pips_scoremap_loss's ((b N + n), s, c)"""
     frames, N, _ = f.shape
     return f.view(frames // S, S, N, C).permute(0, 2, 1, 3).contiguous()
@@ -330,9 +340,12 @@ def _rows_layout(f):
 def run_loss(p, i):
     neg, neg_w = _buf(p.frames * p.N, p.n_split)
     pos, pos_w = _buf(p.frames * p.N)
-    ff = _rows_layout(p.f[i])
-    L.check(L.load().pips_scoremap_loss(L.ptr(p.g_hi), L.ptr(p.g_lo), L.ptr(ff), p.B, S, p.N, p.H8, p.W8, L.ptr(p.target),
-                                        L.ptr(neg), L.ptr(pos), _st()), "pips_scoremap_loss")
+    ff = _rows_layout(p.f[i], p.S)
+    lib = L.load()
+    fn, name = (lib.pips_scoremap_loss, "pips_scoremap_loss") if p.S == 8 else \
+        (lib.pips_scoremap_loss_window, "pips_scoremap_loss_window")
+    L.check(fn(L.ptr(p.g_hi), L.ptr(p.g_lo), L.ptr(ff), p.B, p.S, p.N, p.H8, p.W8, L.ptr(p.target), L.ptr(neg), L.ptr(pos),
+               _st()), name)
     torch.cuda.synchronize()
     return neg, pos, _slack_ok(neg_w, neg.numel()) and _slack_ok(pos_w, pos.numel())
 
@@ -353,10 +366,11 @@ def run_grads(p, coef):
 # ------------------------------------------------------------------------------------------------ 3. the loss, exact
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("H8,W8,N,B", CASES, ids=_ids(CASES))
-def test_scoremap_loss_exact(H8, W8, N, B):
-    """neg_part per (row, split) and pos_part bit-equal to the sums of the tail scores; rows without a target hold 0"""
-    p = exact_problem(H8, W8, N, B, I=2, seed=H8 * W8 + N + B).to(DEV)
+@pytest.mark.parametrize("H8,W8,N,B,S", _windows(CASES, WINDOW_CASES, WINDOWS))
+def test_scoremap_loss_exact(H8, W8, N, B, S):
+    """neg_part per (row, split) and pos_part bit-equal to the sums of the tail scores; rows without a target hold 0.
+    Other window lengths through pips_scoremap_loss_window."""
+    p = exact_problem(H8, W8, N, B, I=2, seed=H8 * W8 + N + B, S=S).to(DEV)
     s = scores(p)
     assert_in_tails(p, s)
     exact_budgets(p, s)
@@ -370,7 +384,7 @@ def test_scoremap_loss_exact(H8, W8, N, B):
         zeros = bool((neg[dropped] == 0).all() and (pos[dropped] == 0).all())
         msgs.append(f"iteration {i}: neg {n_neg}, pos {n_pos} differing; dropped rows 0: {zeros}; slack NaN: {slack}")
         fails += n_neg + n_pos + (not zeros) + (not slack)
-    print(f"scoremap_loss {H8}x{W8} N={N} B={B} ({p.n_split} splits): " + "; ".join(msgs))
+    print(f"scoremap_loss {H8}x{W8} N={N} B={B} S={S} ({p.n_split} splits): " + "; ".join(msgs))
     assert fails == 0
 
 
@@ -463,12 +477,13 @@ def test_scoremap_basis_grad_per_element(H8, W8, N, B):
 # ------------------------------------------------------------------------------------------------ 6. randn data
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("H8,W8,N,B", RANDN_CASES, ids=_ids(RANDN_CASES))
-def test_scoremap_rounding_on_randn(H8, W8, N, B):
+@pytest.mark.parametrize("H8,W8,N,B,S", _windows(RANDN_CASES, [RANDN_CASES[1]], [5, 16]))
+def test_scoremap_rounding_on_randn(H8, W8, N, B, S):
     """the loss and both gradients with scores in the sigmoid's live range, per element: a score's term counts
-    softplus(s) + sigma(s) sum|terms of s| in the loss, |c| + |dc/ds| sum|terms of s| in the gradients, times |Y|"""
+    softplus(s) + sigma(s) sum|terms of s| in the loss, |c| + |dc/ds| sum|terms of s| in the gradients, times |Y|.
+    At other window lengths the loss alone (pips_scoremap_loss_window): the gradient kernels take S = 8 only."""
     I = 3
-    p = randn_problem(H8, W8, N, B, I, seed=H8 + W8 + N + B).to(DEV)
+    p = randn_problem(H8, W8, N, B, I, seed=H8 + W8 + N + B, S=S).to(DEV)
     s, m = scores(p), scores(p, mag=True)
     is_t, kept = _target_mask(p)
     k = int(kept.sum()) * I
@@ -490,6 +505,11 @@ def test_scoremap_rounding_on_randn(H8, W8, N, B):
         m_pos = torch.where(tt, sp[i] + sig[i] * m[i], 0.0).sum(-1).reshape(-1)
         e_loss = max(e_loss, _units(neg, e_neg, m_neg), _units(pos, e_pos, m_pos))
         fails += not slack
+    if S != 8:
+        print(f"scoremap {H8}x{W8} N={N} B={B} S={S} I={I} on randn: loss {e_loss:.3g} (bound {C_LOSS}) units of U "
+              f"sum|terms|; slack NaN: {not fails}")
+        assert e_loss <= C_LOSS and not fails
+        return
     # gradients: c = -cpos sigma(-s) at the target, cneg sigma(s) elsewhere
     c = torch.where(is_t, -cpos * sig, cneg * sig) * mask
     dc = torch.where(is_t, cpos, cneg).double() * sig * (1 - sig) * mask

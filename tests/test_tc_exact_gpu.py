@@ -188,10 +188,12 @@ def _gelu_tail_expected(v):
     return hi, (gv - hi.float()).to(torch.bfloat16)
 
 
-def check_exact_gemm(M, N, K, epi, terms, g, sa=Spec(3, 8), sw=Spec(3, 8), w_rows=None, with_lo=True):
-    """One exact pips_gemm_tc call at lda = K + 8, ldw = K + 8, ldo = N + 4, ldh = N + 8, NaN around everything.
+def check_exact_gemm(M, N, K, epi, terms, g, sa=Spec(3, 8), sw=Spec(3, 8), w_rows=None, with_lo=True, ldo=None,
+                     zero_w_pad=False):
+    """One exact pips_gemm_tc call at lda = K + 8, ldw = K + 8, ldo = N + 4 (or `ldo`), ldh = N + 8, NaN around everything.
     BIAS / BIAS_RESID: out == fp64; BIAS_GELU: pre-activations in the flat tails, hi and lo == expected.  -> (differing
-    elements, a description of any poison that was overwritten)"""
+    elements, a description of any poison that was overwritten).  zero_w_pad: W rows [N, w_rows) are 0, as PackedWeights
+    pads the head, so a column past N that the kernel stores holds 0 instead of the NaN the poison already is."""
     x3 = terms == 3
     gelu = epi == L.EPI_BIAS_GELU
     if gelu:
@@ -201,6 +203,8 @@ def check_exact_gemm(M, N, K, epi, terms, g, sa=Spec(3, 8), sw=Spec(3, 8), w_row
     w_rows = w_rows or (N // 256 + 1) * 256
     a = _operand(sa, a_rows, M, K, K + 8, g)
     w = _operand(sw, w_rows, N, K, K + 8, g)
+    if zero_w_pad:
+        w[0][N:], w[1][N:] = 0, 0
     ra, rw = sa.ranges, sw.ranges
     _, grid = exact_budget(K, ra, rw, terms)
     bias = _tail_bias(N, g) if gelu else on_grid((N,), 4.0, grid, g)
@@ -220,7 +224,7 @@ def check_exact_gemm(M, N, K, epi, terms, g, sa=Spec(3, 8), sw=Spec(3, 8), w_row
             if o is not None and not (torch.isnan(o[M:].float()).all() and torch.isnan(o[:M, N:].float()).all()):
                 bad.append(name)
         return n, bad
-    of = _nan(M + extra_rows, N + 4)
+    of = _nan(M + extra_rows, ldo or N + 4)
     if resid is not None:
         of[:M, :N] = resid
         acc = acc + resid.double()
@@ -297,6 +301,52 @@ def test_gemm_exact_edges(terms, tile, monkeypatch):
                 fails.append((M, N, epi, n, bad))
             i += 1
     print(f"gemm edges tile={tile or 'auto'} terms={terms}: {len(EDGE_M) * len(EDGE_N)} shapes, failing: {fails or 'none'}")
+    assert not fails
+
+
+def check_exact_gemm_f32(M, N, K, g, ldo, w_rows):
+    """One exact pips_gemm_f32 (BIAS) call at lda = ldw = K + 8: A on the grid Q (hi + lo of Spec(3, 8), exact in fp32),
+    W small integers, so every product and partial sum is exact.  NaN in A's and W's rows past the problem and pitch
+    columns, and around the output.  -> (differing elements, whether any poison was overwritten)"""
+    sa, sw = Spec(3, 8), Spec(3, 8)
+    a_hi, a_lo = _operand(sa, (M // 256 + 1) * 256, M, K, K + 8, g)
+    w_hi, _ = _operand(sw, w_rows, N, K, K + 8, g)
+    a, w = a_hi.float() + a_lo.float(), w_hi.float()
+    ra = sa.ranges
+    _, grid = exact_budget(K, Ranges(ra.hi + ra.lo, ra.lo_grid, 0.0, ra.lo_grid), sw.ranges, terms=1)
+    bias = on_grid((N,), 4.0, grid, g)
+    exact_budget(K, Ranges(ra.hi + ra.lo, ra.lo_grid, 0.0, ra.lo_grid), sw.ranges, terms=1, extra=4.0)
+    of = _nan(M + 70, ldo)
+    L.check(L.load().pips_gemm_f32(L.ptr(a), a.shape[1], L.ptr(w), w.shape[1], M, N, K, L.ptr(bias), L.EPI_BIAS, L.ptr(of),
+                                   ldo, _st()), "pips_gemm_f32")
+    torch.cuda.synchronize()
+    ref = a[:M, :K].double() @ w[:N, :K].double().t() + bias.double()
+    return _differ(of[:M, :N], ref), not (torch.isnan(of[M:]).all() and torch.isnan(of[:M, N:]).all())
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("tile", TILES)
+@pytest.mark.parametrize("terms", [3, 1])
+def test_gemm_exact_head_every_window(terms, tile, monkeypatch):
+    """The head Linear(512 -> 130 S) of every window length 2..16 as pips_mixer_forward_s runs it: N = 130 S over
+    PIPS_HEAD_PAD(S) weight rows, into delta rows of PIPS_DELTA_LD(S) floats.  At odd S, N % 8 is 2 or 6, so the bias
+    guards of the last column group and the TMA store's clipping of a partial 32-column box are live, and the 2 pad
+    columns of every row must stay NaN (W's pad rows are zero, as in the packed weights).  M = 300 (512 rows allocated) reaches the pair kernel.  pips_gemm_f32, the fp32
+    precision's head, is checked at the same N and ldo."""
+    monkeypatch.setenv("PIPS_B200_GEMM_TILE", tile)
+    g = _gen(31 + terms)
+    fails = []
+    for S in range(2, L.S_MAX + 1):
+        N, w_rows, ldo = L.head_n(S), L.head_pad(S), L.delta_ld(S)
+        for M in (1, 65, 300):
+            n, bad = check_exact_gemm(M, N, 512, L.EPI_BIAS, terms, g, w_rows=w_rows, ldo=ldo, zero_w_pad=True)
+            if n or bad:
+                fails.append(("tc", S, M, n, bad))
+            if terms == 3 and tile == "":
+                n, bad = check_exact_gemm_f32(M, N, 512, g, ldo, w_rows)
+                if n or bad:
+                    fails.append(("f32", S, M, n, bad))
+    print(f"gemm head S=2..16 tile={tile or 'auto'} terms={terms}: 45 shapes, failing: {fails or 'none'}")
     assert not fails
 
 

@@ -1,5 +1,6 @@
 """Models of window lengths 2..16 on the CUDA path: end to end against the unmodified reference's outputs
-(tests/golden/reference_window.npz), and the token-mixing kernels against fp64."""
+(tests/golden/reference_window.npz).  The kernels themselves are checked per element at these window lengths by
+test_loop_kernels_gpu.py, test_tc_exact_gpu.py and test_scoremap_exact_gpu.py."""
 import os
 import subprocess
 import sys
@@ -132,68 +133,3 @@ def test_refusals():
     with pytest.raises(ValueError, match="S=12"):
         m(xys.to(DEV), rgbs.to(DEV))
     m._shard = None
-
-
-# ------------------------------------------------------------------------------------------------ kernels vs fp64
-
-def _tokenmix_ref(x, p, S):
-    """nets/pips.py:117 + the LayerNorm of :118 in fp64: x (R, S, 512) -> (x + tokenmix, LN2(x + tokenmix))."""
-    ln = lambda v, w, b: torch.nn.functional.layer_norm(v, (512,), w, b, 1e-5)
-    y = ln(x, p["ln1_w"], p["ln1_b"])
-    h = torch.nn.functional.gelu(torch.einsum("rsc,js->rjc", y, p["w1"]) + p["b1"][None, :, None])
-    z = torch.einsum("rjc,sj->rsc", h, p["w2"]) + p["b2"][None, :, None]
-    xn = x + z
-    return xn, ln(xn, p["ln2_w"], p["ln2_b"])
-
-
-@pytest.mark.parametrize("S", [2, 5, 8, 9, 16])
-@pytest.mark.parametrize("path", ["tc", "f32"])
-def test_tokenmix_against_fp64(S, path):
-    lib = L.load()
-    g = torch.Generator().manual_seed(S)
-    R = 37
-    p = {"ln1_w": 1 + 0.1 * torch.randn(512, generator=g), "ln1_b": 0.1 * torch.randn(512, generator=g),
-         "w1": torch.randn(4 * S, S, generator=g) / S ** 0.5, "b1": 0.1 * torch.randn(4 * S, generator=g),
-         "w2": torch.randn(S, 4 * S, generator=g) / (2 * S ** 0.5), "b2": 0.1 * torch.randn(S, generator=g),
-         "ln2_w": 1 + 0.1 * torch.randn(512, generator=g), "ln2_b": 0.1 * torch.randn(512, generator=g)}
-    x = torch.randn(R, S, 512, generator=g) * 2 + 0.5
-    xn_ref, y_ref = _tokenmix_ref(x.double(), {k: v.double() for k, v in p.items()}, S)
-    pd = {k: v.to(DEV).contiguous() for k, v in p.items()}
-    rows = R * S
-    xd = torch.full((rows + 40, 512), float("nan"), device=DEV)          # rows after the last track: NaN, untouched
-    xd[:rows] = x.reshape(rows, 512).to(DEV)
-    args = [pd[k].data_ptr() for k in ("ln1_w", "ln1_b", "w1", "b1", "w2", "b2", "ln2_w", "ln2_b")]
-    if path == "tc":
-        hi = torch.full((rows + 40, 512), float("nan"), dtype=torch.bfloat16, device=DEV)
-        lo = torch.full_like(hi, float("nan"))
-        L.check(lib.pips_tokenmix_tc_s(xd.data_ptr(), R, S, *args, hi.data_ptr(), lo.data_ptr(), None))
-        y = hi.float() + lo.float()
-    else:
-        y = torch.full((rows + 40, 512), float("nan"), device=DEV)
-        L.check(lib.pips_tokenmix_s(xd.data_ptr(), R, S, *args, None, None, y.data_ptr(), None))
-    torch.cuda.synchronize()
-    assert torch.isnan(xd[rows:]).all() and torch.isnan(y[rows:]).all()
-    ex = (xd[:rows].cpu().double() - xn_ref.reshape(rows, 512)).abs().max().item()
-    ey = (y[:rows].cpu().double() - y_ref.reshape(rows, 512)).abs().max().item()
-    print(f"S={S} {path}: residual max |err| {ex:.2e}, LN2 output max |err| {ey:.2e}")
-    assert ex < 1e-4 and ey < (2e-4 if path == "tc" else 1e-4)
-
-
-@pytest.mark.parametrize("S", [5, 16])
-def test_ln_pool_against_fp64(S):
-    lib = L.load()
-    g = torch.Generator().manual_seed(100 + S)
-    R = 29
-    x = torch.randn(R * S, 512, generator=g) * 3 - 1
-    w, b = 1 + 0.1 * torch.randn(512, generator=g), 0.1 * torch.randn(512, generator=g)
-    ref = torch.nn.functional.layer_norm(x.double(), (512,), w.double(), b.double(), 1e-5).reshape(R, S, 512).mean(1)
-    xd = torch.full((R * S + 16, 512), float("nan"), device=DEV)
-    xd[:R * S] = x.to(DEV)
-    out = torch.full((R + 3, 512), float("nan"), device=DEV)
-    wd, bd = w.to(DEV), b.to(DEV)
-    L.check(lib.pips_ln_pool_s(xd.data_ptr(), R, S, wd.data_ptr(), bd.data_ptr(), None, None, out.data_ptr(), None))
-    torch.cuda.synchronize()
-    assert torch.isnan(out[R:]).all()
-    err = (out[:R].cpu().double() - ref).abs().max().item()
-    print(f"S={S}: ln_pool max |err| {err:.2e}")
-    assert err < 1e-5
