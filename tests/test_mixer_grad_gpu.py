@@ -1,8 +1,13 @@
 """Training the DeltaBlock mixer on the sm_90a kernels (Pips(mixer_path='cuda'), torch_path.delta_block_cuda): the
 weight-gradient GEMM, the pre-activation GEMM epilogues and the fused LayerNorm / token-mixing backward against fp64,
-the whole mixer's forward and backward against fp64 autograd of the DeltaBlock module, determinism, a training step
-against mixer_path='torch', memory, routing, and argument validation without a GPU.  Errors are norm-wise relative
-errors against fp64 (``_rel``); bf16x3 products carry about 2^-17 relative error each."""
+the whole mixer's forward and backward against fp64 autograd of the DeltaBlock module, stale rows, determinism, a
+training step against mixer_path='torch', memory, routing, and argument validation without a GPU.
+
+The CUDA-core backward kernels (pips_tokenmix_grad, pips_ln_pool_grad) are checked per element against fp64 references
+that follow their formulas, in units of U * magnitude: the magnitude is the same backward evaluated on absolute values
+with every subtraction turned into an addition (test_loop_kernels_gpu.py's convention).  The bounds are the largest
+ratio measured on an H100 80GB HBM3 with a margin of 2-4x.  The whole DeltaBlock is checked per tensor as
+max|err| / max|ref|.  The GEMM pieces are checked norm-wise here (``_rel``) and bit for bit in test_tc_exact_gpu.py."""
 import ctypes as C
 import math
 
@@ -13,8 +18,24 @@ import torch.nn.functional as F
 from oracle import pips_oracle as po
 from pips_b200 import Pips, _lib as L, torch_path
 from pips_b200.pips import DeltaBlock
+from tests.test_loop_kernels_gpu import _bits, _ln_mag, _nan, _ratio, _report, _tokenmix_inputs
 
 DEV = "cuda:0"
+
+# Bounds, in units of U * magnitude (U = 2^-24), per element.  The kernels' sums run in a fixed order, so these inputs
+# give the same ratios on every run.
+C_TG_DX = 1.0          # pips_tokenmix_grad dx (measured 0.40, plain rows at 2049 sequences)
+C_TG_LN2 = 6.0         # its ln2_w and ln2_b gradients (measured 2.3, plain, 1 sequence): dy is exact, so the magnitudes
+                       # of their terms are tight
+C_TG_PARAM = 0.5       # its other 1576 gradients (measured 0.19, tok_w1): their terms pass through dh and du, whose
+                       # magnitudes carry the rounding of the recomputed hidden layer
+C_LP_DX = 10.0         # pips_ln_pool_grad dx (measured 3.9, plain rows at 2049 sequences)
+C_LP_PARAM = 12.0      # its ln_w and ln_b gradients (measured 4.9, ln_b at 37 sequences)
+# The whole DeltaBlock, max|err| / max|ref| per tensor.  A bf16x3 product or (hi, lo) pair carries about 2^-17 relative
+# error, and a gradient passes through the 38 GEMMs of the forward and about as many of the backward; the rounding
+# errors mostly cancel, and the largest measured is 5.8 x 2^-17 (4.4e-5, block 11's FC1 bias at R = 3072, head x0.05).
+# Strict fp32 torch stays below 4.2e-6, so this floor sets every bound.
+MIX_FLOOR = 16 * 2.0 ** -17
 
 
 def _rel(a, b):
@@ -134,12 +155,22 @@ def test_pre_activation_epilogues_match_fp64(M):
     assert max(e_pre, e_gelu, e_tail, e_grad, e_gtail) <= 1e-4
 
 
+GELU_GRAD_ZERO = -0.7517915246935644                     # gelu'(h) = Phi(h) + h phi(h) = 0: its two terms cancel
+TOK_PARAMS = ("ln1_w", "ln1_b", "tok_w1", "tok_b1", "tok_w2", "tok_b2", "ln2_w", "ln2_b")   # the order of the 2600 gradients
+
+
 def _tok_params(seed):
+    """Token-mixing block parameters.  Hidden units 0, 8, 16, 24 sit in GELU's positive tail (h > 6 nearly everywhere),
+    units 1, 9, 17, 25 in its negative tail, and units 2, 10, 18, 26 within about 3e-3 of gelu''s zero crossing."""
     g = torch.Generator(device=DEV).manual_seed(seed)
     P = {"ln1_w": 1 + 0.2 * torch.randn(512, generator=g, device=DEV), "ln1_b": 0.1 * torch.randn(512, generator=g, device=DEV),
          "tok_w1": torch.randn(32, 8, generator=g, device=DEV) / math.sqrt(8), "tok_b1": 0.3 * torch.randn(32, generator=g, device=DEV),
          "tok_w2": torch.randn(8, 32, generator=g, device=DEV) / math.sqrt(32), "tok_b2": 0.1 * torch.randn(8, generator=g, device=DEV),
          "ln2_w": 1 + 0.2 * torch.randn(512, generator=g, device=DEV), "ln2_b": 0.1 * torch.randn(512, generator=g, device=DEV)}
+    P["tok_b1"][0::8] += 9.0
+    P["tok_b1"][1::8] -= 9.0
+    P["tok_w1"][2::8] *= 1e-3
+    P["tok_b1"][2::8] = GELU_GRAD_ZERO
     return {k: v.contiguous() for k, v in P.items()}
 
 
@@ -151,35 +182,196 @@ def _tok_block64(x, P):
     return x_mid, F.layer_norm(x_mid, (512,), P["ln2_w"], P["ln2_b"])
 
 
+def _ln_back64(x, dy, dymag, w):
+    """fp64 LayerNorm backward over the last axis with ln_backward8's formulas (mixer_grad.cu): xh = (x - m) r and
+    dx = r (w dy - mean(w dy) - xh mean(w dy xh)).  Returns dx and the per-element terms dy xh of the weight gradient,
+    each with the magnitude of its terms: every subtraction becomes an addition, |x - m| becomes (|x| + |m|) r
+    (_ln_mag), and dy comes with its own magnitude dymag."""
+    m = x.mean(-1, keepdim=True)
+    xhmag, r = _ln_mag(x, torch.ones_like(w), torch.zeros_like(w))
+    xh = (x - m) * r
+    gd, gdmag = dy * w, dymag * w.abs()
+    a, amag = gd.mean(-1, keepdim=True), gdmag.mean(-1, keepdim=True)
+    b, bmag = (gd * xh).mean(-1, keepdim=True), (gdmag * xhmag).mean(-1, keepdim=True)
+    return r * (gd - a - xh * b), r * (gdmag + amag + xhmag * bmag), dy * xh, dymag * xhmag
+
+
+def _gelu64(h, hmag):
+    """gelu(h) and gelu'(h) in fp64 with the magnitudes of common.cuh's formulas: 0.5 h (1 + erf(h / sqrt 2)) and
+    Phi(h) + h phi(h), each plus |its derivative| times the magnitude of h (the rounding of the recomputed h)."""
+    phi = torch.exp(-0.5 * h * h) / math.sqrt(2.0 * math.pi)
+    Phi = 0.5 * torch.erfc(-h / math.sqrt(2.0))
+    d1, d2 = Phi + h * phi, phi * (2.0 - h * h)
+    amag = 0.5 * h.abs() * (1.0 + torch.erf(h / math.sqrt(2.0)).abs()) + d1.abs() * hmag
+    return h * Phi, amag, d1, Phi + h.abs() * phi + d2.abs() * hmag
+
+
+def _tokenmix_grad64(x, xm, dy, dxo, P):
+    """pips_tokenmix_grad in fp64, with the formulas of the comment above tokenmix_grad_kernel: dz = dxo + LN2^T(dy),
+    da = W2^T dz, dh = da gelu'(h), du = W1^T dh, dx = dz + LN1^T(du), and the 8 parameter sums.  Every result comes as
+    (value, magnitude): the same backward on absolute values (_ln_back64, _gelu64).  x, xm, dy, dxo: (seqs, 8, 512)."""
+    d = {k: v.double() for k, v in P.items()}
+    out = {}
+    dl, dlmag, tw, twmag = _ln_back64(xm, dy, dy.abs(), d["ln2_w"])
+    dz, dzmag = dxo + dl, dxo.abs() + dlmag
+    out["ln2_w"], out["ln2_b"] = (tw.sum((0, 1)), twmag.sum((0, 1))), (dy.sum((0, 1)), dy.abs().sum((0, 1)))
+    umag, r = _ln_mag(x, d["ln1_w"], d["ln1_b"])
+    u = (x - x.mean(-1, keepdim=True)) * r * d["ln1_w"] + d["ln1_b"]
+    w1, w2 = d["tok_w1"], d["tok_w2"]
+    h = torch.einsum("js,rsc->rjc", w1, u) + d["tok_b1"][None, :, None]
+    hmag = torch.einsum("js,rsc->rjc", w1.abs(), umag) + d["tok_b1"].abs()[None, :, None]
+    a, amag, gp, gpmag = _gelu64(h, hmag)
+    dh = torch.einsum("sj,rsc->rjc", w2, dz) * gp
+    dhmag = torch.einsum("sj,rsc->rjc", w2.abs(), dzmag) * gpmag
+    out["tok_w1"] = (torch.einsum("rjc,rsc->js", dh, u), torch.einsum("rjc,rsc->js", dhmag, umag))
+    out["tok_b1"] = (dh.sum((0, 2)), dhmag.sum((0, 2)))
+    out["tok_w2"] = (torch.einsum("rsc,rjc->sj", dz, a), torch.einsum("rsc,rjc->sj", dzmag, amag))
+    out["tok_b2"] = (dz.sum((0, 2)), dzmag.sum((0, 2)))
+    du, dumag = torch.einsum("js,rjc->rsc", w1, dh), torch.einsum("js,rjc->rsc", w1.abs(), dhmag)
+    dl, dlmag, tw, twmag = _ln_back64(x, du, dumag, d["ln1_w"])
+    out["ln1_w"], out["ln1_b"] = (tw.sum((0, 1)), twmag.sum((0, 1))), (du.sum((0, 1)), dumag.sum((0, 1)))
+    out["dx"] = (dz + dl, dzmag + dlmag)
+    return out
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("seqs", [1, 37, 700])
-def test_tokenmix_grad_matches_fp64(seqs):
-    lib = L.load()
-    g = torch.Generator(device=DEV).manual_seed(seqs)
-    P = _tok_params(seqs)
-    x = torch.randn(seqs, 8, 512, generator=g, device=DEV) * 2 + 0.5
-    dy = torch.randn(seqs, 8, 512, generator=g, device=DEV)
-    dxo = torch.randn(seqs, 8, 512, generator=g, device=DEV)
+def test_tokenmix_grad_reference_matches_autograd():
+    """_tokenmix_grad64 against fp64 autograd of _tok_block64, with x_mid = the forward's, on flat rows and GELU tails:
+    the per-element reference of test_tokenmix_grad_per_element is the module's gradient."""
+    P = _tok_params(5)
+    x = _grad_rows("flat", 37, 501).double().to(DEV)
+    g = torch.Generator(device=DEV).manual_seed(5)
+    dy, dxo = (torch.randn(37, 8, 512, generator=g, device=DEV, dtype=torch.float64) for _ in range(2))
     P64 = {k: v.double().requires_grad_(True) for k, v in P.items()}
-    x64 = x.double().requires_grad_(True)
+    x64 = x.clone().requires_grad_(True)
     x_mid, y = _tok_block64(x64, P64)
-    ((y * dy.double()).sum() + (x_mid * dxo.double()).sum()).backward()
-    xm = x_mid.detach().float().contiguous()
-    dx = dxo.clone()
-    scratch = torch.empty(lib.pips_tokenmix_grad_scratch_floats(seqs), device=DEV)
-    grads = torch.full((2600,), float("nan"), device=DEV)
-    L.check(lib.pips_tokenmix_grad(L.ptr(x), L.ptr(xm), L.ptr(dy), L.ptr(dx), seqs,
-                                   *(L.ptr(P[k]) for k in ("ln1_w", "ln1_b", "tok_w1", "tok_b1", "tok_w2", "tok_b2", "ln2_w", "ln2_b")),
+    ((y * dy).sum() + (x_mid * dxo).sum()).backward()
+    ref = _tokenmix_grad64(x, x_mid.detach(), dy, dxo, P)
+    errs = {k: _rel(ref[k][0], (x64 if k == "dx" else P64[k]).grad) for k in ("dx",) + TOK_PARAMS}
+    print("explicit fp64 backward vs fp64 autograd: " + ", ".join(f"{k} {v:.1e}" for k, v in errs.items()))
+    assert max(errs.values()) <= 1e-10
+
+
+_ROWS = {}
+
+
+def _grad_rows(kind, seqs, seed):
+    """(seqs, 8, 512) fp32 rows on the host: "plain" randn, "offset" (_tokenmix_inputs: mean ~100, spread ~1), "flat"
+    (randn with every third row and every fifth sequence made of one value repeated over the 512 channels) or
+    "nearflat" (a common value per row and a spread of 1e-3: the variance, 1e-6, is below LayerNorm's epsilon).  Made
+    at 2049 sequences and cut, so a smaller call sees the first rows of a larger one."""
+    key = (kind, seed)
+    if key not in _ROWS:
+        x = _tokenmix_inputs(2049, kind == "offset", seed)
+        if kind == "flat":
+            flat = (torch.arange(2049 * 8) % 3 == 0).view(2049, 8)
+            flat[::5] = True
+            x[flat] = x[flat][:, :1].expand(-1, 512).contiguous()
+        elif kind == "nearflat":
+            x = 0.5 + torch.randn(2049, 8, 1, generator=torch.Generator().manual_seed(seed + 1)) + 1e-3 * x
+        _ROWS[key] = x
+    return _ROWS[key][:seqs]
+
+
+def _padded(t, seqs):
+    """t (seqs, 8, 512) on the device in a buffer of seqs + 1 sequences, the last one NaN"""
+    out = torch.full((seqs + 1, 8, 512), float("nan"), device=DEV)
+    out[:seqs] = t
+    return out
+
+
+def _tokenmix_grad_call(x, xm, dy, dxo, P, seqs):
+    """pips_tokenmix_grad over the first `seqs` sequences of NaN-padded buffers, with NaN scratch and NaN grads 64 floats
+    longer than the 2600 it writes.  Returns dx (all seqs + 1 sequences) and grads (2664 floats) on the host."""
+    lib = L.load()
+    dx = _padded(dxo[:seqs], seqs)
+    scratch = _nan(lib.pips_tokenmix_grad_scratch_floats(seqs))
+    grads = _nan(2600 + 64)
+    ins = [_padded(t[:seqs], seqs) for t in (x, xm, dy)]
+    L.check(lib.pips_tokenmix_grad(*(L.ptr(t) for t in ins), L.ptr(dx), seqs, *(L.ptr(P[k]) for k in TOK_PARAMS),
                                    L.ptr(scratch), L.ptr(grads), _st()), "pips_tokenmix_grad")
-    errs = {"dx": _rel(dx, x64.grad)}
+    torch.cuda.synchronize()
+    return dx.cpu(), grads.cpu()
+
+
+GRAD_KINDS = ["plain", "offset", "flat", "nearflat"]
+GRAD_SEQS = [1, 37, 700, 2049]       # 700: a partial last CTA; 2049: 257 CTAs, so the partial rows take two colsum levels
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("kind", GRAD_KINDS)
+@pytest.mark.parametrize("seqs", GRAD_SEQS)
+def test_tokenmix_grad_per_element(seqs, kind):
+    """pips_tokenmix_grad per element against _tokenmix_grad64: dx and each of the 2600 gradients within C_TG_* units of
+    U * magnitude.  x and x_mid are both inputs of the kernel and both take the row kind; the GELU-tail parameters
+    of _tok_params throughout.  dx is updated in place and grads is written exactly; the bits repeat, and the first 37
+    sequences' dx does not depend on how many sequences share the call."""
+    P = _tok_params(seqs)
+    x, xm = _grad_rows(kind, seqs, 111), _grad_rows(kind, seqs, 112)
+    g = torch.Generator().manual_seed(113)
+    dy, dxo = torch.randn(2049, 8, 512, generator=g)[:seqs], torch.randn(2049, 8, 512, generator=g)[:seqs]
+    dev = [t.to(DEV) for t in (x, xm, dy, dxo)]
+    dx, grads = _tokenmix_grad_call(*dev, P, seqs)
+    assert torch.isnan(dx[seqs]).all(), "pips_tokenmix_grad wrote dx past the last sequence"
+    assert not torch.isnan(grads[:2600]).any() and torch.isnan(grads[2600:]).all(), "grads: not exactly 2600 floats written"
+    dx2, grads2 = _tokenmix_grad_call(*dev, P, seqs)
+    assert torch.equal(_bits(dx), _bits(dx2)) and torch.equal(_bits(grads), _bits(grads2)), "a second run differs"
+    if seqs > 37:
+        dx37, _ = _tokenmix_grad_call(*dev, P, 37)
+        assert torch.equal(_bits(dx[:37]), _bits(dx37[:37])), "dx of the first 37 sequences depends on seqs"
+    ref = _tokenmix_grad64(*(t.double() for t in dev), P)
+    tag = f"tokenmix_grad seqs={seqs} {kind}"
+    u = F.layer_norm(dev[0].double(), (512,), P["ln1_w"].double(), P["ln1_b"].double())
+    hidden = torch.einsum("js,rsc->rjc", P["tok_w1"].double(), u) + P["tok_b1"].double()[None, :, None]
+    print(f"{tag}: {int((hidden > 6).sum())} h > 6, {int((hidden < -6).sum())} h < -6, "
+          f"{int(((hidden - GELU_GRAD_ZERO).abs() < 0.01).sum())} |h - h0| < 0.01")
+    _report(f"{tag} dx: err / (U mag)", _ratio(dx[:seqs], ref["dx"][0], ref["dx"][1]), C_TG_DX)
     off = 0
-    for k in ("ln1_w", "ln1_b", "tok_w1", "tok_b1", "tok_w2", "tok_b2", "ln2_w", "ln2_b"):
+    for k in TOK_PARAMS:
         n = P[k].numel()
-        ref = P64[k].grad.reshape(-1)
-        errs[k] = _rel(grads[off:off + n], ref)             # dxo reaches x_mid directly: no gradient here is 0
+        _report(f"{tag} {k}: err / (U mag)", _ratio(grads[off:off + n], ref[k][0].reshape(-1), ref[k][1].reshape(-1)),
+                C_TG_LN2 if k.startswith("ln2") else C_TG_PARAM)
         off += n
-    print(f"tokenmix backward, {seqs} sequences: " + ", ".join(f"{k} {v:.2e}" for k, v in errs.items()))
-    assert max(errs.values()) <= 1e-4
+
+
+def _ln_pool_grad_call(x, dp, w, b, seqs):
+    """pips_ln_pool_grad over `seqs` sequences: x and dx in buffers of seqs + 1 sequences (x's last NaN), NaN scratch and
+    NaN grads 64 floats longer than the 1024 it writes.  Returns dx and grads on the host."""
+    lib = L.load()
+    xd = _padded(x, seqs)
+    dx = _nan(seqs + 1, 8, 512)
+    scratch = _nan(lib.pips_ln_pool_grad_scratch_floats(seqs))
+    grads = _nan(1024 + 64)
+    L.check(lib.pips_ln_pool_grad(L.ptr(xd), L.ptr(dp), seqs, L.ptr(w), L.ptr(b), L.ptr(dx), L.ptr(scratch), L.ptr(grads),
+                                  _st()), "pips_ln_pool_grad")
+    torch.cuda.synchronize()
+    return dx.cpu(), grads.cpu()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("kind", GRAD_KINDS[:3])
+@pytest.mark.parametrize("seqs", GRAD_SEQS)
+def test_ln_pool_grad_per_element(seqs, kind):
+    """pips_ln_pool_grad (the backward of LayerNorm -> mean over the 8 rows) per element against fp64: dx within C_LP_DX
+    and the 1024 gradients within C_LP_PARAM units of U * magnitude.  dx is overwritten (it starts NaN, rows past seqs
+    stay NaN), ln_b is not read (NaN there gives the same bits), and exactly 1024 floats of grads are written."""
+    g = torch.Generator(device=DEV).manual_seed(seqs)
+    w = (1 + 0.2 * torch.randn(512, generator=g, device=DEV)).contiguous()
+    b = 0.1 * torch.randn(512, generator=g, device=DEV)
+    x = _grad_rows(kind, seqs, 121).to(DEV)
+    dp = torch.randn(2049, 512, generator=torch.Generator().manual_seed(122))[:seqs].to(DEV)
+    dx, grads = _ln_pool_grad_call(x, dp, w, b, seqs)
+    assert not torch.isnan(dx[:seqs]).any() and torch.isnan(dx[seqs]).all(), "dx: not exactly the live rows written"
+    assert not torch.isnan(grads[:1024]).any() and torch.isnan(grads[1024:]).all(), "grads: not exactly 1024 floats written"
+    dx_nb, grads_nb = _ln_pool_grad_call(x, dp, w, torch.full_like(b, float("nan")), seqs)
+    assert torch.equal(_bits(dx), _bits(dx_nb)) and torch.equal(_bits(grads), _bits(grads_nb)), "ln_b changed the result"
+    x64, dp64 = x.double(), dp.double()
+    gy = (dp64 / 8)[:, None, :].expand(-1, 8, -1)
+    ref, mag, tw, twmag = _ln_back64(x64, gy, gy.abs(), w.double())
+    tag = f"ln_pool_grad seqs={seqs} {kind}"
+    _report(f"{tag} dx: err / (U mag)", _ratio(dx[:seqs], ref, mag), C_LP_DX)
+    _report(f"{tag} ln_w: err / (U mag)", _ratio(grads[:512], tw.sum((0, 1)), twmag.sum((0, 1))), C_LP_PARAM)
+    _report(f"{tag} ln_b: err / (U mag)", _ratio(grads[512:1024], gy.sum((0, 1)), gy.abs().sum((0, 1))), C_LP_PARAM)
 
 
 def _delta_block(seed, head_scale, dtype=torch.float32):
@@ -205,30 +397,87 @@ def _fwd_bwd(m, x, cuda, dy):
 @pytest.mark.gpu
 @pytest.mark.parametrize("R", [1, 37, 3072])
 @pytest.mark.parametrize("head_scale", [0.05, 1.0])
-def test_delta_block_cuda_matches_fp64_autograd(R, head_scale):
+def test_delta_block_cuda_matches_fp64_autograd(monkeypatch, R, head_scale):
+    """The output, dx and each of the 150 parameter gradients against fp64 autograd of the module, as max|err| / max|ref|
+    per tensor, within max(2 x strict fp32 torch's own error, MIX_FLOOR).  The token-mixing FC2 biases have an exact
+    gradient of 0 (every path from them meets a LayerNorm that removes a per-row constant): they are compared to the
+    norm of all gradients instead."""
+    monkeypatch.setattr(torch.backends.cudnn, "allow_tf32", False)
+    monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
     m = _delta_block(3, head_scale)
     m64 = _delta_block(3, head_scale, torch.float64)
     x = _mixer_input(R, R)
     dy = torch.randn(R, 8, 130, device=DEV, generator=torch.Generator(device=DEV).manual_seed(R + 1))
     o64, dx64, g64 = _fwd_bwd(m64, x.double(), False, dy.double())
     oc, dxc, gc = _fwd_bwd(m, x, True, dy)
+    o32, dx32, g32 = _fwd_bwd(m, x, False, dy)
     assert len(gc) == 150
     total = torch.cat([g.flatten() for g in g64.values()]).norm().item()
     zero = {n for n in g64 if g64[n].norm().item() <= 1e-6 * total}
-    assert all(n.endswith("0.fn.3.bias") for n in zero), zero
-    e = {n: _rel(gc[n], g64[n]) for n in g64 if n not in zero}
-    worst = max(e, key=e.get)
-    noise = max([(gc[n].double() - g64[n]).norm().item() / total for n in zero], default=0.0)
-    e_out, e_dx = _rel(oc, o64), _rel(dxc, dx64)
-    e_all = _rel(torch.cat([gc[n].flatten() for n in g64]), torch.cat([g64[n].flatten() for n in g64]))
-    msg = ""
-    if R <= 37:
-        o32, dx32, g32 = _fwd_bwd(m, x, False, dy)
-        msg = (f" | fp32 torch: out {_rel(o32, o64):.2e}, dx {_rel(dx32, dx64):.2e}, all gradients "
-               f"{_rel(torch.cat([g32[n].flatten() for n in g64]), torch.cat([g64[n].flatten() for n in g64])):.2e}")
-    print(f"R={R} head x{head_scale}: out {e_out:.2e}, dx {e_dx:.2e}, all gradients {e_all:.2e}, worst {worst} {e[worst]:.2e}, "
-          f"{len(zero)} zero-gradient biases {noise:.2e} of the norm{msg}")
-    assert e_out <= 1e-3 and e_dx <= 1e-3 and e[worst] <= 1e-3 and noise <= 1e-5
+    assert all(n.endswith("0.fn.3.bias") for n in zero) and len(zero) == 12, zero
+    noise = max((gc[n].double() - g64[n]).norm().item() / total for n in zero)
+
+    def err(a, b):
+        return ((a.double() - b).abs().max() / b.abs().max().clamp(min=1e-300)).item()
+
+    cases = {"out": (oc, o32, o64), "dx": (dxc, dx32, dx64), **{n: (gc[n], g32[n], g64[n]) for n in g64 if n not in zero}}
+    e = {n: (err(c, r), err(t, r)) for n, (c, t, r) in cases.items()}
+    ratio = {n: ec / max(2 * et, MIX_FLOOR) for n, (ec, et) in e.items()}
+    worst = max(ratio, key=ratio.get)
+    top = sorted(e, key=lambda n: e[n][0], reverse=True)[:4]
+    print(f"R={R} head x{head_scale}: max|err| / max|ref|, cuda / fp32 torch: out {e['out'][0]:.2e} / {e['out'][1]:.2e}, "
+          f"dx {e['dx'][0]:.2e} / {e['dx'][1]:.2e}, largest " + ", ".join(f"{n} {e[n][0]:.2e} / {e[n][1]:.2e}" for n in top)
+          + f"; worst against its bound {worst} {ratio[worst]:.2f}; {len(zero)} zero-gradient biases {noise:.2e} of the norm")
+    assert ratio[worst] <= 1.0 and noise <= 1e-5
+
+
+def _fwd_bwd_filled(m, x, dy, fill, monkeypatch):
+    """_fwd_bwd on the CUDA path with every uninitialised allocation of the delta_block_cuda call (torch.empty and
+    _MixerRun.rows, in its forward and its backward) filled with `fill`"""
+    real = torch.empty
+
+    def empty(*a, **k):
+        return real(*a, **k).fill_(fill)
+
+    m.zero_grad(set_to_none=True)
+    xr = x.clone().requires_grad_(True)
+    with monkeypatch.context() as mp:
+        mp.setattr(torch, "empty", empty)
+        mp.setattr(torch_path._MixerRun, "rows", lambda self, n, cols, dtype=torch.float32: empty(n, cols, dtype=dtype,
+                                                                                                   device=self.dev))
+        out = torch_path.delta_block_cuda(m, xr)
+        (out * dy).sum().backward()
+    return out.detach(), xr.grad, {n: p.grad.detach().clone() for n, p in m.named_parameters()}
+
+
+@pytest.mark.gpu
+def test_delta_block_cuda_stale_rows(monkeypatch):
+    """Every buffer of a call holds whole 256-row tiles (M = 296 rows at R = 37 live in 512-row buffers) from the
+    caching allocator, and rows past M are never written: whatever they hold must not reach a result.  With every
+    uninitialised allocation filled with NaN, and then with zeros, the output, dx and all 150 gradients have the same
+    bits, and no NaN."""
+    m = _delta_block(3, 1.0)
+    x = _mixer_input(37, 71)
+    dy = torch.randn(37, 8, 130, device=DEV, generator=torch.Generator(device=DEV).manual_seed(72))
+    nan = _fwd_bwd_filled(m, x, dy, float("nan"), monkeypatch)
+    zero = _fwd_bwd_filled(m, x, dy, 0.0, monkeypatch)
+    assert len(zero[2]) == 150
+    for name, a, b in [("out", nan[0], zero[0]), ("dx", nan[1], zero[1])] + [(n, nan[2][n], zero[2][n]) for n in zero[2]]:
+        assert not torch.isnan(b).any(), f"{name}: NaN with zero-filled buffers"
+        assert torch.equal(_bits(a), _bits(b)), f"{name}: stale rows changed the result"
+
+
+@pytest.mark.gpu
+def test_delta_block_cuda_prefix():
+    """The output and dx of a sequence do not depend on how many other sequences share the call: the first 37 rows are
+    the same bits at R = 37 and R = 300."""
+    m = _delta_block(3, 1.0)
+    x = _mixer_input(300, 73)
+    dy = torch.randn(300, 8, 130, device=DEV, generator=torch.Generator(device=DEV).manual_seed(74))
+    o300, dx300, _ = _fwd_bwd(m, x, True, dy)
+    o37, dx37, _ = _fwd_bwd(m, x[:37], True, dy[:37])
+    assert torch.equal(_bits(o300[:37]), _bits(o37)), "the output of the first 37 sequences depends on R"
+    assert torch.equal(_bits(dx300[:37]), _bits(dx37)), "dx of the first 37 sequences depends on R"
 
 
 @pytest.mark.gpu
@@ -438,6 +687,13 @@ def test_mixer_grad_entry_points_validate_arguments_without_gpu():
     assert lp(p, None, 4, p, p, p, p, p, None) != 0 and b"pips_ln_pool_grad: null pointer" in lib.pips_last_error()
     assert lp(p, p, 0, p, p, p, p, p, None) != 0 and b"no sequences" in lib.pips_last_error()
     assert lp(p, q, 4, p, p, p, p, p, None) != 0 and b"16-byte aligned" in lib.pips_last_error()
+    # one partial row of P floats per CTA of 8 sequences; above 256 CTAs pips_colsum adds them in two levels, with one
+    # more row per split of 256
+    for fn, P in ((lib.pips_ln_pool_grad_scratch_floats, 1024), (lib.pips_tokenmix_grad_scratch_floats, 2600)):
+        for seqs in (1, 2048, 2049):
+            ctas = (seqs + 7) // 8
+            assert fn(seqs) == ctas * P + ((ctas + 255) // 256 * P if ctas > 256 else 0), (P, seqs)
+    assert lib.pips_ln_pool_grad_scratch_floats(0) == 0
 
     ga = lib.pips_gemm_tc_aux
     assert ga(p, p, 512, 256, p, p, 512, 2048, 256, 2048, 512, p, L.EPI_GELU_GRAD, None, 0, p, p, 2048, None, 0, None) != 0
