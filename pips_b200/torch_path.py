@@ -853,8 +853,15 @@ def forward_torch(model, xys, rgbs, coords_init=None, feat_init=None, iters=3, t
             for i, v in enumerate(vols):                                        # :355-382
                 h, w = v.shape[-2:]
                 loc = coords.reshape(B * S * N, 1, 1, 2) / 2 ** i + window
-                grid = torch.cat([2 * loc[..., :1] / (w - 1) - 1, 2 * loc[..., 1:] / (h - 1) - 1], dim=-1)
-                taps.append(F.grid_sample(v.reshape(B * S * N, 1, h, w), grid, align_corners=True).view(B, S, N, -1))
+                if h > 1 and w > 1:
+                    grid = torch.cat([2 * loc[..., :1] / (w - 1) - 1, 2 * loc[..., 1:] / (h - 1) - 1], dim=-1)
+                    taps.append(F.grid_sample(v.reshape(B * S * N, 1, h, w), grid, align_corners=True).view(B, S, N, -1))
+                else:
+                    # a level one pixel high or wide (level 3 of an 8 to 15 px map): align_corners=True divides by
+                    # size - 1 = 0 and every tap is NaN.  align_corners=False puts pixel j at j as well, so this is the
+                    # same bilinear sample with zero padding, the one local_corr_cuda and pips_corr_gather take.
+                    grid = torch.cat([(2 * loc[..., :1] + 1) / w - 1, (2 * loc[..., 1:] + 1) / h - 1], dim=-1)
+                    taps.append(F.grid_sample(v.reshape(B * S * N, 1, h, w), grid, align_corners=False).view(B, S, N, -1))
             fcorr = torch.cat(taps, dim=-1).permute(0, 2, 1, 3).reshape(B * N, S, -1)
         flow = (coords - coords[:, 0:1]).permute(0, 2, 1, 3).reshape(B * N, S, 2)
         flow = torch.cat([flow, times.expand(B * N, -1, -1)], dim=2)
