@@ -9,9 +9,9 @@
  *   - returns 0 on success, non-zero on error with the message available from pips_last_error().
  * All tensors are contiguous unless a leading dimension is given.  The feature dimension is 128
  * (nets/pips.py:408).  S (frames per window, the model's constructor argument, nets/pips.py:401) is 8 for the
- * entry points without an S of their own and for training and chained tracking; the inference entry points
- * (pips_refine_iter, pips_corr_gather, pips_init_gather, pips_update, pips_vis_head, pips_heatmap and the _s /
- * _window siblings) take any 2 <= S <= PIPS_S_MAX.  Sizes that depend on S: the head GEMM's N = PIPS_HEAD_N(S) = 130*S,
+ * entry points without an S of their own, for the mixer's training kernels and for chained tracking; the inference
+ * entry points (pips_refine_iter, pips_corr_gather, pips_init_gather, pips_update, pips_vis_head, pips_heatmap) and the
+ * _s / _window siblings, including those of the correlation and score-map gradients, take any 2 <= S <= PIPS_S_MAX.  Sizes that depend on S: the head GEMM's N = PIPS_HEAD_N(S) = 130*S,
  * padded to PIPS_HEAD_PAD(S) rows (a multiple of 256).
  *
  * Layouts
@@ -131,7 +131,8 @@ int pips_init_gather_groups(const pips_groups* groups, int B, int S, int N, cons
                             float* ffeat /* (B*N,128) */, float* ffeats /* (B*N,S,128) */, void* stream);
 
 /* Backward of pips_corr_gather's correlation columns (x[:, 128:324]) for training (csrc/corr_grad.cu), with respect to
- * the ffeats and the 4 fp32 levels; the coordinates get no gradient.  S == 8, fp32, no frame_base.  dcorr is the
+ * the ffeats and the 4 fp32 levels; the coordinates get no gradient.  S == 8 (the _window siblings below take
+ * 2 <= S <= PIPS_S_MAX), fp32, no frame_base.  dcorr is the
  * gradient of those 196 columns, (B*N*S, ld_dcorr) in mixer row order, ld_dcorr >= 196.  Per unit and level the
  * adjoint of the 49-tap blend is an 8x8 weight matrix A over the unit's footprint (the pixels pips_corr_gather read):
  *   A[j][i] = (1/sqrt(128)) sum_{dy,dx in {0,1}} w_{dy,dx} dcorr[l*49 + (i-dx)*7 + (j-dy)]   (0 <= i-dx, j-dy < 7)
@@ -143,6 +144,12 @@ int pips_corr_grad_feats(const float* const* lvl, int B, int S, int N, int H, in
                          const float* dcorr, int ld_dcorr, float* dffeat_rows, void* stream);
 int pips_corr_grad_levels(int B, int S, int N, int H, int W, const float* coords, const float* ffeat_rows,
                           const float* dcorr, int ld_dcorr, float* const* dlvl, void* stream);
+/* pips_corr_grad_feats / pips_corr_grad_levels for windows of 2 <= S <= PIPS_S_MAX frames (the entry points above take
+ * S == 8 only): the same arguments and checks; at S == 8 the same kernels, so the same bits. */
+int pips_corr_grad_feats_window(const float* const* lvl, int B, int S, int N, int H, int W, const float* coords,
+                                const float* dcorr, int ld_dcorr, float* dffeat_rows, void* stream);
+int pips_corr_grad_levels_window(int B, int S, int N, int H, int W, const float* coords, const float* ffeat_rows,
+                                 const float* dcorr, int ld_dcorr, float* const* dlvl, void* stream);
 
 /* nn.Linear on tensor cores: out = epi(A[M,K] . W[N,K]^T + bias).  a_lo/w_lo NULL => plain bf16. */
 int pips_gemm_tc(const void* a_hi, const void* a_lo, int lda, int a_rows,
@@ -293,7 +300,8 @@ int pips_scoremap_loss_window(const void* G_hi, const void* G_lo, const float* f
 /* Backward of the score-map loss over `iters` iterations (csrc/scoremap_grad.cu), without the dense score maps.
  * coef (device, 2 floats) holds g/(eps+K) and g/(eps+K(P-1)): g the upstream gradient, K the kept rows times iters,
  * P = H8*W8, eps = 1e-6.  target is that of pips_scoremap_loss; G_hi / G_lo that of pips_scoremap_basis.  Each output
- * element is summed in a fixed order (deterministic, no atomics); the score GEMMs run in bf16x3.
+ * element is summed in a fixed order (deterministic, no atomics); the score GEMMs run in bf16x3.  S == 8; the _window
+ * siblings take 2 <= S <= PIPS_S_MAX.
  * pips_scoremap_grad_feats: dffeats = dloss/dffeats, both (iters, B*S, N, 128) fp32 frame-major
  *   (ffeats[i, b*S+s, n] is the ffeats of track (b, n) in frame s at the start of iteration i).
  * pips_scoremap_grad_basis: dG = dloss/dG (B*S, H8*W8, 128) fp32, from F_hi / F_lo, the bf16 (hi, lo) split of those
@@ -304,6 +312,13 @@ int pips_scoremap_grad_feats(const void* G_hi, const void* G_lo, const float* ff
                              int H8, int W8, const int* target, const float* coef, float* dffeats, void* stream);
 int pips_scoremap_grad_basis(const void* G_hi, const void* G_lo, const void* F_hi, const void* F_lo, int iters, int B,
                              int S, int N, int H8, int W8, const int* target, const float* coef, float* dG, void* stream);
+/* pips_scoremap_grad_feats / pips_scoremap_grad_basis for windows of 2 <= S <= PIPS_S_MAX frames: the same arguments,
+ * checks and kernels (at S == 8 the same bits). */
+int pips_scoremap_grad_feats_window(const void* G_hi, const void* G_lo, const float* ffeats, int iters, int B, int S, int N,
+                                    int H8, int W8, const int* target, const float* coef, float* dffeats, void* stream);
+int pips_scoremap_grad_basis_window(const void* G_hi, const void* G_lo, const void* F_hi, const void* F_lo, int iters,
+                                    int B, int S, int N, int H8, int W8, const int* target, const float* coef, float* dG,
+                                    void* stream);
 int pips_scoremap_basis_grad(const float* dG, int frames, int H8, int W8, float* const* dlvl_f32, void* stream);
 
 /* v -> (hi, lo) bf16 with hi = rn(v), lo = rn(v - hi); lo may be NULL.  Used to pack weights. */

@@ -101,6 +101,8 @@ _SIGNATURES = {
     "pips_corr_gather_groups": (_i, [C.POINTER(Groups), _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p]),
     "pips_corr_grad_feats": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _p, _p, _i, _p, _p]),
     "pips_corr_grad_levels": (_i, [_i, _i, _i, _i, _i, _p, _p, _p, _i, C.POINTER(_p), _p]),
+    "pips_corr_grad_feats_window": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i, _p, _p, _i, _p, _p]),
+    "pips_corr_grad_levels_window": (_i, [_i, _i, _i, _i, _i, _p, _p, _p, _i, C.POINTER(_p), _p]),
     "pips_peer_alloc": (_i, [C.c_size_t, C.POINTER(_p), C.c_char_p]),
     "pips_peer_open": (_i, [C.c_char_p, C.POINTER(_p)]),
     "pips_peer_close": (_i, [_p]),
@@ -116,6 +118,8 @@ _SIGNATURES = {
     "pips_scoremap_loss_window": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "pips_scoremap_grad_feats": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "pips_scoremap_grad_basis": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "pips_scoremap_grad_feats_window": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "pips_scoremap_grad_basis_window": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "pips_scoremap_basis_grad": (_i, [_p, _i, _i, _i, C.POINTER(_p), _p]),
     "pips_gemm_tc": (_i, [_p, _p, _i, _i, _p, _p, _i, _i, _i, _i, _i, _p, _i, _p, _i, _p, _p, _i, _p]),
     "pips_gemm_tc_aux": (_i, [_p, _p, _i, _i, _p, _p, _i, _i, _i, _i, _i, _p, _i, _p, _i, _p, _p, _i, _p, _i, _p]),

@@ -1,7 +1,7 @@
 // Backward of the local correlation (corr_gather.cu's columns 128:324) with respect to the ffeats and the 4 pyramid
 // levels; the coordinates are detached at the top of every iteration (nets/pips.py:500), so they get no gradient.
 //
-// Per unit u = (b, s, n) (mixer row (b*N + n)*8 + s) and level l, the forward blends the dot products of the unit's 8x8
+// Per unit u = (b, s, n) (mixer row (b*N + n)*S + s) and level l, the forward blends the dot products of the unit's 8x8
 // footprint (origin o = floor(c) - 3, c the clamped level-l position, fractional part (fx, fy)) into 49 taps:
 //   corr[l*49 + i*7 + j] = sum_{dy,dx in {0,1}} w_{dy,dx} <ffeat_u, level_l[frame, o_y + j + dy, o_x + i + dx]> / sqrt(128)
 // Its adjoint is one 8x8 matrix of weights per unit and level,
@@ -43,9 +43,9 @@ constexpr uint32_t CF_SMEM_BYTES = CF_WARPS * (CF_STAGES * CF_BOX_BYTES + CF_AUX
 
 struct CfArgs {
     CgArgs a;                 // B, N, H, W, coords (frame_base null)
-    const float* dcorr;       // (B*N*8, ld) fp32, columns [0, 196) used
+    const float* dcorr;       // (B*N*S, ld) fp32, columns [0, 196) used
     int ld;
-    float* dffeat;            // (B*N*8, 128)
+    float* dffeat;            // (B*N*S, 128)
 };
 
 // one CTA per SM (its shared memory fills the SM): the register budget is the whole file's, no spills
@@ -60,7 +60,7 @@ corr_grad_feats_kernel(const __grid_constant__ CgMaps maps, const CfArgs g) {
     const uint32_t bar0 = smem_u32(A + 64);
     const uint32_t stage0 = smem_u32(stage_buf);
 
-    const int total = a.B * 8 * a.N;
+    const int total = a.B * a.S * a.N;
     const int nwarps = static_cast<int>(gridDim.x) * CF_WARPS;
     int u = static_cast<int>(blockIdx.x) * CF_WARPS + warp;
     if (u >= total) return;                         // whole warp exits together
@@ -134,15 +134,15 @@ constexpr int CL_THREADS = 256;       // warp r owns tile row r, lane c channels
 constexpr int CL_BATCH = 32;          // overlapping units staged in shared memory per pass
 
 struct ClArgs {
-    int N;
+    int S, N;
     int H[PIPS_LEVELS], W[PIPS_LEVELS];
     int tiles_x[PIPS_LEVELS];
     int tile0[PIPS_LEVELS + 1];       // first tile of each level in a frame's tile list; tile0[4] = tiles per frame
     const float* coords;              // (B,S,N,2)
-    const float* ffeat;               // (B*N*8, 128)
-    const float* dcorr;               // (B*N*8, ld)
+    const float* ffeat;               // (B*N*S, 128)
+    const float* dcorr;               // (B*N*S, ld)
     int ld;
-    float* dlvl[PIPS_LEVELS];         // (B*8, H_l, W_l, 128)
+    float* dlvl[PIPS_LEVELS];         // (B*S, H_l, W_l, 128)
 };
 
 __global__ void __launch_bounds__(CL_THREADS)
@@ -153,7 +153,7 @@ corr_grad_levels_kernel(const __grid_constant__ ClArgs g) {
     __shared__ float4 sW[CL_THREADS];
     __shared__ int wcount[CL_THREADS / 32];
 
-    const int frame = blockIdx.y, b = frame >> 3, s = frame & 7;
+    const int S = g.S, frame = blockIdx.y, b = frame / S, s = frame - b * S;
     const int tile = blockIdx.x;
     const int level = (tile >= g.tile0[1]) + (tile >= g.tile0[2]) + (tile >= g.tile0[3]);
     const int t = tile - g.tile0[level];
@@ -163,6 +163,7 @@ corr_grad_levels_kernel(const __grid_constant__ ClArgs g) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float* coords = g.coords + static_cast<size_t>(frame) * N * 2;
     const float sc = 1.0f / static_cast<float>(1 << level);
+    const size_t unit0 = static_cast<size_t>(b) * N * S + s;       // unit (b, s, n) is mixer row unit0 + n*S
 
     float4 acc[8];
 #pragma unroll
@@ -209,14 +210,14 @@ corr_grad_levels_kernel(const __grid_constant__ ClArgs g) {
                 float v = 0.f;
                 if (j >= 0 && j < 8 && i >= 0 && i < 8) {
                     const float4 w4 = sW[k0 + k];
-                    const size_t u = (static_cast<size_t>(b) * N + sN[k0 + k]) * 8 + s;
+                    const size_t u = unit0 + static_cast<size_t>(sN[k0 + k]) * S;
                     v = adjoint_weight(g.dcorr + u * g.ld + level * 49, TapWeights{w4.x, w4.y, w4.z, w4.w}, j, i);
                 }
                 sA[k][py][px] = v;
             }
             for (int e = tid; e < nb * 32; e += CL_THREADS) {
                 const int k = e >> 5, c4 = e & 31;
-                const size_t u = (static_cast<size_t>(b) * N + sN[k0 + k]) * 8 + s;
+                const size_t u = unit0 + static_cast<size_t>(sN[k0 + k]) * S;
                 sF[k][c4] = *reinterpret_cast<const float4*>(g.ffeat + u * 128 + c4 * 4);
             }
             __syncthreads();
@@ -244,23 +245,81 @@ corr_grad_levels_kernel(const __grid_constant__ ClArgs g) {
     }
 }
 
-// the checks both entry points share; `who` prefixes every message
-static int check_problem(const char* who, int B, int S, int N, int H, int W, const float* coords, const float* dcorr,
-                         int ld_dcorr) {
+// `who`: `what`, as pips_last_error()
+static int fail_as(const char* who, const char* what) {
     char msg[160];
-    auto bad = [&](const char* what) {
-        snprintf(msg, sizeof msg, "%s: %s", who, what);
-        return fail(msg);
-    };
-    if (!coords || !dcorr) return bad("null pointer");
-    if (S != PIPS_S) return bad("S must be 8");
-    if (B <= 0 || N <= 0) return bad("empty problem");
-    if (H < 8 || W < 8) return bad("level-0 map must be at least 8x8");
-    if (ld_dcorr < 4 * 49) return bad("ld_dcorr must be >= 196");
-    if (static_cast<long long>(B) * S * N >= (1LL << 31)) return bad("more than 2^31 units in one call");
+    snprintf(msg, sizeof msg, "%s: %s", who, what);
+    return fail(msg);
+}
+
+// the checks all four entry points share; `who` prefixes every message.  The S == 8 entry points pass s_min = s_max = 8,
+// their _window siblings 2..PIPS_S_MAX: the kernels take S as a parameter
+static int check_problem(const char* who, int s_min, int s_max, int B, int S, int N, int H, int W, const float* coords,
+                         const float* dcorr, int ld_dcorr) {
+    if (!coords || !dcorr) return fail_as(who, "null pointer");
+    if (S < s_min || S > s_max) return fail_as(who, s_min == s_max ? "S must be 8" : "S must be in 2..16");
+    if (B <= 0 || N <= 0) return fail_as(who, "empty problem");
+    if (H < 8 || W < 8) return fail_as(who, "level-0 map must be at least 8x8");
+    if (ld_dcorr < 4 * 49) return fail_as(who, "ld_dcorr must be >= 196");
+    if (static_cast<long long>(B) * S * N >= (1LL << 31)) return fail_as(who, "more than 2^31 units in one call");
     if ((reinterpret_cast<uintptr_t>(coords) & 7) || (reinterpret_cast<uintptr_t>(dcorr) & 3))
-        return bad("coords must be 8-byte and dcorr 4-byte aligned");
+        return fail_as(who, "coords must be 8-byte and dcorr 4-byte aligned");
     return 0;
+}
+
+// pips_corr_grad_feats (S == 8) and pips_corr_grad_feats_window (2 <= S <= PIPS_S_MAX)
+static int corr_grad_feats_entry(const char* who, int s_min, int s_max, const float* const* lvl, int B, int S, int N, int H,
+                                 int W, const float* coords, const float* dcorr, int ld_dcorr, float* dffeat_rows,
+                                 void* stream) {
+    if (!lvl || !dffeat_rows) return fail_as(who, "null pointer");
+    if (check_problem(who, s_min, s_max, B, S, N, H, W, coords, dcorr, ld_dcorr)) return 1;
+    CfArgs g = {};
+    g.a.B = B; g.a.S = S; g.a.N = N; g.a.T = S;
+    for (int l = 0, h = H, w = W; l < PIPS_LEVELS; ++l, h /= 2, w /= 2) {
+        if (!lvl[l]) return fail_as(who, "null level pointer");
+        if (reinterpret_cast<uintptr_t>(lvl[l]) & 15) return fail_as(who, "the levels and dffeat_rows must be 16-byte aligned");
+        g.a.H[l] = h; g.a.W[l] = w;
+    }
+    if (reinterpret_cast<uintptr_t>(dffeat_rows) & 15) return fail_as(who, "the levels and dffeat_rows must be 16-byte aligned");
+    g.a.coords = coords;
+    g.dcorr = dcorr; g.ld = ld_dcorr; g.dffeat = dffeat_rows;
+    char what[96];
+    snprintf(what, sizeof what, "%s: cuTensorMapEncodeTiled failed", who);
+    CgMaps maps;
+    if (encode_level_maps(maps, reinterpret_cast<const void* const*>(lvl), CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.a.H, g.a.W, B * S,
+                          what))
+        return 1;
+    const long long units = static_cast<long long>(B) * S * N;
+    long long grid = (units + CF_WARPS - 1) / CF_WARPS;
+    const long long cap = static_cast<long long>(sm_count());      // 8 warps x (3 x 8 KB + 320 B) fill one SM
+    if (grid > cap) grid = cap;
+    snprintf(what, sizeof what, "%s: launch", who);
+    return launch_kernel<corr_grad_feats_kernel>(what, false, dim3(static_cast<unsigned>(grid)), dim3(CF_WARPS * 32),
+                                                 CF_SMEM_BYTES, static_cast<cudaStream_t>(stream), maps, g);
+}
+
+// pips_corr_grad_levels (S == 8) and pips_corr_grad_levels_window (2 <= S <= PIPS_S_MAX)
+static int corr_grad_levels_entry(const char* who, int s_min, int s_max, int B, int S, int N, int H, int W, const float* coords,
+                                  const float* ffeat_rows, const float* dcorr, int ld_dcorr, float* const* dlvl, void* stream) {
+    if (!ffeat_rows || !dlvl) return fail_as(who, "null pointer");
+    if (check_problem(who, s_min, s_max, B, S, N, H, W, coords, dcorr, ld_dcorr)) return 1;
+    if (reinterpret_cast<uintptr_t>(ffeat_rows) & 15) return fail_as(who, "ffeat_rows and the levels must be 16-byte aligned");
+    ClArgs g = {};
+    g.S = S; g.N = N;
+    g.tile0[0] = 0;
+    for (int l = 0, h = H, w = W; l < PIPS_LEVELS; ++l, h /= 2, w /= 2) {
+        if (!dlvl[l]) return fail_as(who, "null level pointer");
+        if (reinterpret_cast<uintptr_t>(dlvl[l]) & 15) return fail_as(who, "ffeat_rows and the levels must be 16-byte aligned");
+        g.H[l] = h; g.W[l] = w; g.dlvl[l] = dlvl[l];
+        g.tiles_x[l] = (w + 7) / 8;
+        g.tile0[l + 1] = g.tile0[l] + g.tiles_x[l] * ((h + 7) / 8);
+    }
+    g.coords = coords; g.ffeat = ffeat_rows; g.dcorr = dcorr; g.ld = ld_dcorr;
+    if (B * S > 65535) return fail_as(who, "more than 65535 frames in one call");
+    char what[96];
+    snprintf(what, sizeof what, "%s: launch", who);
+    return launch_kernel<corr_grad_levels_kernel>(what, false, dim3(g.tile0[PIPS_LEVELS], B * S), dim3(CL_THREADS), 0,
+                                                  static_cast<cudaStream_t>(stream), g);
 }
 
 }  // namespace pips
@@ -269,47 +328,24 @@ using namespace pips;
 
 extern "C" int pips_corr_grad_feats(const float* const* lvl, int B, int S, int N, int H, int W, const float* coords,
                                     const float* dcorr, int ld_dcorr, float* dffeat_rows, void* stream) {
-    if (!lvl || !dffeat_rows) return fail("pips_corr_grad_feats: null pointer");
-    if (check_problem("pips_corr_grad_feats", B, S, N, H, W, coords, dcorr, ld_dcorr)) return 1;
-    CfArgs g = {};
-    g.a.B = B; g.a.S = S; g.a.N = N; g.a.T = S;
-    for (int l = 0, h = H, w = W; l < PIPS_LEVELS; ++l, h /= 2, w /= 2) {
-        if (!lvl[l]) return fail("pips_corr_grad_feats: null level pointer");
-        if (reinterpret_cast<uintptr_t>(lvl[l]) & 15) return fail("pips_corr_grad_feats: the levels and dffeat_rows must be 16-byte aligned");
-        g.a.H[l] = h; g.a.W[l] = w;
-    }
-    if (reinterpret_cast<uintptr_t>(dffeat_rows) & 15) return fail("pips_corr_grad_feats: the levels and dffeat_rows must be 16-byte aligned");
-    g.a.coords = coords;
-    g.dcorr = dcorr; g.ld = ld_dcorr; g.dffeat = dffeat_rows;
-    CgMaps maps;
-    if (encode_level_maps(maps, reinterpret_cast<const void* const*>(lvl), CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.a.H, g.a.W, B * S,
-                          "pips_corr_grad_feats: cuTensorMapEncodeTiled failed"))
-        return 1;
-    const long long units = static_cast<long long>(B) * S * N;
-    long long grid = (units + CF_WARPS - 1) / CF_WARPS;
-    const long long cap = static_cast<long long>(sm_count());      // 8 warps x (3 x 8 KB + 320 B) fill one SM
-    if (grid > cap) grid = cap;
-    return launch_kernel<corr_grad_feats_kernel>("pips_corr_grad_feats: launch", false, dim3(static_cast<unsigned>(grid)),
-                                                 dim3(CF_WARPS * 32), CF_SMEM_BYTES, static_cast<cudaStream_t>(stream), maps, g);
+    return corr_grad_feats_entry("pips_corr_grad_feats", PIPS_S, PIPS_S, lvl, B, S, N, H, W, coords, dcorr, ld_dcorr,
+                                 dffeat_rows, stream);
+}
+
+extern "C" int pips_corr_grad_feats_window(const float* const* lvl, int B, int S, int N, int H, int W, const float* coords,
+                                           const float* dcorr, int ld_dcorr, float* dffeat_rows, void* stream) {
+    return corr_grad_feats_entry("pips_corr_grad_feats_window", 2, PIPS_S_MAX, lvl, B, S, N, H, W, coords, dcorr, ld_dcorr,
+                                 dffeat_rows, stream);
 }
 
 extern "C" int pips_corr_grad_levels(int B, int S, int N, int H, int W, const float* coords, const float* ffeat_rows,
                                      const float* dcorr, int ld_dcorr, float* const* dlvl, void* stream) {
-    if (!ffeat_rows || !dlvl) return fail("pips_corr_grad_levels: null pointer");
-    if (check_problem("pips_corr_grad_levels", B, S, N, H, W, coords, dcorr, ld_dcorr)) return 1;
-    if (reinterpret_cast<uintptr_t>(ffeat_rows) & 15) return fail("pips_corr_grad_levels: ffeat_rows and the levels must be 16-byte aligned");
-    ClArgs g = {};
-    g.N = N;
-    g.tile0[0] = 0;
-    for (int l = 0, h = H, w = W; l < PIPS_LEVELS; ++l, h /= 2, w /= 2) {
-        if (!dlvl[l]) return fail("pips_corr_grad_levels: null level pointer");
-        if (reinterpret_cast<uintptr_t>(dlvl[l]) & 15) return fail("pips_corr_grad_levels: ffeat_rows and the levels must be 16-byte aligned");
-        g.H[l] = h; g.W[l] = w; g.dlvl[l] = dlvl[l];
-        g.tiles_x[l] = (w + 7) / 8;
-        g.tile0[l + 1] = g.tile0[l] + g.tiles_x[l] * ((h + 7) / 8);
-    }
-    g.coords = coords; g.ffeat = ffeat_rows; g.dcorr = dcorr; g.ld = ld_dcorr;
-    if (B * S > 65535) return fail("pips_corr_grad_levels: more than 65535 frames in one call");
-    return launch_kernel<corr_grad_levels_kernel>("pips_corr_grad_levels: launch", false, dim3(g.tile0[PIPS_LEVELS], B * S),
-                                                  dim3(CL_THREADS), 0, static_cast<cudaStream_t>(stream), g);
+    return corr_grad_levels_entry("pips_corr_grad_levels", PIPS_S, PIPS_S, B, S, N, H, W, coords, ffeat_rows, dcorr,
+                                  ld_dcorr, dlvl, stream);
+}
+
+extern "C" int pips_corr_grad_levels_window(int B, int S, int N, int H, int W, const float* coords, const float* ffeat_rows,
+                                            const float* dcorr, int ld_dcorr, float* const* dlvl, void* stream) {
+    return corr_grad_levels_entry("pips_corr_grad_levels_window", 2, PIPS_S_MAX, B, S, N, H, W, coords, ffeat_rows, dcorr,
+                                  ld_dcorr, dlvl, stream);
 }

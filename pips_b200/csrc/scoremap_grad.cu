@@ -298,12 +298,16 @@ int launch_grad(const char* name, const void* y_hi, const void* y_lo, long long 
 
 using namespace pips;
 
-extern "C" int pips_scoremap_grad_feats(const void* G_hi, const void* G_lo, const float* ffeats, int iters, int B, int S,
-                                        int N, int H8, int W8, const int* target, const float* coef, float* dffeats,
-                                        void* stream) {
+// pips_scoremap_grad_feats (S == 8) and pips_scoremap_grad_feats_window (2 <= S <= PIPS_S_MAX): the kernel indexes frames
+// as b*S + s and never reads S itself
+static int scoremap_grad_feats_entry(int s_min, int s_max, const void* G_hi, const void* G_lo, const float* ffeats, int iters,
+                                     int B, int S, int N, int H8, int W8, const int* target, const float* coef, float* dffeats,
+                                     void* stream) {
     if (!G_hi || !G_lo || !ffeats || !target || !coef || !dffeats) return fail("pips_scoremap_grad_feats: null pointer");
     if (iters <= 0 || B <= 0 || S <= 0 || N <= 0 || H8 <= 0 || W8 <= 0) return fail("pips_scoremap_grad_feats: empty problem");
-    if (S != PIPS_S) return fail("pips_scoremap_grad_feats: S must be 8");
+    if (S < s_min || S > s_max)
+        return fail(s_min == s_max ? "pips_scoremap_grad_feats: S must be 8 (pips_scoremap_grad_feats_window takes 2..16)"
+                                   : "pips_scoremap_grad_feats_window: S must be in 2..16");
     if ((reinterpret_cast<uintptr_t>(G_hi) | reinterpret_cast<uintptr_t>(G_lo) | reinterpret_cast<uintptr_t>(ffeats)
          | reinterpret_cast<uintptr_t>(dffeats)) & 15)
         return fail("pips_scoremap_grad_feats: G_hi, G_lo, ffeats and dffeats must be 16-byte aligned");
@@ -317,12 +321,15 @@ extern "C" int pips_scoremap_grad_feats(const void* G_hi, const void* G_lo, cons
                               stream);
 }
 
-extern "C" int pips_scoremap_grad_basis(const void* G_hi, const void* G_lo, const void* F_hi, const void* F_lo, int iters,
-                                        int B, int S, int N, int H8, int W8, const int* target, const float* coef, float* dG,
-                                        void* stream) {
+// pips_scoremap_grad_basis (S == 8) and pips_scoremap_grad_basis_window (2 <= S <= PIPS_S_MAX)
+static int scoremap_grad_basis_entry(int s_min, int s_max, const void* G_hi, const void* G_lo, const void* F_hi,
+                                     const void* F_lo, int iters, int B, int S, int N, int H8, int W8, const int* target,
+                                     const float* coef, float* dG, void* stream) {
     if (!G_hi || !G_lo || !F_hi || !F_lo || !target || !coef || !dG) return fail("pips_scoremap_grad_basis: null pointer");
     if (iters <= 0 || B <= 0 || S <= 0 || N <= 0 || H8 <= 0 || W8 <= 0) return fail("pips_scoremap_grad_basis: empty problem");
-    if (S != PIPS_S) return fail("pips_scoremap_grad_basis: S must be 8");
+    if (S < s_min || S > s_max)
+        return fail(s_min == s_max ? "pips_scoremap_grad_basis: S must be 8 (pips_scoremap_grad_basis_window takes 2..16)"
+                                   : "pips_scoremap_grad_basis_window: S must be in 2..16");
     if ((reinterpret_cast<uintptr_t>(G_hi) | reinterpret_cast<uintptr_t>(G_lo) | reinterpret_cast<uintptr_t>(F_hi)
          | reinterpret_cast<uintptr_t>(F_lo) | reinterpret_cast<uintptr_t>(dG)) & 15)
         return fail("pips_scoremap_grad_basis: G_hi, G_lo, F_hi, F_lo and dG must be 16-byte aligned");
@@ -335,6 +342,32 @@ extern "C" int pips_scoremap_grad_basis(const void* G_hi, const void* G_lo, cons
     a.target = target; a.coef = coef; a.out = dG;
     a.frames = B * S; a.N = N; a.P = P; a.iters = iters;
     return launch_grad<true>("pips_scoremap_grad_basis", F_hi, F_lo, rows, dim3((P + BM - 1) / BM, B * S), a, stream);
+}
+
+extern "C" int pips_scoremap_grad_feats(const void* G_hi, const void* G_lo, const float* ffeats, int iters, int B, int S,
+                                        int N, int H8, int W8, const int* target, const float* coef, float* dffeats,
+                                        void* stream) {
+    return scoremap_grad_feats_entry(PIPS_S, PIPS_S, G_hi, G_lo, ffeats, iters, B, S, N, H8, W8, target, coef, dffeats, stream);
+}
+
+extern "C" int pips_scoremap_grad_feats_window(const void* G_hi, const void* G_lo, const float* ffeats, int iters, int B,
+                                               int S, int N, int H8, int W8, const int* target, const float* coef,
+                                               float* dffeats, void* stream) {
+    return scoremap_grad_feats_entry(2, PIPS_S_MAX, G_hi, G_lo, ffeats, iters, B, S, N, H8, W8, target, coef, dffeats,
+                                     stream);
+}
+
+extern "C" int pips_scoremap_grad_basis(const void* G_hi, const void* G_lo, const void* F_hi, const void* F_lo, int iters,
+                                        int B, int S, int N, int H8, int W8, const int* target, const float* coef, float* dG,
+                                        void* stream) {
+    return scoremap_grad_basis_entry(PIPS_S, PIPS_S, G_hi, G_lo, F_hi, F_lo, iters, B, S, N, H8, W8, target, coef, dG, stream);
+}
+
+extern "C" int pips_scoremap_grad_basis_window(const void* G_hi, const void* G_lo, const void* F_hi, const void* F_lo,
+                                               int iters, int B, int S, int N, int H8, int W8, const int* target,
+                                               const float* coef, float* dG, void* stream) {
+    return scoremap_grad_basis_entry(2, PIPS_S_MAX, G_hi, G_lo, F_hi, F_lo, iters, B, S, N, H8, W8, target, coef, dG,
+                                     stream);
 }
 
 extern "C" int pips_scoremap_basis_grad(const float* dG, int frames, int H8, int W8, float* const* dlvl_f32, void* stream) {

@@ -46,9 +46,9 @@ Extra, optional knobs (keyword-only; the reference signature is unchanged):
               taps by grid_sample, every volume kept until the backward (whose grid_sample adjoint accumulates with
               atomics).  'cuda' is torch_path.local_corr_cuda: pips_corr_gather's 8x8 footprints forward and
               deterministic gather kernels backward, with no volume; volumes are then built only for the dense score
-              maps (loss_path other than 'fused').  CPU tensors, S != 8 (the gradient kernels are written for 8-frame
-              windows) and maps under 8x8 keep the torch formulation;
-              plain inference is unaffected.  Independent of the other paths
+              maps (loss_path other than 'fused').  Any window of 2 to 16 frames: S != 8 runs the _window entry points
+              of the same gradient kernels.  CPU tensors and maps under 8x8 keep the torch formulation; plain inference
+              is unaffected.  Independent of the other paths
 Environment overrides: PIPS_B200_PRECISION, PIPS_B200_FEAT, PIPS_B200_FNET, PIPS_B200_LOSSES, PIPS_B200_MIXER,
 PIPS_B200_ENCODER, PIPS_B200_CORR.
 """

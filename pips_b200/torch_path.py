@@ -7,7 +7,7 @@ semantics, including the dense score map ``fcps`` that only the score-map loss c
 without ``fcps``, and with ``model.mixer_path == 'cuda'`` on CUDA tensors, where ``delta_block_cuda`` runs the
 DeltaBlock mixer forward and backward on the sm_90a kernels, with ``model.encoder_path == 'cuda'`` on CUDA tensors
 that need no gradient, where ``encoder_cuda`` does the same for the feature encoder, and with ``model.corr_path ==
-'cuda'`` on CUDA tensors (S = 8, feature maps of at least 8x8), where ``local_corr_cuda`` computes the local correlation
+'cuda'`` on CUDA tensors (feature maps of at least 8x8), where ``local_corr_cuda`` computes the local correlation
 and its gradients without the all-pairs volumes.
 
 Not used -- and not a fallback -- for plain inference: that path is CUDA-only (pips.py).
@@ -73,6 +73,12 @@ def score_map_targets(trajs_g, vis_g, valids, H8, W8):
     return torch.where(keep, y * W8 + x, torch.full_like(x, -1)).to(torch.int32).reshape(B, S, N).contiguous()
 
 
+def _window_entry(name, S):
+    """The C entry point for a window of S frames: ``name`` itself at S = 8, its ``_window`` sibling (2 <= S <= 16; the
+    same kernel, so the same bits at S = 8) otherwise."""
+    return name if S == 8 else name + "_window"
+
+
 class _FusedScoreMapLoss(torch.autograd.Function):
     """score_map_loss from the per-iteration ffeats and the pyramid, without the dense score maps, forward and backward
     on the CUDA kernels of csrc/scoremap_loss.cu and csrc/scoremap_grad.cu.  Saves G (hi, lo), the targets and the
@@ -96,10 +102,11 @@ class _FusedScoreMapLoss(torch.autograd.Function):
         n_split = lib.pips_scoremap_splits(H8, W8)
         neg = torch.empty(n_iters, B * S * N, n_split, device=dev)
         pos = torch.empty(n_iters, B * S * N, device=dev)
+        name = _window_entry("pips_scoremap_loss", S)
         for i, f in enumerate(ffeats):
             fi = f.detach().float().permute(0, 2, 1, 3).contiguous()        # ((b*N + n), s, c): free for the loop's state
-            L.check(lib.pips_scoremap_loss(L.ptr(g_hi), L.ptr(g_lo), L.ptr(fi), B, S, N, H8, W8, L.ptr(target),
-                                           L.ptr(neg[i]), L.ptr(pos[i]), st), "pips_scoremap_loss")
+            L.check(getattr(lib, name)(L.ptr(g_hi), L.ptr(g_lo), L.ptr(fi), B, S, N, H8, W8, L.ptr(target),
+                                       L.ptr(neg[i]), L.ptr(pos[i]), st), name)
         ctx.save_for_backward(g_hi, g_lo, target, *ffeats)
         ctx.n_iters, ctx.level_shapes = n_iters, [lv.shape for lv in levels]
         return _score_map_loss(neg, pos, target, n_iters, P)
@@ -124,8 +131,9 @@ class _FusedScoreMapLoss(torch.autograd.Function):
         dF = None
         if need_f:
             dF = torch.empty_like(F_)
-            L.check(lib.pips_scoremap_grad_feats(L.ptr(g_hi), L.ptr(g_lo), L.ptr(F_), I, B, S, N, H8, W8, L.ptr(target),
-                                                 L.ptr(coef), L.ptr(dF), st), "pips_scoremap_grad_feats")
+            name = _window_entry("pips_scoremap_grad_feats", S)
+            L.check(getattr(lib, name)(L.ptr(g_hi), L.ptr(g_lo), L.ptr(F_), I, B, S, N, H8, W8, L.ptr(target),
+                                       L.ptr(coef), L.ptr(dF), st), name)
         dls = [None] * len(ctx.level_shapes)
         if need_l:
             f_hi = torch.empty(F_.shape, dtype=torch.bfloat16, device=dev)
@@ -133,8 +141,9 @@ class _FusedScoreMapLoss(torch.autograd.Function):
             L.check(lib.pips_split_bf16(L.ptr(F_), L.ptr(f_hi), L.ptr(f_lo), F_.numel(), st), "pips_split_bf16")
             del F_
             dG = torch.empty(B * S, P, C, device=dev)
-            L.check(lib.pips_scoremap_grad_basis(L.ptr(g_hi), L.ptr(g_lo), L.ptr(f_hi), L.ptr(f_lo), I, B, S, N, H8, W8,
-                                                 L.ptr(target), L.ptr(coef), L.ptr(dG), st), "pips_scoremap_grad_basis")
+            name = _window_entry("pips_scoremap_grad_basis", S)
+            L.check(getattr(lib, name)(L.ptr(g_hi), L.ptr(g_lo), L.ptr(f_hi), L.ptr(f_lo), I, B, S, N, H8, W8,
+                                       L.ptr(target), L.ptr(coef), L.ptr(dG), st), name)
             del f_hi, f_lo
             dl = [torch.empty(B * S, sh[-2], sh[-1], C, device=dev) for sh in ctx.level_shapes]
             L.check(lib.pips_scoremap_basis_grad(L.ptr(dG), B * S, H8, W8, L.ptr_array(dl), st), "pips_scoremap_basis_grad")
@@ -690,8 +699,8 @@ def encoder_cuda(fnet, rgbs):
 class _LocalCorrFn(torch.autograd.Function):
     """The 196 correlation columns of pips_corr_gather, differentiable in the ffeats and the 4 levels.  The forward is
     pips_corr_gather into an fp32 row buffer, so it has the bits the inference path feeds its mixer; the backward is
-    pips_corr_grad_feats and pips_corr_grad_levels.  Saves the inputs only: no all-pairs volume exists in either
-    direction."""
+    pips_corr_grad_feats and pips_corr_grad_levels (their _window siblings at S != 8).  Saves the inputs only: no
+    all-pairs volume exists in either direction."""
 
     @staticmethod
     def forward(ctx, coords, ffeat_rows, *levels):
@@ -724,13 +733,15 @@ class _LocalCorrFn(torch.autograd.Function):
         dff = None
         if ctx.needs_input_grad[1]:
             dff = torch.empty(B * N, S, 128, device=dev)
-            L.check(lib.pips_corr_grad_feats(L.ptr_array(levels), B, S, N, H, W, L.ptr(coords), L.ptr(grad), ld, L.ptr(dff),
-                                             st), "pips_corr_grad_feats")
+            name = _window_entry("pips_corr_grad_feats", S)
+            L.check(getattr(lib, name)(L.ptr_array(levels), B, S, N, H, W, L.ptr(coords), L.ptr(grad), ld, L.ptr(dff), st),
+                    name)
         dls = [None] * len(levels)
         if any(ctx.needs_input_grad[2:]):
             dls = [torch.empty_like(lv) for lv in levels]
-            L.check(lib.pips_corr_grad_levels(B, S, N, H, W, L.ptr(coords), L.ptr(ffeat_rows), L.ptr(grad), ld,
-                                              L.ptr_array(dls), st), "pips_corr_grad_levels")
+            name = _window_entry("pips_corr_grad_levels", S)
+            L.check(getattr(lib, name)(B, S, N, H, W, L.ptr(coords), L.ptr(ffeat_rows), L.ptr(grad), ld, L.ptr_array(dls),
+                                       st), name)
         return (None, dff, *dls)
 
 
@@ -740,14 +751,17 @@ def local_corr_cuda(ffeat_rows, levels, coords):
     ``coords`` (detached at the top of every iteration, nets/pips.py:500).  ffeat_rows (B*N, S, 128) fp32; levels the 4
     channels-last (B*S, H>>l, W>>l, 128) fp32 pyramid levels; coords (B, S, N, 2) fp32 in feature-map pixels.  Returns
     fcorr (B*N, S, 196): channel l*49 + a*7 + b samples x = cx/2^l + a - 3, y = cy/2^l + b - 3, as forward_torch's.
-    Neither direction builds an all-pairs volume.  S = 8 and a level 0 of at least 8x8 only; allocates through torch's
-    caching allocator on the inputs' device and runs on its current stream, with no CUDA graph and no cache."""
+    Neither direction builds an all-pairs volume.  Windows of 2 <= S <= 16 frames (S = 8 runs the S = 8 entry points,
+    any other S their _window siblings: the same kernels) and a level 0 of at least 8x8 only; the window length is
+    checked before any tensor is touched.  Allocates through torch's caching allocator on the inputs' device and runs on
+    its current stream, with no CUDA graph and no cache."""
     levels = list(levels)
+    if not isinstance(coords, torch.Tensor) or coords.dim() != 4 or not 2 <= coords.shape[1] <= 16 or coords.shape[3] != 2:
+        shape = tuple(coords.shape) if isinstance(coords, torch.Tensor) else type(coords).__name__
+        raise ValueError(f"local_corr_cuda: coords must be (B, S, N, 2) with 2 <= S <= 16 frames; got {shape}")
     if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in [ffeat_rows, coords] + levels):
         raise RuntimeError("local_corr_cuda runs on the CUDA kernels only; use forward_torch's matmul + grid_sample "
                            "for CPU tensors")
-    if coords.dim() != 4 or coords.shape[1] != 8 or coords.shape[3] != 2:
-        raise ValueError(f"local_corr_cuda: coords must be (B, 8, N, 2) (S = 8 frames); got {tuple(coords.shape)}")
     B, S, N, _ = coords.shape
     if B == 0 or N == 0:
         raise ValueError("local_corr_cuda: no tracks")
@@ -829,7 +843,7 @@ def forward_torch(model, xys, rgbs, coords_init=None, feat_init=None, iters=3, t
     # corr_path='cuda': the correlation comes from local_corr_cuda over channels-last levels (built once; a no-op after
     # encoder_cuda, whose channels-last strides avg_pool2d keeps), so no all-pairs volume is kept for a backward; the
     # volumes are only built where the dense score maps need them
-    corr_cuda = (getattr(model, "corr_path", "torch") == "cuda" and rgbs.is_cuda and S == 8 and H8 >= 8 and W8 >= 8)
+    corr_cuda = (getattr(model, "corr_path", "torch") == "cuda" and rgbs.is_cuda and H8 >= 8 and W8 >= 8)
     if corr_cuda:
         levels_cl = [lv.permute(0, 1, 3, 4, 2).contiguous().flatten(0, 1) for lv in pyramid]
     preds, anim, fcps, ffeats_per_iter = [], [coords.detach() * stride] * 2, [], []
