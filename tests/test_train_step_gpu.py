@@ -52,14 +52,15 @@ def _reference_step(fnet, delta_block, norm, ffeat_updater, vis_predictor, rgbs,
 
     offs = torch.linspace(-r, r, 2 * r + 1, device=dev, dtype=dtype)
     window = torch.stack(torch.meshgrid(offs, offs, indexing="ij"), dim=-1).view(1, 2 * r + 1, 2 * r + 1, 2)
-    times = torch.linspace(0, S, S, device=dev).to(dtype).reshape(1, S, 1)      # the model's fp32 constants
+    # the model's fp32 constants (nets/pips.py:519, :397): in fp64, the exact sqrt(128) is 1.7e-8 off the model's
+    times = torch.linspace(0, S, S, device=dev).to(dtype).reshape(1, S, 1)
+    scale = torch.sqrt(torch.tensor(float(fmaps.shape[2]))).to(dtype)
     preds, fcps, used = [], [], []
     for i in range(iters):
         c = c.detach() if coords is None else coords[i].to(dtype)
         used.append(c)
         feats_ = ffeats.permute(0, 2, 1, 3).reshape(B * N, S, -1)
-        vols = [torch.matmul(ffeats, f.flatten(3)).reshape(B, S, N, *f.shape[-2:])
-                / torch.sqrt(torch.tensor(float(f.shape[2]), dtype=dtype)) for f in pyramid]
+        vols = [torch.matmul(ffeats, f.flatten(3)).reshape(B, S, N, *f.shape[-2:]) / scale for f in pyramid]
         fcps.append(sum(F.interpolate(v.flatten(0, 1), (H8, W8), mode="bilinear", align_corners=True).reshape(B, S, N, H8, W8)
                         for v in vols))
         taps = []
@@ -229,14 +230,22 @@ def test_composed_step_matches_fp64(monkeypatch, B, N, H, W, stride, iters, head
     (BF16X3_BOUND).  The free-running fp64 step's errors are printed, not bounded: a ReLU or a cell decided the other way
     moves a gradient by far more than rounding.  Worst ratio per case, measured on an H100 80GB HBM3 (700 W): see
     DESIGN.md section 7."""
+    model = _cuda_model(stride, head_scale)
+    inputs = _inputs(B, N, H, W, seed=H + N, dev=DEV)
+    check_pinned_step(monkeypatch, model, inputs, iters, f"B={B} N={N} {H}x{W}/{stride} iters={iters} head x{head_scale}")
+
+
+def check_pinned_step(monkeypatch, model, inputs, iters, label):
+    """test_composed_step_matches_fp64's check of one step of a CUDA-path model (the four nodes, or the three other
+    than delta_block_cuda where model.mixer_path == 'torch') on inputs (rgbs, xys, trajs_g, vis_g, valids); asserts
+    its bound and returns the step's (losses, {parameter name: gradient})"""
     monkeypatch.setattr(torch.backends.cudnn, "allow_tf32", False)
     monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
     monkeypatch.setattr(torch.backends.cuda.matmul, "allow_tf32", False)
-    model = _cuda_model(stride, head_scale)
-    inputs = _inputs(B, N, H, W, seed=H + N, dev=DEV)
     rgbs = inputs[0]
     lc, gc, coords, calls = _spied_step(monkeypatch, model, inputs, iters)
-    assert calls == {"encoder_cuda": 1, "local_corr_cuda": iters, "delta_block_cuda": iters, "fused_score_map_loss": 1}
+    mix = iters if model.mixer_path == "cuda" else 0
+    assert calls == {"encoder_cuda": 1, "local_corr_cuda": iters, "delta_block_cuda": mix, "fused_score_map_loss": 1}
     masks = _cuda_masks(model.fnet, rgbs)
     m64, m32 = _copies(model, torch.float64), _copies(model, torch.float32)
     l64, g64, _ = _reference_grads(m64, inputs, iters, masks=masks, coords=coords)
@@ -265,12 +274,13 @@ def test_composed_step_matches_fp64(monkeypatch, B, N, H, W, stride, iters, head
     ratio = {n: ec / max(2 * et, floor[n]) for n, (ec, et, _) in e.items()}
     worst = max(ratio, key=ratio.get)
     top = sorted(ratio, key=ratio.get, reverse=True)[:4]
-    print(f"\nB={B} N={N} {H}x{W}/{stride} iters={iters} head x{head_scale}: worst {worst} ratio {ratio[worst]:.3f}; "
+    print(f"\n{label}: worst {worst} ratio {ratio[worst]:.3f}; "
           f"cuda / fp32 / cuda vs free-running fp64: {e[worst][0]:.2e} / {e[worst][1]:.2e} / {e[worst][2]:.2e}; "
           f"{relu_diff} ReLU decisions and {cell_diff} sample cells differ from the free-running fp64 step; losses "
           + " ".join(f"{ratio[f'loss{i}']:.3f}" for i in range(3)) + "; next " + ", ".join(f"{n} {ratio[n]:.3f}" for n in top[1:])
           + f"; worst free-running fp64 {max(v[2] for v in e.values()):.2e}")
     assert ratio[worst] <= 1.0, f"{worst}: {ratio[worst]:.3f} of its bound"
+    return lc, gc
 
 
 # ------------------------------------------------------------------------------------------- three checks of the step
