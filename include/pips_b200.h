@@ -379,6 +379,44 @@ int pips_conv_tc_stats(const void* x_hi, const void* x_lo, int N, int H, int W, 
  * 2*(rgb/255)-1 at x = 2*ox + s - 3, zero outside the image / for k >= 21.  (ABI 3; ABI 2 unfolded the columns only.) */
 int pips_stem_pack(const void* rgb, int dtype, int N, int H, int W, void* out_hi, void* out_lo, void* stream);
 
+/* ---- the whole feature encoder in one call (csrc/encoder.cu; BasicEncoder.forward, nets/pips.py:247-281) ----
+ * Filters of one convolution: the bf16 (hi, lo) pack of the weight pack's fnet.<conv>.w_hi / .w_lo entries
+ * (pips_conv_tc's layout; the stem's is pips_stem_pack's 4x1 layout, (64, 4*64)) and its bias [Cout] fp32.  Only conv3's
+ * bias is read (it may be NULL: no bias): every other convolution feeds an InstanceNorm, which removes a per-channel
+ * constant again. */
+typedef struct pips_conv_weights {
+    const void *w_hi, *w_lo;
+    const float* b;
+} pips_conv_weights;
+
+/* one field per convolution, named as the pack's fnet.* entries with '.' -> '_', in module order */
+typedef struct pips_encoder_weights {
+    pips_conv_weights conv1;
+    pips_conv_weights layer1_0_conv1, layer1_0_conv2, layer1_1_conv1, layer1_1_conv2;
+    pips_conv_weights layer2_0_conv1, layer2_0_conv2, layer2_0_downsample_0, layer2_1_conv1, layer2_1_conv2;
+    pips_conv_weights layer3_0_conv1, layer3_0_conv2, layer3_0_downsample_0, layer3_1_conv1, layer3_1_conv2;
+    pips_conv_weights layer4_0_conv1, layer4_0_conv2, layer4_0_downsample_0, layer4_1_conv1, layer4_1_conv2;
+    pips_conv_weights conv2, conv3;
+} pips_encoder_weights;
+
+/* Scratch bytes of one pips_encode call: the stem operand, the convolution outputs, the partial statistics, the (hi, lo)
+ * pairs and the concatenation, each region 256-byte aligned.  A pure function of the shapes, covering every kernel
+ * choice of PIPS_B200_CONV_ROWS / PIPS_B200_CONV_STATS; 0 for shapes pips_encode refuses. */
+size_t pips_encode_workspace_bytes(int N, int H, int W, int stride);
+/* Kernels one pips_encode call of these shapes launches under the current PIPS_B200_CONV_ROWS / PIPS_B200_CONV_STATS
+ * (0 for refused shapes). */
+int pips_encode_launches(int N, int H, int W, int stride);
+/* rgb (N,3,H,W) with values 0..255, fp32 (dtype 0) or bf16 (dtype 1) -> fmaps_nhwc (N, H/stride, W/stride, 128) fp32,
+ * channels-last: the input of pips_pyramid_build_nhwc.  stride 4 or 8, H, W >= stride, 1 <= N <= 65535.  Enqueues
+ * the stem (pips_stem_pack + 4x1 wgmma convolution), the 8 ResBlocks, the 4 resizes into the concatenation and the
+ * head on `stream`: no allocation, no synchronisation, capturable into a CUDA graph.  workspace: at least
+ * pips_encode_workspace_bytes(N, H, W, stride) bytes, 256-byte aligned; fmaps_nhwc 16-byte aligned.
+ * keep: NULL, or 9 pointers (16-byte aligned) that receive the block boundaries, fp32 channels-last: [0] the stem's
+ * output (N, (H-1)/2+1, (W-1)/2+1, 64), [1 + 2l + j] the output of ResBlock j of layer l+1 (64, 96, 128, 128 channels,
+ * halved in size per layer from layer 2 on).  Arguments are checked before the first launch. */
+int pips_encode(const pips_encoder_weights* w, const void* rgb, int dtype, int N, int H, int W, int stride, void* workspace,
+                size_t workspace_bytes, float* fmaps_nhwc, float* const* keep, void* stream);
+
 /* ---- backward of the feature encoder (csrc/conv_grad.cu, csrc/encoder_grad.cu).  Every sum runs in a fixed order that
  * depends on the shape only: no atomics, the same bits on any GPU. ----
  * Weight gradient of a convolution on the tensor cores, bf16x3:

@@ -88,6 +88,22 @@ class Problem(C.Structure):
                 ("frame_base", _p), ("frames_per_batch", _i), ("peer", PeerOut)]
 
 
+# the convolutions of BasicEncoder in module order: the fields of pips_encoder_weights ('.' -> '_') and the fnet.* names
+# of the weight pack
+ENCODER_CONVS = ("conv1",) + tuple(
+    f"layer{i}.{j}.{c}" for i in range(1, 5) for j in range(2)
+    for c in (("conv1", "conv2", "downsample.0") if i > 1 and j == 0 else ("conv1", "conv2"))) + ("conv2", "conv3")
+
+
+class ConvWeights(C.Structure):
+    _fields_ = [("w_hi", _p), ("w_lo", _p), ("b", _p)]
+
+
+class EncoderWeights(C.Structure):
+    """pips_encoder_weights: one ConvWeights per convolution, named as ENCODER_CONVS with '.' -> '_'."""
+    _fields_ = [(n.replace(".", "_"), ConvWeights) for n in ENCODER_CONVS]
+
+
 _SIGNATURES = {
     "pips_abi_version": (_i, []),
     "pips_last_error": (C.c_char_p, []),
@@ -149,6 +165,9 @@ _SIGNATURES = {
     "pips_conv_tc": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p]),
     "pips_conv_tc_aniso": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p]),
     "pips_stem_pack": (_i, [_p, _i, _i, _i, _i, _p, _p, _p]),
+    "pips_encode_workspace_bytes": (C.c_size_t, [_i] * 4),
+    "pips_encode_launches": (_i, [_i] * 4),
+    "pips_encode": (_i, [C.POINTER(EncoderWeights), _p, _i, _i, _i, _i, _i, _p, C.c_size_t, _p, C.POINTER(_p), _p]),
     "pips_conv_tc_chunks": (_i, [_i] * 8),
     "pips_conv_tc_stats": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
     "pips_conv_rows_chunks": (_i, [_i, _i]),

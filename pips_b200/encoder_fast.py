@@ -11,6 +11,7 @@ Reference semantics: BasicEncoder.forward nets/pips.py:247-281, ResidualBlock.fo
 """
 from __future__ import annotations
 
+import ctypes as C
 import os
 
 import torch
@@ -327,52 +328,58 @@ def stem_tc(rgb: torch.Tensor, w):
     return unf, y, s_stem
 
 
+def encoder_weights(enc: Encoder, packs=None):
+    """-> (pips_encoder_weights of ``enc``, the tensors it points into).  ``packs``: {conv module: (hi, lo)} filter packs
+    to use instead of the modules' caches (which are then neither read nor written)."""
+    w = L.EncoderWeights()
+    hold = []
+    convs = dict(packed_convs(enc))
+    for name in L.ENCODER_CONVS:
+        conv = convs[name]
+        hi, lo = packed_filter(enc, name, conv) if packs is None else packs[conv]
+        b = None if conv.bias is None else conv.bias.detach().float().contiguous()
+        f = getattr(w, name.replace(".", "_"))
+        f.w_hi, f.w_lo, f.b = L.ptr(hi), L.ptr(lo), L.ptr(b)
+        hold += [hi, lo, b]
+    return w, hold
+
+
+def keep_shapes(N: int, H: int, W: int):
+    """Shapes of the 9 block boundaries pips_encode can keep: the stem output, then every ResBlock output (NHWC)."""
+    h, w = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    out = [(N, h, w, 64)]
+    for i, c in enumerate((64, 96, 128, 128)):
+        if i:
+            h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        out += [(N, h, w, c)] * 2
+    return out
+
+
 def _fnet_tc(enc: Encoder, rgb: torch.Tensor, packs=None, keep=None) -> torch.Tensor:
-    """``packs``: {conv module: (hi, lo)} filter packs to use instead of the modules' caches (torch_path.encoder_cuda);
+    """The whole encoder as one pips_encode call, its workspace from torch's caching allocator.
+    ``packs``: {conv module: (hi, lo)} filter packs to use instead of the modules' caches (torch_path.encoder_cuda);
     ``keep``: a list that receives the block boundaries -- the stem output and every ResBlock output, fp32."""
     lib = L.load()
-    LAUNCHES[0] = 0
     rgb = rgb.contiguous()
-    ops = _Ops(rgb.device)
     N, _, H, W = rgb.shape
-    H8, W8 = H // enc.stride, W // enc.stride
-    x = rgb
-
-    _, y, s_stem = stem_tc(rgb, _packed_stem_weight(enc.conv1) if packs is None else packs[enc.conv1])
-    X, XP = _apply_pair(ops, y, s_stem, relu_main=True, plain=True)
-    pk = (lambda conv: None) if packs is None else packs.__getitem__
+    dev = rgb.device
+    w, hold = encoder_weights(enc, packs)
+    nbytes = lib.pips_encode_workspace_bytes(N, H, W, enc.stride)
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    out = torch.empty(N, H // enc.stride, W // enc.stride, 128, dtype=torch.float32, device=dev)
+    kept = [torch.empty(s, dtype=torch.float32, device=dev) for s in keep_shapes(N, H, W)] if keep is not None else None
+    L.check(lib.pips_encode(C.byref(w), L.ptr(rgb), 0 if rgb.dtype == torch.float32 else 1, N, H, W, enc.stride, L.ptr(ws),
+                            nbytes, L.ptr(out), None if kept is None else L.ptr_array(kept), _st()), "pips_encode")
+    LAUNCHES[0] = lib.pips_encode_launches(N, H, W, enc.stride)
     if keep is not None:
-        keep.append(X)
-
-    ctot = 64 + 96 + 128 + 128
-    cat = _Pair(N, H8, W8, ctot, x.device)
-    c_off = 0
-    for i in range(1, 5):
-        for blk in getattr(enc, f"layer{i}"):
-            y1, s1 = _conv_stats(ops, XP, blk.conv1, pk(blk.conv1))
-            _, AP = _apply_pair(ops, y1, s1, relu_main=True)
-            y2, s2 = _conv_stats(ops, AP, blk.conv2, pk(blk.conv2))
-            if blk.downsample is not None:
-                d, sd = _conv_stats(ops, XP, blk.downsample[0], pk(blk.downsample[0]))
-                X, XP = _apply_pair(ops, y2, s2, r=d, stats_r=sd, relu_main=True, relu_out=True, plain=True)
-            else:
-                X, XP = _apply_pair(ops, y2, s2, r=X, relu_main=True, relu_out=True, plain=True)
-            if keep is not None:
-                keep.append(X)
-        Ns, Hs, Ws, Cs = X.shape
-        L.check(ops.lib.pips_resize_pair(L.ptr(X), Ns, Hs, Ws, Cs, L.ptr(cat.hi), L.ptr(cat.lo), H8, W8, cat.Cp, c_off, _st()),
-                "pips_resize_pair")
-        LAUNCHES[0] += 1
-        c_off += Cs
-
-    y, sy = _conv_stats(ops, cat, enc.conv2, pk(enc.conv2))
-    _, AP = _apply_pair(ops, y, sy, relu_main=True)
-    return conv_tc(AP, enc.conv3, bias=True, w=pk(enc.conv3))
+        keep.extend(kept)
+    return out
 
 
 # ---- the whole encoder as one CUDA graph per input shape ---------------------------------------------------
-# ~130 launches per call; for few frames (the demo clip, a rank's share of a frame-sharded batch, chained
-# windows) the kernels are microseconds long and the encoder is launch-bound when enqueued one by one.
+# pips_encode launches 66 kernels per call (pips_encode_launches); for few frames (the demo clip, a rank's share of a
+# frame-sharded batch, chained windows) the kernels are microseconds long and the encoder is launch-bound when enqueued
+# one by one.
 
 class _FnetGraph:
     def __init__(self, enc: Encoder, shape, dtype, dev):

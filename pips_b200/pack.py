@@ -47,7 +47,8 @@ def fingerprint(module: torch.nn.Module) -> str:
 
 def _collect(model) -> Dict[str, torch.Tensor]:
     """Every packed tensor of ``model`` (a pips_b200.Pips on a CUDA device), named.  Mixer / head tensors use
-    the field names of ``pips_weights``; encoder filters are "fnet.<conv path>.w_hi" / ".w_lo"."""
+    the field names of ``pips_weights``; encoder filters are "fnet.<conv path>.w_hi" / ".w_lo" and their biases
+    "fnet.<conv path>.b" (fp32), the fields of ``pips_encoder_weights``."""
     from . import encoder_fast as EF
 
     w = model.engine.weights(model)
@@ -55,6 +56,8 @@ def _collect(model) -> Dict[str, torch.Tensor]:
     for name, conv in EF.packed_convs(model.fnet):
         hi, lo = EF.packed_filter(model.fnet, name, conv)
         out[f"fnet.{name}.w_hi"], out[f"fnet.{name}.w_lo"] = hi, lo
+        if conv.bias is not None:
+            out[f"fnet.{name}.b"] = conv.bias.detach().float().contiguous()
     return out
 
 
